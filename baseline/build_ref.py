@@ -63,7 +63,6 @@ def main():
             rc = 1
     shutil.copy(os.path.join(shim, "mpirun"), os.path.join(out, "bin", "mpirun"))
     json.dump(log, open(os.path.join(out, "BUILD_LOG.json"), "w"), indent=1)
-    shutil.copy(os.path.join(out, "BUILD_LOG.json"), os.path.join(HERE, "BUILD_LOG.json"))
     return rc
 
 

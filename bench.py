@@ -3,7 +3,7 @@
 
 Metric (BASELINE.json): images/sec, whole job, device-timed, max over ranks, for the CIFAR-10
 ResNet D-PSGD training step -- the dcifar10/event configuration of the reference
-(/root/reference/dcifar10/event/event.cpp:29-42, :91, :196-200): ResNet{2,2,2,2} exactly as the
+(dcifar10/event/event.cpp:29-42, :91, :196-200): ResNet{2,2,2,2} exactly as the
 reference builds it (12 BasicBlocks, 86 tensors, 17 444 682 parameters), GLOBAL batch 256 split
 over the ranks (strong scaling), SGD lr 1e-2 momentum 0.9, ring gossip with both neighbours every
 step.  Default algorithm = dense D-PSGD (every tensor pushed every step -- the most communication
@@ -47,7 +47,7 @@ def parse():
                    help="compute dtype of forward/backward. fp32 (default) = IEEE fp32 with TF32 OFF, the reference's "
                         "precision (event.cpp:279); the exchange / optimizer kernels are fp32 in every mode")
     p.add_argument("--conv-tc", default="auto", choices=["auto", "on", "off"],
-                   help="fp32 only: 3x3 convolutions on the tcgen05 tensor cores at fp32 accuracy (csrc/conv_tc.cu; "
+                   help="fp32 only: 3x3 convolutions on the wgmma tensor cores at fp32 accuracy (csrc/conv_tc.cu; "
                         "auto = on) or cuDNN's SIMT fp32 kernels (off)")
     p.add_argument("--also", default="fp32_cudnn,bf16,tf32",
                    help="extra dtypes measured after the headline (device-timed only) and reported under "
@@ -57,9 +57,7 @@ def parse():
     p.add_argument("--topk", type=float, default=10.0)
     p.add_argument("--no-graph", action="store_true")
     p.add_argument("--overlap", default="auto", choices=["auto", "on", "off"],
-                   help="split step: pushes on a side stream overlapping forward/backward "
-                        "(auto = on for N >= 2: measured 2.65 vs 2.83 ms/step at N=2, 1.95 vs 2.22 at N=4, "
-                        "1.89 vs 2.09 at N=8)")
+                   help="split step: pushes on a side stream overlapping forward/backward (auto = on for N >= 2)")
     p.add_argument("--ce-push", action="store_true", help="copy-engine push in the split step (decent + overlap)")
     p.add_argument("--double-buffer", action=argparse.BooleanOptionalAction, default=None,
                    help="fused (non-split) decent step: two inbox slots, no WAR ack (default on where it applies)")
@@ -67,7 +65,37 @@ def parse():
     p.add_argument("--no-e2e", action="store_true")
     p.add_argument("--out", default="")
     p.add_argument("--profile", default="", help="write a torch.profiler kernel table of a few e2e steps here")
+    p.add_argument("--dump-outputs", default="", metavar="DIR",
+                   help="after the timed steps, write what the last timed step computed (loss, per-tensor parameter "
+                        "norms, a fixed seeded sample of the updated parameters) as DIR/<name>.npy")
     return p.parse_args()
+
+
+DUMP_SAMPLE = 1 << 20     # parameter elements kept by --dump-outputs (12 MB of files in all)
+
+
+def dump_outputs(tr, out_dir):
+    """The arrays a caller of the timed step receives: the loss it returns and the parameter arena it updates.  The
+    arena is sampled at fixed seeded positions so that the files stay small and two builds can be compared element
+    for element."""
+    import numpy as np
+    import torch
+    table, arena = tr.arena.table, tr.arena
+    torch.cuda.synchronize()
+    pos = torch.cat([torch.arange(o, o + n, dtype=torch.int64) for o, n in zip(table.offsets, table.numels)])
+    if pos.numel() > DUMP_SAMPLE:
+        pick = torch.randperm(pos.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_SAMPLE]
+        pos = pos[pick.sort().values]
+    idx = pos.to(arena.theta.device)
+    theta = arena.theta.detach()
+    norms = [theta[o:o + n].double().norm().item() for o, n in zip(table.offsets, table.numels)]
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": np.asarray([float(tr.last_loss)], dtype=np.float32),
+              "param_norms": np.asarray(norms, dtype=np.float64),
+              "params_sample": theta[idx].float().cpu().numpy(),
+              "sample_index": pos.double().numpy()}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def reference_arm(args):
@@ -78,7 +106,7 @@ def reference_arm(args):
     return ref_arm.run(args)
 
 
-def measure(args, env, dtype, want_e2e, src, sample_clocks):
+def measure(args, env, dtype, want_e2e, src, sample_clocks, dump_dir=""):
     """One Trainer at `dtype`: device-timed K steps (+ optionally the end-to-end loop).  Returns a dict.
     `fp32_cudnn` = fp32 with the tensor-core convolutions switched off (cuDNN's SIMT fp32 kernels, NCHW)."""
     conv_tc = {"auto": None, "on": True, "off": False}[args.conv_tc]
@@ -137,6 +165,8 @@ def measure(args, env, dtype, want_e2e, src, sample_clocks):
     barrier(env)
     ms = max_over_ranks(e0.elapsed_time(e1), env)
     tr.backend.check_status() if hasattr(tr.backend, "check_status") else None
+    if dump_dir and env.rank == 0:
+        dump_outputs(tr, dump_dir)
     res = {"dtype": dtype, "ms_per_step": ms / args.steps, "value": gb * args.steps / (ms / 1e3),
            "loss": float(tr.last_loss), "clocks": clocks, "gpu_launches": int(own_launches),
            "own_kernels_per_step": dict(tr.own_launches_per_step), "cfg": cfg, "gb": gb, "per_rank": per_rank,
@@ -240,7 +270,7 @@ def main():
     from eventgrad_b200.utils.dist import init_distributed, shutdown
 
     if not torch.cuda.is_available():
-        print(json.dumps({"impl": args.impl, "error": "bench.py needs a CUDA device (run it through gpurun / on the B200 box)"}))
+        print(json.dumps({"impl": args.impl, "error": "bench.py needs a CUDA device"}))
         return 2
     env = init_distributed("cuda")
     N = env.world
@@ -249,7 +279,7 @@ def main():
     gb = args.global_batch if args.scaling == "strong" else args.global_batch * N
     n_train = max(max(1, gb // N) * N * 8, 4096)
     src = synthetic_source("cifar10", n_train).pin()
-    r = measure(args, env, args.dtype, not args.no_e2e, src, True)
+    r = measure(args, env, args.dtype, not args.no_e2e, src, True, args.dump_outputs)
     others = {}
     for dt in [d for d in args.also.split(",") if d and d != args.dtype]:
         if dt == "fp32_cudnn" and (args.dtype != "fp32" or not r["cfg"].conv_tc):
@@ -269,9 +299,9 @@ def main():
                    "global_batch": r["gb"], "per_gpu_batch": r["per_rank"], "seq_len": None, "image": "3x32x32",
                    "parallelism": f"dp{N}-ring-gossip" if algo != "cent" else f"dp{N}-allreduce",
                    "algorithm": args.algo, "backend": r["backend"], "sync_mode": cfg.sync_mode,
-                   "precision": {"fp32": ("fp32 storage and fp32 accuracy, TF32 off; eligible 3x3 convolutions on the tcgen05 "
+                   "precision": {"fp32": ("fp32 storage and fp32 accuracy, TF32 off; eligible 3x3 convolutions on the wgmma "
                                           "tensor cores via 3 bf16 planes x 6 MMAs per product with fp32 round-to-nearest "
-                                          "accumulation (rms error vs fp64 1e-7, cuDNN's fp32 kernels: 2-4e-7, "
+                                          "accumulation (rms error vs fp64 checked against cuDNN's fp32 kernels in "
                                           "tests/test_gpu_conv_tc.py); the other convs on cuDNN fp32"
                                           if cfg.conv_tc else "IEEE fp32 forward/backward on cuDNN, TF32 off")
                                          + " (reference precision)",
@@ -285,7 +315,7 @@ def main():
                                if (args.overlap == "auto" and not args.no_graph and not args.no_channels_last
                                    and args.conv_tc == "auto" and not args.ce_push and args.double_buffer is None) else "overridden by flags",
                    "l2_policy": "per-step working set (theta,grad,mom,2 inboxes = "
-                                f"{5 * table.n_padded * 4 / 1e6:.0f} MB + activations) exceeds the 126 MB L2; "
+                                f"{5 * table.n_padded * 4 / 1e6:.0f} MB + activations) exceeds the 50 MB L2; "
                                 "no explicit flush"},
         "gpu_launches": r["gpu_launches"],
         "gpu_launches_how": "counted by the extension's launchers (csrc/api.h eg_count_launch) inside the timed "

@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Per-layer timing of the tcgen05 fp32-accuracy 3x3 convolution (csrc/conv_tc.cu) against cuDNN fp32 (TF32 off).
+"""Per-layer timing of the wgmma fp32-accuracy 3x3 convolution (csrc/conv_tc.cu) against cuDNN fp32 (TF32 off).
 
 For every distinct 3x3/stride-1 conv of the reference ResNet (dcifar10/common/resnet.hpp) at the headline batch:
 forward, data gradient and weight gradient -- the raw kernels on pre-split planes, the fp32->planes split passes,
 and cuDNN's fp32 NCHW (its best fp32 layout) for the same op.  CUDA events, rotating buffers larger than L2.
 
-    python benchmarks/conv_tc_bench.py --batch 256 --out profiles/conv_tc_bench.json
+    python benchmarks/conv_tc_bench.py --batch 256 --out conv_tc_bench.json
 """
 import argparse
 import json

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Two launches of each tcgen05 conv kernel instantiation at the headline shapes (batch 256): the ncu target.
+"""Two launches of each wgmma conv kernel instantiation at the headline shapes (batch 256): the ncu target.
     ncu --set full --import-source on --clock-control none -k regex:conv3x3 -o gpurun_out/conv_tc python benchmarks/conv_tc_ncu.py
 """
 import os

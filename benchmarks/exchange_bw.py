@@ -3,8 +3,8 @@
 
 For the ResNet arena (69.8 MB of parameters, 86 tensors) it reports per launch:
   * fused dense gossip step (push both neighbours + handshake + mix + SGD + norm-on-write):
-    time, NVLink egress GB/s per GPU (2 x model bytes / time) against the measured 770 GB/s
-    per-direction peer-copy ceiling, and HBM bytes/s of the mix+SGD stream;
+    time, NVLink egress GB/s per GPU (2 x model bytes / time) against the 450 GB/s per direction of
+    H100 NVLink 4 (data sheet), and HBM bytes/s of the mix+SGD stream;
   * fused event step at a chosen fire fraction (bytes scale with events);
   * fused all-reduce(+1/R+SGD) vs NCCL all_reduce + eager scale + eager SGD;
   * the NCCL-only gossip baseline (batch_isend_irecv + eager mix + eager SGD).
@@ -28,6 +28,7 @@ from eventgrad_b200.utils.dist import barrier, init_distributed, max_over_ranks,
 
 
 NVL = None          # NvlinkCounters of this rank's GPU (set in main)
+NVLINK_GBPS = 450.0  # H100 SXM, NVLink 4, one direction (data sheet)
 LAST_NVLINK = {}    # measured NVLink bytes per launch of the most recent timed() call (this rank)
 
 
@@ -36,7 +37,7 @@ def timed(fn, env, iters, warm=5):
         fn()
     torch.cuda.synchronize()
     # the NVML counter read takes tens of ms and differs per rank: do it BEFORE the barrier, or the ranks enter the
-    # timed region skewed and the first launch of the fast ranks spins on the slow one (seen as +2.4 ms/launch at R=8)
+    # timed region skewed and the first launch of the fast ranks spins on the slow one
     c0 = NVL.read() if (NVL is not None and NVL.ok) else None
     barrier(env)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -84,8 +85,7 @@ def main():
 
     # ---- dense fused gossip (decent) -----------------------------------------------------------
     # "ack_*": single inbox slot + WAR ack (round-1 protocol); "dbuf": two slots, no ack (the default since round 2)
-    for name, dbuf, kw in (("ack_v256", False, dict(vec256_push=True)), ("ack_v128", False, dict(vec256_push=False)),
-                           ("ack_d1", False, dict(group_iters=1)), ("ack_d4", False, dict(group_iters=4)),
+    for name, dbuf, kw in (("ack", False, dict()), ("ack_d1", False, dict(group_iters=1)), ("ack_d4", False, dict(group_iters=4)),
                            ("dbuf", None, dict()), ("dbuf_d4", None, dict(group_iters=4))):
         if not want(f"gossip_dense_{name}"):
             continue
@@ -97,7 +97,7 @@ def main():
         be.check_status()
         wire = (1 if be.wire_dedup else 2) * n_bytes          # 2-rank ring: theta crosses the link once
         res[f"gossip_dense_{name}"] = {"ms": ms, "egress_GBps_per_gpu": wire / ms / 1e6,
-                                      "frac_of_770": wire / ms / 1e6 / 770, "frac_of_900": wire / ms / 1e6 / 900,
+                                      "frac_of_nvlink": wire / ms / 1e6 / NVLINK_GBPS,
                                       "wire_bytes_per_gpu": wire,
                                       "hbm_GBps": 9 * arena.table.n_padded * 4 / ms / 1e6, "grid": be.grid, **LAST_NVLINK}
         be.close()
@@ -131,7 +131,7 @@ def main():
     n_bytes = arena.table.n_elems * 4
     ms = timed(be.step, env, a.iters)
     wire = (1 if be.wire_dedup else 2) * n_bytes
-    res["event_async_allfire"] = {"ms": ms, "egress_GBps_per_gpu": wire / ms / 1e6, "frac_of_770": wire / ms / 1e6 / 770,
+    res["event_async_allfire"] = {"ms": ms, "egress_GBps_per_gpu": wire / ms / 1e6, "frac_of_nvlink": wire / ms / 1e6 / NVLINK_GBPS,
                                   "wire_bytes_per_gpu": wire, **LAST_NVLINK}
     be.close(); del arena, be; torch.cuda.empty_cache()
     cfg = TrainConfig(algo="event", sync_mode="iter", thres_type=0, constant=1e30, initial_comm_passes=0,

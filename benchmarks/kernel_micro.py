@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Single-GPU micro-benchmark of the fused step kernel variants (self-loop ring: pushes land in
-this GPU's own HBM), device-timed.  Also the command profiled with ncu (profiles/)."""
+this GPU's own HBM), device-timed.  Also the command to profile with ncu."""
 import argparse
 import json
 import os

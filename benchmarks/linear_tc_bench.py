@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tcgen05 fused Linear+bias+ReLU vs cuBLAS (torch F.linear + relu) on the MNIST-MLP shapes."""
+"""wgmma fused Linear+bias+ReLU vs cuBLAS (torch F.linear + relu) on the MNIST-MLP shapes."""
 import json, os, sys
 import torch
 import torch.nn.functional as F
@@ -25,8 +25,8 @@ for M in (7500, 30000, 60000):
     us_tc = t(lambda: linear_tc_forward(x, w, b, True, torch.bfloat16))
     us_cublas = t(lambda: F.relu(F.linear(x, w, bb)))
     flops = 2.0 * M * K * N
-    res.append({"M": M, "K": K, "N": N, "tcgen05_fused_us": us_tc, "cublas_plus_relu_us": us_cublas,
-                "tcgen05_TFLOPs": flops / us_tc / 1e6, "cublas_TFLOPs": flops / us_cublas / 1e6,
+    res.append({"M": M, "K": K, "N": N, "wgmma_fused_us": us_tc, "cublas_plus_relu_us": us_cublas,
+                "wgmma_TFLOPs": flops / us_tc / 1e6, "cublas_TFLOPs": flops / us_cublas / 1e6,
                 "min_bytes_GBps_tc": (M * K * 2 + M * N * 2 + N * K * 2) / us_tc / 1e3})
     print(json.dumps(res[-1]))
 if len(sys.argv) > 1:

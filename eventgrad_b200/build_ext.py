@@ -1,8 +1,8 @@
-"""Build the sm_100a extension in-tree: eventgrad_b200/_C*.so.
+"""Build the sm_90a (H100) extension in-tree: eventgrad_b200/_C*.so.
 
-nvcc cross-compiles here without a GPU; the built .so travels with the repo snapshot to the
-B200 box (it is git-ignored, not gpurun-ignored).  No torch headers are involved, so a full
-rebuild takes a few seconds; objects are cached by source mtime under csrc/build/.
+nvcc cross-compiles without a GPU; the built .so is git-ignored and rebuilt from csrc/ on demand.
+No torch headers are involved, so a full rebuild takes a few seconds; objects are cached by source
+mtime under csrc/build/.
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(CSRC, "build")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
                            "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 CU_SOURCES = ["gossip.cu", "gossip_dbuf.cu", "ce_push.cu", "allreduce.cu", "allreduce_nvls.cu", "sparse.cu", "augment.cu", "ipc.cu", "bn_act.cu", "bn_nchw.cu", "linear_tc_tma.cu", "conv_tc.cu"]

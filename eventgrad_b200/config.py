@@ -45,14 +45,14 @@ class TrainConfig:
     initial_comm_passes: int = 30
     topk_percent: float = 10.0       # spevent only
     # ---- communication ---------------------------------------------------
-    backend: str = "auto"            # auto | p2p (fused sm_100a kernels) | nccl | gloo | refport (reference-structured)
+    backend: str = "auto"            # auto | p2p (fused sm_90a kernels) | nccl | gloo | refport (reference-structured)
     sync_mode: str = "iter"          # iter (deterministic handshake) | async (reference RMA semantics)
     final_divide_all: bool = True    # reference divides on rank 0 only (Q5)
     grad_table: bool = True          # p2p gossip: step kernel reads autograd's gradients in place (+ bf16
                                      # shadow weights under dtype=bf16) instead of an fp32 grad arena
     overlap_push: Optional[bool] = None   # p2p: launch the push half of the step on a side stream so it overlaps
                                      # forward/backward (False = single fused kernel).  None = auto: on for
-                                     # decent/event on >= 2 GPUs (measured faster at N=2/4/8, profiles/README.md)
+                                     # decent/event on >= 2 GPUs
     spevent_fresh_replicas: bool = False   # reference quirk Q8: prev/left/right replicas of spevent are three
                                      # MORE randomly initialised networks (spevent.cpp:123-136) instead of theta_0
     ce_push: bool = False            # decent + overlap_push: the push half of the split step is copy-engine memcpys
@@ -73,7 +73,7 @@ class TrainConfig:
     device: str = "auto"             # auto | cuda | cpu
     dtype: str = "fp32"              # fp32 | tf32 | bf16 (compute dtype; arena is fp32)
     channels_last: Optional[bool] = None   # None = auto on CUDA: NHWC, except fp32 with conv_tc off (cuDNN's fp32 convs are NCHW)
-    conv_tc: Optional[bool] = None         # fp32 only: 3x3 convs on the tcgen05 tensor cores at fp32 accuracy (csrc/conv_tc.cu);
+    conv_tc: Optional[bool] = None         # fp32 only: 3x3 convs on the wgmma tensor cores at fp32 accuracy (csrc/conv_tc.cu);
                                            # None = on for CUDA (EGB_CONV_TC=0 turns it off); False = cuDNN's SIMT fp32 kernels
     cuda_graph: Optional[bool] = None      # None = auto: whole-step CUDA graph on CUDA
     max_steps: int = 0               # >0: stop after this many steps (tests / bench)
@@ -120,8 +120,8 @@ class TrainConfig:
             conv_tc = kw["conv_tc"] = bool(cuda and self.dtype == "fp32" and os.environ.get("EGB_CONV_TC", "1") != "0")
         if self.channels_last is None:
             # bf16 / tf32 / fp32 on our tensor-core convolutions: NHWC.  fp32 on cuDNN (conv_tc off): its IEEE-fp32
-            # convolutions are NCHW kernels -- fed NHWC they transpose around every conv (measured 36.9 vs 27.8 ms/step
-            # on B200) -- so that path stays NCHW; the fused BN kernels exist for both layouts
+            # convolutions are NCHW kernels -- fed NHWC they transpose around every conv -- so that path stays NCHW;
+            # the fused BN kernels exist for both layouts
             kw["channels_last"] = cuda and (self.dtype != "fp32" or conv_tc)
         if self.cuda_graph is None:
             kw["cuda_graph"] = cuda
@@ -197,7 +197,7 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--channels-last", action=argparse.BooleanOptionalAction, default=None, help="default: on for CUDA")
     p.add_argument("--cuda-graph", action=argparse.BooleanOptionalAction, default=None, help="default: on for CUDA")
     p.add_argument("--conv-tc", action=argparse.BooleanOptionalAction, default=None,
-                   help="fp32: convolutions on the tcgen05 tensor cores at fp32 accuracy (default: on for CUDA); "
+                   help="fp32: convolutions on the wgmma tensor cores at fp32 accuracy (default: on for CUDA); "
                         "--no-conv-tc = cuDNN's SIMT fp32 kernels")
     p.add_argument("--no-cudnn-benchmark", dest="cudnn_benchmark", action="store_false", default=None)
     p.add_argument("--max-steps", type=int, default=None)

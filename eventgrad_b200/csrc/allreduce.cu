@@ -1,5 +1,5 @@
 // eventgrad_b200 -- one-shot / two-shot all-reduce over peer-mapped memory fused with the
-// 1/R scale and (cent) the SGD step (K4).  sm_100a.
+// 1/R scale and (cent) the SGD step (K4).  sm_90a.
 //
 // Replaces the per-tensor MPI_Allreduce(SUM) + grad/numranks + optimizer.step() of
 // /root/reference/dmnist/cent/cent.cpp:130-145 and the final parameter averaging of

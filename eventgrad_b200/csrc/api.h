@@ -1,4 +1,4 @@
-// eventgrad_b200 -- host-visible launch API of the sm_100a kernels.
+// eventgrad_b200 -- host-visible launch API of the sm_90a kernels.
 // Pure CUDA (no torch headers) so the .cu files compile in seconds; bindings.cpp adapts tensors.
 #pragma once
 #include <cuda_runtime.h>
@@ -97,7 +97,6 @@ struct GossipParams {
   int send_ack;             // sync: write acks in the tail (0 when another kernel acks)
   int zero_grad;
   int group_iters;          // iter-sync software-pipeline depth in tiles (push j, mix j-D)
-  int vec256_push;          // 1: 256-bit peer stores, 0: 2x128-bit
   const struct SparseParams* sparse;   // spevent: device copy of the sparse parameters -> the kernel's prologue scatters
                             // the arrived (value, index) records into inbox_l / inbox_r (the replicas) first
   int need_norm;            // 0: skip norm-on-write + trigger entirely (decent/cent without logs)
@@ -244,8 +243,8 @@ cudaError_t launch_bn_nchw(const BnParams& p, int hw, int which, int sm_count, c
 // which: 0 training forward, 1 apply only (eval), 2 backward
 cudaError_t launch_bn(const BnParams& p, int which, int sm_count, cudaStream_t s);
 
-// ------------------------------------------------------------------ tcgen05 fused Linear(+bias)(+ReLU)
-// Y[M,N] = act(X[M,K] * W[N,K]^T + b): bf16 operands, fp32 accumulation in TMEM (csrc/linear_tc_tma.cu).
+// ------------------------------------------------------------------ wgmma fused Linear(+bias)(+ReLU)
+// Y[M,N] = act(X[M,K] * W[N,K]^T + b): bf16 operands, fp32 accumulation in registers (csrc/linear_tc_tma.cu).
 struct LinearParams {
   const __nv_bfloat16* x;   // [M, K] row-major
   const __nv_bfloat16* w;   // [N, K] row-major (nn.Linear weight layout)
@@ -255,10 +254,10 @@ struct LinearParams {
   int relu;
   int out_bf16;
 };
-// TMA + SWIZZLE_128B + persistent CTAs (one per SM) + double-buffered TMEM accumulator
+// TMA + SWIZZLE_128B + persistent CTAs (one per SM) + two wgmma warpgroups
 cudaError_t launch_linear_tc_tma(const LinearParams& p, int sm_count, cudaStream_t s);
 
-// ------------------------------------------------------------------ tcgen05 convolutions at fp32 accuracy
+// ------------------------------------------------------------------ wgmma convolutions at fp32 accuracy
 // (csrc/conv_tc.cu): fp32 tensors split into three bf16 planes, six bf16 MMAs per fp32 product, fp32 accumulation.
 // One kernel pair + a tap table covers 3x3 stride 1/2, 1x1 stride 2 and the 3-channel stem (see conv_tc.cu).
 struct ConvTcParams {

@@ -1,4 +1,4 @@
-// eventgrad_b200 -- fused decode + augmentation of a uint8 image batch (sm_100a).
+// eventgrad_b200 -- fused decode + augmentation of a uint8 image batch (sm_90a).
 // ConstantPad(4) -> RandomHorizontalFlip -> RandomCrop(HxW) of the reference
 // (/root/reference/dcifar10/common/transform.hpp:68-101) collapse into one gather, fused with
 // the uint8->float conversion, normalisation, optional bf16 cast and NCHW->NHWC relayout:

@@ -51,7 +51,7 @@ static const std::unordered_map<std::string, Setter<GossipParams>> kGossip = {
     NUMF(GossipParams, timeout_ns), NUMF(GossipParams, lr), NUMF(GossipParams, mu),
     NUMF(GossipParams, do_mix), NUMF(GossipParams, do_push), NUMF(GossipParams, sync),
     NUMF(GossipParams, send_ack), NUMF(GossipParams, zero_grad), NUMF(GossipParams, group_iters),
-    NUMF(GossipParams, vec256_push), PTRF(GossipParams, sparse), NUMF(GossipParams, need_norm), NUMF(GossipParams, phase), TAB_FIELDS(GossipParams),
+    PTRF(GossipParams, sparse), NUMF(GossipParams, need_norm), NUMF(GossipParams, phase), TAB_FIELDS(GossipParams),
     PTRF2(GossipParams, fsm, thres), PTRF2(GossipParams, fsm, last_norm), PTRF2(GossipParams, fsm, last_iter),
     PTRF2(GossipParams, fsm, slopes), PTRF2(GossipParams, fsm, fire), PTRF2(GossipParams, fsm, cur_norm),
     PTRF2(GossipParams, fsm, counters), PTRF2(GossipParams, fsm, pass_num), PTRF2(GossipParams, fsm, log_ring),
@@ -138,9 +138,9 @@ void eg_count_launch(int family, int n) {
 }  // namespace egb
 
 PYBIND11_MODULE(_C, m) {
-  m.doc() = "eventgrad_b200 sm_100a kernels";
+  m.doc() = "eventgrad_b200 sm_90a kernels";
   m.attr("TILE") = EG_TILE;
-  m.attr("arch") = "sm_100a";
+  m.attr("arch") = "sm_90a";
   bind_params<GossipParams>(m, "GossipParams", kGossip);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
   bind_params<SparseParams>(m, "SparseParams", kSparse);

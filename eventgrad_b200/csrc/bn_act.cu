@@ -1,9 +1,9 @@
 // eventgrad_b200 -- fused BatchNorm2d (+ residual add) (+ ReLU), training forward + backward,
 // channels-last activations in fp32 (the reference's precision, event.cpp:279) or bf16 -- every kernel is a
-// template over the element type -- fp32 statistics/parameters.  sm_100a.
+// template over the element type -- fp32 statistics/parameters.  sm_90a.
 //
-// Why: a launch-level profile of the flagship step (CIFAR ResNet, bf16 autocast, see profiles/)
-// shows ATen's batch-norm + elementwise kernels taking ~2/3 of the GPU time while the tcgen05
+// Why: a launch-level profile of the flagship step (CIFAR ResNet, bf16 autocast)
+// shows ATen's batch-norm + elementwise kernels taking ~2/3 of the GPU time while the tensor-core
 // convolutions take under 1/3.  The block pattern of the reference's ResNet
 // (/root/reference/dcifar10/common/resnet.hpp:39-52: bn -> relu, bn -> += residual -> relu) is
 // memory-bound glue.

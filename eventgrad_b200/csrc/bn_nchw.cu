@@ -1,11 +1,11 @@
 // eventgrad_b200 -- fused BatchNorm2d (+ residual add) (+ ReLU) for fp32 NCHW activations, training forward +
-// backward.  sm_100a.
+// backward.  sm_90a.
 //
 // Why a second layout: the headline runs at the reference's precision (IEEE fp32, event.cpp:279), and cuDNN's
-// fp32 convolutions are NCHW kernels -- handed NHWC tensors they transpose around every conv (36.9 vs 27.8 ms per
-// step on B200).  So the fp32 path keeps activations NCHW and these kernels replace cuDNN's BN + ATen's add / ReLU
-// (measured in that 27.8 ms step: cudnn_batch_norm 1.4 ms + cudnn_batch_norm_backward 3.9 ms + ~2 ms of
-// elementwise kernels) with the same 2 + 2 launch structure as csrc/bn_act.cu (NHWC, bf16 / fp32):
+// fp32 convolutions are NCHW kernels -- handed NHWC tensors they transpose around every conv.  So the fp32 path
+// keeps activations NCHW and these kernels replace cuDNN's BN + ATen's add / ReLU (separate batch-norm forward,
+// batch-norm backward and elementwise kernels) with the same 2 + 2 launch structure as csrc/bn_act.cu (NHWC, bf16 /
+// fp32):
 //   forward : stats kernel (per-channel sum / sum-of-squares, last CTA of a channel finalises mean, invstd and
 //             the running statistics) -> apply kernel  y = relu(x * sc + sh (+ res))
 //   backward: reduce kernel (dbeta = sum dz, dgamma = sum dz * xhat with dz = dy * (y > 0))

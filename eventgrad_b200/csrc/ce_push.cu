@@ -1,7 +1,7 @@
-// eventgrad_b200 -- copy-engine push for the split step of dense gossip (decent).  sm_100a.
+// eventgrad_b200 -- copy-engine push for the split step of dense gossip (decent).  sm_90a.
 //
 // The split step (csrc/gossip.cu, phase 1 / phase 2) hides the neighbour pushes behind forward/backward,
-// but its phase-1 kernel occupies up to 128 CTAs for the ~0.2 ms the 2 x 70 MB take over NVLink -- SMs and
+// but its phase-1 kernel occupies up to 128 CTAs while the 2 x 70 MB cross NVLink -- SMs and
 // issue slots taken from the convolutions it overlaps with.  For `decent` every tile is pushed every step,
 // so the push is a plain contiguous copy: this path hands it to the DMA engines instead,
 //

@@ -1,11 +1,11 @@
-// eventgrad_b200 -- common device helpers (sm_100a).
+// eventgrad_b200 -- common device helpers (sm_90a).
 //
 // Conventions
 //   * EG_TILE fp32 elements per tile; every tile belongs to exactly one parameter tensor
 //     (parallel/arena.py pads tensors to whole tiles).  One CTA iteration = one tile:
-//     256 threads x 8 floats, moved with 256-bit LDG/STG (LDG.E.ENL2.256 on sm_100a).
+//     256 threads x 8 floats, moved as two 128-bit LDG/STG (Hopper's widest global access).
 //   * Peer memory is reached through CUDA-IPC mapped pointers: a plain st.global on such a
-//     pointer travels over NVLink 5 / NVSwitch into the neighbour's HBM.
+//     pointer travels over NVLink / NVSwitch into the neighbour's HBM.
 //   * Cross-GPU ordering: data stores (weak) -> bar.sync -> one thread: fence.acq_rel.sys +
 //     st.release.sys flag.  Consumer: ld.acquire.sys spin -> bar.sync -> ld.global.cg data
 //     (L1 is bypassed for anything a peer may have written).
@@ -24,13 +24,15 @@ struct alignas(32) F8 {
   float v[8];
 };
 
-// ---------------------------------------------------------------- 256-bit global access
+// ---------------------------------------------------------------- 8-float global access (2 x 128 bit)
 __device__ __forceinline__ F8 ld_f8(const float* p) {  // default caching (local, private data)
   F8 r;
-  asm volatile("ld.global.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]), "=f"(r.v[4]), "=f"(r.v[5]),
-                 "=f"(r.v[6]), "=f"(r.v[7])
+  asm volatile("ld.global.v4.f32 {%0,%1,%2,%3}, [%4];"
+               : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3])
                : "l"(p));
+  asm volatile("ld.global.v4.f32 {%0,%1,%2,%3}, [%4];"
+               : "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]), "=f"(r.v[7])
+               : "l"(p + 4));
   return r;
 }
 // L2-only load: for buffers a peer GPU may be writing (inboxes, peer gradients).
@@ -45,12 +47,6 @@ __device__ __forceinline__ F8 ld_f8_cg(const float* p) {
   return r;
 }
 __device__ __forceinline__ void st_f8(float* p, const F8& r) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(r.v[0]), "f"(r.v[1]),
-               "f"(r.v[2]), "f"(r.v[3]), "f"(r.v[4]), "f"(r.v[5]), "f"(r.v[6]), "f"(r.v[7])
-               : "memory");
-}
-// 2 x 128-bit variant (A/B against the 256-bit store on the NVLink path)
-__device__ __forceinline__ void st_f8_v4(float* p, const F8& r) {
   asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(r.v[0]), "f"(r.v[1]), "f"(r.v[2]),
                "f"(r.v[3])
                : "memory");

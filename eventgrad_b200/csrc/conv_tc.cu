@@ -1,15 +1,14 @@
 // eventgrad_b200 -- the convolutions of the ResNet family (3x3 stride 1/2, 1x1 stride 1/2, 3-channel stem: forward, data
-// gradient, weight gradient) on the 5th-generation tensor cores at fp32 accuracy (sm_100a).
+// gradient, weight gradient) on the Hopper tensor cores (wgmma) at fp32 accuracy (sm_90a).
 //
-// The reference trains in fp32 (/root/reference/dcifar10/event/event.cpp:259-276 feeds fp32 tensors to
-// torch::nn::Conv2d, resnet.hpp:3-9), and fp32 has no tensor-core path: cuDNN's fp32 kernels are SIMT (74 TFLOP/s
-// peak on a B200) and take ~22 of the 24 ms of the headline step.  These kernels keep fp32 STORAGE and fp32
-// ACCURACY but do the multiply-accumulate work with tcgen05.mma:
+// The reference trains in fp32 (dcifar10/event/event.cpp:259-276 feeds fp32 tensors to torch::nn::Conv2d,
+// resnet.hpp:3-9), and fp32 has no tensor-core path: cuDNN's fp32 kernels are SIMT (67 TFLOP/s peak on an H100 SXM).
+// These kernels keep fp32 STORAGE and fp32 ACCURACY but do the multiply-accumulate work with wgmma.mma_async:
 //
 //   every fp32 operand is split once into three bf16 planes  x = x0 + x1 + x2  (8+8+8 mantissa bits: exact up to
-//   2^-24 |x|), and the product is accumulated in fp32 in TMEM from the six significant cross terms
+//   2^-24 |x|), and the product is accumulated in fp32 from the six significant cross terms
 //       x0*w0 + x0*w1 + x1*w0 + x1*w1 + x0*w2 + x2*w0        (dropped: x1*w2, x2*w1, x2*w2 <= 2^-25 |x*w|)
-//   so one "fp32 MMA" costs six bf16 MMAs: 2.25 PFLOP/s / 6 = 375 TFLOP/s of fp32-equivalent peak, 5x the SIMT
+//   so one "fp32 MMA" costs six bf16 MMAs: 989 TFLOP/s / 6 = 165 TFLOP/s of fp32-equivalent peak, 2.5x the SIMT
 //   peak.  tests/test_gpu_conv_tc.py measures the error against an fp64 convolution next to cuDNN's fp32 error.
 //
 // Implicit GEMM, no im2col buffer: activations are NHWC planes [3][N][H][W][C]; the A tile of filter tap (r,s) is a
@@ -18,17 +17,15 @@
 //
 //   conv3x3_fprop_kernel   Y[pix, co] = sum_{tap,ci} X[pix+tap, ci] * Wt[co, tap, ci]        (forward; also the data
 //                          gradient: X := dY planes, Wt := flipped/transposed weights [ci][8-tap][co])
-//       persistent CTAs, tile 128 pixels x NT channels, K loop = 9 taps x Cin/64; warp 0 TMA producer, warp 1 MMA
-//       issuer (24 tcgen05.mma per stage into a FRESH TMEM accumulator), warps 2-5 drain every k-block's accumulator
-//       into fp32 registers (round-to-nearest adds: the tensor core itself truncates) and store the tile at the end.
+//       persistent CTAs, tile 128 pixels x NT channels, K loop = 9 taps x Cin/64; warpgroup 0 is the TMA producer,
+//       warpgroups 1 and 2 each own 64 rows of the tile: 24 wgmma per stage into five FRESH register accumulators,
+//       each added into the fp32 tile sum (round-to-nearest adds: the tensor core itself truncates).
 //   conv3x3_wgrad_kernel   dW[tap, ci, co] = sum_pix X[pix+tap, ci] * dY[pix, co]            (weight gradient)
 //       both operands are "MN-major" (the contiguous dimension is the channel, K = pixels), expressed with MN-major
 //       SWIZZLE_128B descriptors over the very same TMA boxes; split over pixel ranges, partial sums in a workspace
 //       (one split: dW is written directly).
 //   conv_wgrad_reduce_kernel   fixed-tree (bitwise reproducible) sum of the partials + transpose to the OHWI layout.
 //   conv_fprop_reduce_kernel   sum of the K-split partial tiles of the forward kernel on small grids (per-GPU batch 32).
-//   Measured (B200, batch 256, 19.3 GFLOP per launch): forward 93-137 us, wgrad 84-163 us = 140-230 TFLOP/s
-//   fp32-equivalent, 1e-7 rms against fp64 (cuDNN fp32: 2-4e-7); A/B history and ncu in profiles/README.md section 0a.
 //   split3_kernel          fp32 -> three bf16 planes (flat; "parity" variant: the four (h%2, w%2) sub-images of the
 //                          input of a STRIDE-2 conv, so that its taps become unit-stride boxes; "stem" variant: the 27
 //                          (tap, rgb) values of the 3-channel stem gathered into one 64-wide K block = a 1x1 conv)
@@ -48,17 +45,86 @@
 namespace egb {
 using namespace tc;
 
-#define CV_THREADS 192
-// TMEM accumulator ring: all 512 columns (8 accumulators at N tile 64, 4 at 128).  With two, the MMA of k-block i+2
-// has to wait for the drain of k-block i (barrier wake-up + tcgen05.ld + 64-128 adds + arrive); a deeper ring takes that
-// latency off the MMA's critical path.  (Measured neutral at batch 256 -- see the A/B list in profiles/README.md 0a.)
-#define CV_HV 1   // independent TMEM accumulators per k-block that the K steps alternate between; 2 measured neutral (A/B list)
-#define CV_NACC(NT) (512 / (CV_HV * (NT)))
+#define CV_THREADS 384     // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + epilogue, 64 rows of the tile each
+#define CV_CONSUMERS 256   // threads that arrive on an empty[] barrier (every MMA thread, after its wgmma wait)
 #define CV_APLANE 16384u   // one bf16 plane of an operand tile with 128 rows: 128 x 128 B
+#define CV_SMS 132         // grid cap of the element-wise launches (H100 SXM: 132 SMs)
+// N tile: 64 output channels.  Three register accumulators of NT/2 floats per thread (sum + two in flight) must fit
+// the 168 registers a thread of a 384-thread CTA can hold; NT = 128 would spill.
+#define CV_NT 64
+#define CV_STAGES 3        // 3 x 72 KB operand stages (A 3 x 16 KB + B 3 x 8 KB) of the 227 KB of shared memory
 
 // the six cross terms (plane of A, plane of B), largest last so that the small corrections are summed first
 #define CV_TERM_A(t) ((t) == 0 ? 2 : ((t) == 2 || (t) == 3) ? 1 : 0)
 #define CV_TERM_B(t) ((t) == 1 ? 2 : ((t) == 2 || (t) == 4) ? 1 : 0)
+
+template <int NT, int TA, int TB>
+__device__ __forceinline__ void mma_nt(float (&d)[NT / 2], uint64_t da, uint64_t db, uint32_t acc) {
+  static_assert(NT == 64, "N tile");
+  wgmma_m64n64<TA, TB>(d, da, db, acc);
+}
+
+// One k-block of the six-term product for this warpgroup's 64 rows.  The tensor core TRUNCATES every accumulation
+// to fp32, relative to the largest magnitude in it; a chain of MMAs onto a full-magnitude accumulator therefore drifts
+// towards zero (with one accumulator per 24-MMA k-block, results shrank by ~6e-8 relative on H100).  So: the five small correction terms (20 MMAs) go into one
+// fresh accumulator, and every 16-K MMA of the main term x0*w0 into a fresh accumulator of its own; each is added
+// into the fp32 sum `acc` with round-to-nearest.  Two accumulator sets (d, e) alternate so that one MMA group is
+// always queued on the tensor core while the previous one is being added.
+// k_step: byte offset of 16 K elements inside an operand plane.
+template <int NT, int TA, int TB>
+__device__ __forceinline__ void term_mma(float (&d)[NT / 2], uint32_t sa, uint32_t sb, uint32_t lbo, uint32_t scale_d) {
+  const uint64_t da = TA ? desc_mn_sw128(sa, lbo) : desc_k_sw128(sa);
+  const uint64_t db = TB ? desc_mn_sw128(sb, lbo) : desc_k_sw128(sb);
+  mma_nt<NT, TA, TB>(d, da, db, scale_d);
+}
+// acc += d, and half an ulp of d back with d's sign: the MMA's final rounding is towards zero (it loses half an ulp on
+// average, a bias that a deep network amplifies), the correction makes each partial unbiased.
+template <int R>
+__device__ __forceinline__ void add_group(float (&acc)[R], float (&d)[R]) {
+  wgmma_fence_regs(d);
+#pragma unroll
+  for (int j = 0; j < R; ++j) {
+    const float half_ulp = __int_as_float(__float_as_int(d[j]) & 0xff800000) * 5.9604645e-8f;   // sign * 2^(e-24)
+    acc[j] += d[j];
+    acc[j] += half_ulp;
+  }
+}
+template <int NT, int TA, int TB>
+__device__ __forceinline__ void six_term_kblock(float (&acc)[NT / 2], float (&d)[NT / 2], float (&e)[NT / 2],
+                                                uint32_t a0, uint32_t a_plane, uint32_t b0, uint32_t b_plane,
+                                                uint32_t lbo, uint32_t k_step) {
+  wgmma_fence();
+#pragma unroll
+  for (int t = 0; t < 5; ++t)
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4)
+      term_mma<NT, TA, TB>(d, a0 + CV_TERM_A(t) * a_plane + k4 * k_step, b0 + CV_TERM_B(t) * b_plane + k4 * k_step, lbo,
+                           (t > 0 || k4 > 0) ? 1u : 0u);
+  wgmma_commit();
+  // main term (plane 0 of both operands), one fresh accumulator per K step
+  wgmma_fence();
+  term_mma<NT, TA, TB>(e, a0, b0, lbo, 0u);
+  wgmma_commit();
+  wgmma_wait<1>();
+  add_group(acc, d);
+  wgmma_fence();
+  term_mma<NT, TA, TB>(d, a0 + k_step, b0 + k_step, lbo, 0u);
+  wgmma_commit();
+  wgmma_wait<1>();
+  add_group(acc, e);
+  wgmma_fence();
+  term_mma<NT, TA, TB>(e, a0 + 2 * k_step, b0 + 2 * k_step, lbo, 0u);
+  wgmma_commit();
+  wgmma_wait<1>();
+  add_group(acc, d);
+  wgmma_fence();
+  term_mma<NT, TA, TB>(d, a0 + 3 * k_step, b0 + 3 * k_step, lbo, 0u);
+  wgmma_commit();
+  wgmma_wait<1>();
+  add_group(acc, e);
+  wgmma_wait<0>();
+  add_group(acc, d);
+}
 
 // ------------------------------------------------------------------------------------------------ forward / dgrad
 template <int NT, int STAGES>
@@ -67,16 +133,12 @@ conv3x3_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                      const ConvTcParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   constexpr uint32_t A_BYTES = 3u * CV_APLANE, B_PLANE = (uint32_t)NT * 128u, STAGE = A_BYTES + 3u * B_PLANE;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const uint32_t smem_unaligned = s_u32(smem_raw);
   const uint32_t smem0 = (smem_unaligned + 1023u) & ~1023u;
   unsigned char* smem_al = smem_raw + (smem0 - smem_unaligned);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_al + STAGES * STAGE);
   const uint32_t full0 = s_u32(bars), empty0 = full0 + 8u * STAGES;
-  constexpr uint32_t NACC = CV_NACC(NT);
-  const uint32_t tfull0 = empty0 + 8u * STAGES, tempty0 = tfull0 + 8u * NACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 2 * NACC);
-  constexpr uint32_t NCOLS = NACC * CV_HV * NT;            // the whole TMEM: 512 columns
   const int cpb = p.Ca / 64, num_kb_all = p.ntaps * cpb;
   const int n_tiles = p.Cb / NT;
   const int ksplits = p.ksplits;                           // > 1: few tiles (small batch): split the K loop over CTAs,
@@ -88,26 +150,18 @@ conv3x3_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
   const int mt = tile_ / n_tiles, nt = tile_ - mt * n_tiles;                   \
   const int kb_lo = ks * kper, kb_hi = min(num_kb_all, kb_lo + kper);
 
-  if (warp == 2) tmem_alloc(s_u32(tmem_slot), NCOLS);
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
       bar_init(full0 + 8u * i, 1);
-      bar_init(empty0 + 8u * i, 1);
-    }
-    for (int i = 0; i < (int)NACC; ++i) {
-      bar_init(tfull0 + 8u * i, 1);
-      bar_init(tempty0 + 8u * i, 4);
+      bar_init(empty0 + 8u * i, CV_CONSUMERS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  tmem_fence_before();
   __syncthreads();
-  tmem_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
 
-  if (warp == 0) {
-    // ===================== TMA PRODUCER =====================
-    if (lane == 0) {
+  if (wg == 0) {
+    // ===================== TMA PRODUCER (one thread) =====================
+    if (tid == 0) {
       uint32_t it = 0;
       for (int work = blockIdx.x; work < total; work += gridDim.x) {
         CV_DECODE_WORK
@@ -129,94 +183,52 @@ conv3x3_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA ISSUER (whole warp walks the loop, one elected lane issues) =====================
-    {
-      const uint32_t idesc = idesc_bf16_f32(128, NT, 0, 0);
-      uint32_t it = 0;
-      for (int work = blockIdx.x; work < total; work += gridDim.x) {
-        CV_DECODE_WORK
-        (void)mt; (void)nt;
-        for (int kb = kb_lo; kb < kb_hi; ++kb, ++it) {
-          const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-          const uint32_t as = it % NACC, aph = (it / NACC) & 1u;
-          bar_wait(full0 + 8u * s, ph);                          // operands have landed
-          bar_wait(tempty0 + 8u * as, aph ^ 1u);                 // the accumulator of k-block it-NACC has been drained
-          tmem_fence_after();
-          const uint32_t tmem_d = tmem_base + as * (CV_HV * NT);
-          const uint32_t sa = smem0 + s * STAGE;
-          // The tensor core TRUNCATES every accumulation to fp32 (measured: a bias of ~0.5 ulp per MMA towards zero,
-          // growing linearly with K).  So each k-block starts a fresh accumulator that the epilogue warps add into
-          // fp32 registers with round-to-nearest, and inside the k-block the five small correction terms come first:
-          // only the last four MMAs (x0*w0) accumulate onto a full-magnitude value.
-          if (elect_one_sync()) {
-#pragma unroll
-            for (int t = 0; t < 6; ++t) {
-#pragma unroll
-              for (int k4 = 0; k4 < 4; ++k4) {
-                const uint64_t da = desc_k_sw128(sa + CV_TERM_A(t) * CV_APLANE) + (uint64_t)(k4 * 2);
-                const uint64_t db = desc_k_sw128(sa + A_BYTES + CV_TERM_B(t) * B_PLANE) + (uint64_t)(k4 * 2);
-                // consecutive MMAs alternate between CV_HV accumulators: no MMA waits for the accumulate of its predecessor
-                umma_bf16(tmem_d + (uint32_t)(k4 % CV_HV) * NT, da, db, idesc, (k4 >= CV_HV || t > 0) ? 1u : 0u);
-              }
-            }
-            umma_commit(empty0 + 8u * s);
-            umma_commit(tfull0 + 8u * as);
-          }
-          __syncwarp();
-        }
-      }
-    }
   } else {
-    // ===================== EPILOGUE (4 warps, one TMEM lane quadrant each) =====================
-    const int q = warp & 3;
-    uint32_t it = 0;
+    // ===================== MMA + EPILOGUE (rows 64g .. 64g+63 of every tile) =====================
+    const int g = wg - 1, warp = (tid >> 5) & 3, lane = tid & 31;
     const long long M = (long long)p.N * p.H * p.W;
+    float d[NT / 2], e[NT / 2];
+#pragma unroll
+    for (int j = 0; j < NT / 2; ++j) d[j] = e[j] = 0.f;
+    uint32_t it = 0;
     for (int work = blockIdx.x; work < total; work += gridDim.x) {
       CV_DECODE_WORK
-      float acc[NT];
+      float acc[NT / 2];
 #pragma unroll
-      for (int j = 0; j < NT; ++j) acc[j] = 0.f;
+      for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
       for (int kb = kb_lo; kb < kb_hi; ++kb, ++it) {
-        const uint32_t as = it % NACC, aph = (it / NACC) & 1u;
-        bar_wait(tfull0 + 8u * as, aph);
-        tmem_fence_after();
-#pragma unroll
-        for (int cb = 0; cb < NT; cb += 32) {
-#pragma unroll
-          for (int hv = 0; hv < CV_HV; ++hv) {
-            uint32_t v[32];
-            tmem_ld32(tmem_base + as * (CV_HV * NT) + (uint32_t)(hv * NT + cb) + ((uint32_t)(q * 32) << 16), v);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[cb + j] += __uint_as_float(v[j]);    // fp32 round-to-nearest
-          }
-        }
-        tmem_fence_before();
-        __syncwarp();
-        if (lane == 0) bar_arrive(tempty0 + 8u * as);
+        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
+        bar_wait(full0 + 8u * s, ph);                          // operands have landed
+        const uint32_t sa = smem0 + s * STAGE;
+        // K-major operands: +16 K elements = +32 bytes inside the 128-byte swizzled row
+        six_term_kblock<NT, 0, 0>(acc, d, e, sa + (uint32_t)g * 8192u, CV_APLANE, sa + A_BYTES, B_PLANE, 0u, 32u);
+        bar_arrive(empty0 + 8u * s);                           // this thread's MMAs no longer read the stage
       }
-      const long long row = (long long)mt * 128 + q * 32 + lane;
-      if (ksplits > 1) {                                       // partial tile, dense rows: ws[ks][m_tiles*128][Cb]
-        float4* dst = reinterpret_cast<float4*>(p.ws + (((size_t)ks * p.m_tiles * 128) + (size_t)row) * p.Cb + nt * NT);
 #pragma unroll
-        for (int j = 0; j < NT / 4; ++j) dst[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-      } else if (row < M) {
-        long long opix = row;
-        if (p.os != 1 || p.OH != p.H || p.OW != p.W) {          // strided scatter (data gradient of a stride-2 conv)
-          const int hw = p.H * p.W;
-          const int n = (int)(row / hw), rem = (int)(row - (long long)n * hw);
-          const int i = rem / p.W, j = rem - i * p.W;
-          opix = ((long long)n * p.OH + i * p.os + p.op) * p.OW + j * p.os + p.oq;
+      for (int h = 0; h < 2; ++h) {
+        const long long row = (long long)mt * 128 + g * 64 + warp * 16 + (lane >> 2) + h * 8;
+        float* dst;
+        if (ksplits > 1) {                                     // partial tile, dense rows: ws[ks][m_tiles*128][Cb]
+          dst = p.ws + (((size_t)ks * p.m_tiles * 128) + (size_t)row) * p.Cb + nt * NT;
+        } else if (row < M) {
+          long long opix = row;
+          if (p.os != 1 || p.OH != p.H || p.OW != p.W) {        // strided scatter (data gradient of a stride-2 conv)
+            const int hw = p.H * p.W;
+            const int n = (int)(row / hw), rem = (int)(row - (long long)n * hw);
+            const int i = rem / p.W, j = rem - i * p.W;
+            opix = ((long long)n * p.OH + i * p.os + p.op) * p.OW + j * p.os + p.oq;
+          }
+          dst = p.out + (size_t)opix * p.Cb + nt * NT;
+        } else {
+          continue;
         }
-        float4* dst = reinterpret_cast<float4*>(p.out + (size_t)opix * p.Cb + nt * NT);
+        dst += 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < NT / 4; ++j) dst[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+        for (int j = 0; j < NT / 8; ++j)
+          *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
       }
     }
   }
-  tmem_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, NCOLS);
 }
 
 // out[pixel(row)][c] = sum_ks ws[ks][row][c] (fixed order), with the same output mapping as the un-split epilogue
@@ -246,6 +258,7 @@ __global__ void __launch_bounds__(256) conv_fprop_reduce_kernel(const ConvTcPara
 // ------------------------------------------------------------------------------------------------ weight gradient
 // grid (ceil(U/2), Cb/NT, splits); U = ntaps * Ca/64 "units" (tap, 64-channel block of the input); one CTA accumulates
 // D[128 = two units][NT] over its range of 64-pixel K blocks and writes the partial to ws[split][unit*64 + ci][co].
+// MMA warpgroup g owns unit g of the pair (tile rows 64g .. 64g+63).
 template <int NT, int STAGES>
 __global__ void __launch_bounds__(CV_THREADS, 1)
 conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmG,
@@ -253,16 +266,12 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   constexpr uint32_t A_BYTES = 3u * CV_APLANE, B_PLANE = (uint32_t)NT * 128u, STAGE = A_BYTES + 3u * B_PLANE;
   constexpr uint32_t BLK = 8192u;                           // one [64 pixels][64 channels] block
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const uint32_t smem_unaligned = s_u32(smem_raw);
   const uint32_t smem0 = (smem_unaligned + 1023u) & ~1023u;
   unsigned char* smem_al = smem_raw + (smem0 - smem_unaligned);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_al + STAGES * STAGE);
   const uint32_t full0 = s_u32(bars), empty0 = full0 + 8u * STAGES;
-  constexpr uint32_t NACC = CV_NACC(NT);
-  const uint32_t tfull0 = empty0 + 8u * STAGES, tempty0 = tfull0 + 8u * NACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 2 * NACC);
-  constexpr uint32_t NCOLS = NACC * CV_HV * NT;
   const int cpb = p.Ca / 64, U = p.ntaps * cpb;
   const int u0 = 2 * blockIdx.x, u1 = (u0 + 1 < U) ? u0 + 1 : u0;
   const int per = (p.k_blocks + (int)gridDim.z - 1) / (int)gridDim.z;
@@ -270,25 +279,17 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   const int nkb = kb1 > kb0 ? kb1 - kb0 : 0;
   const int bpi = p.bn == 1 ? p.H / p.bh : 1;              // 64-pixel blocks per image
 
-  if (warp == 2) tmem_alloc(s_u32(tmem_slot), NCOLS);
   if (tid == 0) {
     for (int i = 0; i < STAGES; ++i) {
       bar_init(full0 + 8u * i, 1);
-      bar_init(empty0 + 8u * i, 1);
-    }
-    for (int i = 0; i < (int)NACC; ++i) {
-      bar_init(tfull0 + 8u * i, 1);
-      bar_init(tempty0 + 8u * i, 4);
+      bar_init(empty0 + 8u * i, CV_CONSUMERS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  tmem_fence_before();
   __syncthreads();
-  tmem_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (tid == 0) {
       int tap[2], cb64[2];
       tap[0] = u0 / cpb; cb64[0] = u0 - tap[0] * cpb;
       tap[1] = u1 / cpb; cb64[1] = u1 - tap[1] * cpb;
@@ -316,77 +317,43 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
                         n0, pl);
       }
     }
-  } else if (warp == 1) {
-    {                                                       // whole warp walks the loop, one elected lane issues
-      const uint32_t idesc = idesc_bf16_f32(128, NT, 1, 1);
-      for (int i = 0; i < nkb; ++i) {
-        const uint32_t s = (uint32_t)i % STAGES, ph = ((uint32_t)i / STAGES) & 1u;
-        const uint32_t as = (uint32_t)i % NACC, aph = ((uint32_t)i / NACC) & 1u;
-        bar_wait(full0 + 8u * s, ph);
-        bar_wait(tempty0 + 8u * as, aph ^ 1u);
-        tmem_fence_after();
-        const uint32_t sa = smem0 + s * STAGE;
-        // fresh accumulator per k-block, correction terms first (see conv3x3_fprop_kernel)
-        if (elect_one_sync()) {
-#pragma unroll
-          for (int t = 0; t < 6; ++t) {
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {                 // 16 pixels (two 8-row atoms = 2048 B) per MMA
-              const uint64_t da = desc_mn_sw128(sa + CV_TERM_A(t) * CV_APLANE + k4 * 2048u, BLK);
-              const uint64_t db = desc_mn_sw128(sa + A_BYTES + CV_TERM_B(t) * B_PLANE + k4 * 2048u, BLK);
-              umma_bf16(tmem_base + as * (CV_HV * NT) + (uint32_t)(k4 % CV_HV) * NT, da, db, idesc,
-                        (k4 >= CV_HV || t > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(empty0 + 8u * s);
-          umma_commit(tfull0 + 8u * as);
-        }
-        __syncwarp();
-      }
-    }
   } else {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int unit = m < 64 ? u0 : u1;
-    const bool store = (m < 64) || (u1 != u0);
-    float acc[NT];
+    const int g = wg - 1, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int unit = g == 0 ? u0 : u1;
+    const bool store = (g == 0) || (u1 != u0);
+    float acc[NT / 2], d[NT / 2], e[NT / 2];
 #pragma unroll
-    for (int j = 0; j < NT; ++j) acc[j] = 0.f;
+    for (int j = 0; j < NT / 2; ++j) acc[j] = d[j] = e[j] = 0.f;
     for (int i = 0; i < nkb; ++i) {
-      const uint32_t as = (uint32_t)i % NACC, aph = ((uint32_t)i / NACC) & 1u;
-      bar_wait(tfull0 + 8u * as, aph);
-      tmem_fence_after();
-#pragma unroll
-      for (int cb = 0; cb < NT; cb += 32) {
-#pragma unroll
-        for (int hv = 0; hv < CV_HV; ++hv) {
-          uint32_t v[32];
-          tmem_ld32(tmem_base + as * (CV_HV * NT) + (uint32_t)(hv * NT + cb) + ((uint32_t)(q * 32) << 16), v);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[cb + j] += __uint_as_float(v[j]);
-        }
-      }
-      tmem_fence_before();
-      __syncwarp();
-      if (lane == 0) bar_arrive(tempty0 + 8u * as);
+      const uint32_t s = (uint32_t)i % STAGES, ph = ((uint32_t)i / STAGES) & 1u;
+      bar_wait(full0 + 8u * s, ph);
+      const uint32_t sa = smem0 + s * STAGE;
+      // MN-major operands: 16 pixels = two 8-row atoms = +2048 bytes; the next 64 channels of B are one BLK further
+      six_term_kblock<NT, 1, 1>(acc, d, e, sa + (uint32_t)g * BLK, CV_APLANE, sa + A_BYTES, B_PLANE, BLK, 2048u);
+      bar_arrive(empty0 + 8u * s);
     }
     if (store) {
-      const size_t rows_all = (size_t)p.ntaps * p.Ca, my_row = (size_t)unit * 64 + (m & 63);
-      if (gridDim.z == 1) {
-        // one pixel split: this tile IS the result -- write dW[co][row] (OHWI) directly; lanes = consecutive rows
-        float* dw = p.dwout + (size_t)(blockIdx.y * NT) * rows_all + my_row;
+      const size_t rows_all = (size_t)p.ntaps * p.Ca;
 #pragma unroll
-        for (int j = 0; j < NT; ++j) dw[(size_t)j * rows_all] = acc[j];
-      } else {
-        float4* dst = reinterpret_cast<float4*>(p.out + ((size_t)blockIdx.z * rows_all + my_row) * p.Cb + blockIdx.y * NT);
+      for (int h = 0; h < 2; ++h) {
+        const size_t my_row = (size_t)unit * 64 + warp * 16 + (lane >> 2) + h * 8;
+        const int c0 = blockIdx.y * NT + 2 * (lane & 3);
+        if (gridDim.z == 1) {
+          // one pixel split: this tile IS the result -- write dW[co][row] (OHWI) directly
 #pragma unroll
-        for (int j = 0; j < NT / 4; ++j) dst[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+          for (int j = 0; j < NT / 8; ++j) {
+            p.dwout[(size_t)(c0 + 8 * j) * rows_all + my_row] = acc[4 * j + 2 * h];
+            p.dwout[(size_t)(c0 + 8 * j + 1) * rows_all + my_row] = acc[4 * j + 2 * h + 1];
+          }
+        } else {
+          float* dst = p.out + ((size_t)blockIdx.z * rows_all + my_row) * p.Cb + c0;
+#pragma unroll
+          for (int j = 0; j < NT / 8; ++j)
+            *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
       }
     }
   }
-  tmem_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, NCOLS);
 }
 
 // dw[co][row] = sum_z ws[z][row][co]   (row = tap*Ca + ci; fixed summation order => bitwise reproducible)
@@ -592,7 +559,7 @@ bool conv_tc_supported(int N, int H, int W, int Ca, int Cb) {
 int conv_wgrad_splits(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count) {
   int bh, bn, kblocks;
   if (!tile_geometry(N, H, W, 64, &bh, &bn, &kblocks)) return 0;
-  const int NT = (Cb % 128 == 0) ? 128 : 64;
+  const int NT = CV_NT;
   const int U = ntaps * (Ca / 64);
   const int work = ((U + 1) / 2) * (Cb / NT);
   int s = sm_count / work;
@@ -612,7 +579,7 @@ static bool taps_ok(const ConvTcParams& p) {
 int conv_fprop_ksplits(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count) {
   int bh, bn, m_tiles;
   if (!tile_geometry(N, H, W, 128, &bh, &bn, &m_tiles)) return 0;
-  const int NT = (Cb % 128 == 0) ? 128 : 64;
+  const int NT = CV_NT;
   const int tiles = m_tiles * (Cb / NT), num_kb = ntaps * (Ca / 64);
   if (tiles * 2 > sm_count || num_kb < 4) return 1;
   int ks = sm_count / tiles;
@@ -650,17 +617,17 @@ cudaError_t launch_conv_fprop(const ConvTcParams& p0, int sm_count, cudaStream_t
     if (p.ksplits != want) return cudaErrorInvalidValue;
   }
   CUtensorMap tmA, tmB;
-  const int NT = (p.Cb % 128 == 0) ? 128 : 64;
+  const int NT = CV_NT;
   if (!make_map_w(&tmB, p.b, (uint64_t)p.wtaps * p.Ca, (uint64_t)3 * p.Cb, (uint32_t)NT)) return cudaErrorNotSupported;
   const int total = p.m_tiles * (p.Cb / NT) * p.ksplits;
   const int grid = total < sm_count ? total : sm_count;
   if (!make_map_act(&tmA, p.a, p.Ca, p.W, p.H, p.N, 3 * p.nsrc, p.W, p.bh, p.bn)) return cudaErrorNotSupported;
   eg_count_launch(EG_FAM_CONV, p.ksplits > 1 ? 2 : 1);
-  cudaError_t e = NT == 128 ? fprop_launch<128, 2>(tmA, tmB, p, grid, s) : fprop_launch<64, 3>(tmA, tmB, p, grid, s);
+  cudaError_t e = fprop_launch<CV_NT, CV_STAGES>(tmA, tmB, p, grid, s);
   if (e != cudaSuccess || p.ksplits == 1) return e;
   const long long n4 = (long long)p.N * p.H * p.W * (p.Cb / 4);
   long long blocks = (n4 + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count * 8) blocks = sm_count * 8;
   conv_fprop_reduce_kernel<<<(unsigned)blocks, 256, 0, s>>>(p);
   return cudaGetLastError();
 }
@@ -683,14 +650,14 @@ cudaError_t launch_conv_wgrad(const ConvTcParams& p0, float* dw, int splits, cud
   tile_geometry(p.N, p.H, p.W, 64, &p.bh, &p.bn, &p.k_blocks);
   if (splits > p.k_blocks) splits = p.k_blocks;
   CUtensorMap tmX, tmG;
-  const int NT = (p.Cb % 128 == 0) ? 128 : 64;
+  const int NT = CV_NT;
   if (!make_map_act(&tmX, p.a, p.Ca, p.W, p.H, p.N, 3 * p.nsrc, p.W, p.bh, p.bn)) return cudaErrorNotSupported;
   if (!make_map_act(&tmG, p.b, p.Cb, p.W, p.H, p.N, 3, p.W, p.bh, p.bn)) return cudaErrorNotSupported;
   const int U = p.ntaps * (p.Ca / 64);
   const dim3 grid((U + 1) / 2, p.Cb / NT, splits);
   p.dwout = dw;
   eg_count_launch(EG_FAM_CONV, splits > 1 ? 2 : 1);
-  cudaError_t e = NT == 128 ? wgrad_launch<128, 2>(tmX, tmG, p, grid, s) : wgrad_launch<64, 3>(tmX, tmG, p, grid, s);
+  cudaError_t e = wgrad_launch<CV_NT, CV_STAGES>(tmX, tmG, p, grid, s);
   if (e != cudaSuccess || splits == 1) return e;
   const int rows = p.ntaps * p.Ca;
   conv_wgrad_reduce_kernel<<<dim3((rows + 31) / 32, p.Cb / 32), 256, 0, s>>>(p.out, dw, rows, p.Cb, splits);
@@ -699,7 +666,7 @@ cudaError_t launch_conv_wgrad(const ConvTcParams& p0, float* dw, int splits, cud
 
 static unsigned split_blocks(size_t n8) {
   size_t blocks = (n8 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CV_SMS * 16) blocks = CV_SMS * 16;
   if (blocks < 1) blocks = 1;
   return (unsigned)blocks;
 }

@@ -1,10 +1,10 @@
-// eventgrad_b200 -- fused event-triggered gossip step (K1/K2) for sm_100a.
+// eventgrad_b200 -- fused event-triggered gossip step (K1/K2) for sm_90a.
 //
 // What one launch does on every rank (persistent grid, one tile of EG_TILE floats per CTA
 // iteration):
 //   1. push   : tiles of tensors whose trigger fired are stored straight into the LEFT
 //               neighbour's "from-right" inbox and the RIGHT neighbour's "from-left" inbox
-//               (peer-mapped pointers -> NVLink 5 / NVSwitch).  Below threshold nothing is
+//               (peer-mapped pointers -> NVLink 4 / NVSwitch).  Below threshold nothing is
 //               stored, so link bytes scale with events (MPI_Put semantics,
 //               /root/reference/dcifar10/event/event.cpp:317-332).
 //   2. sync   : iter mode publishes one release-flag per (tile, warp) and waits for the two
@@ -176,13 +176,8 @@ __device__ __forceinline__ void cta_finish_tensors(const GossipParams& p, const 
 // -------------------------------------------------------------------------------------------
 __device__ __forceinline__ void push_tile(const GossipParams& p, size_t base, const F8& th) {
   // push_r == nullptr: 2-rank ring, the one neighbour is both left and right and reads the single copy twice
-  if (p.vec256_push) {
-    st_f8(p.push_l + base, th);
-    if (p.push_r != nullptr) st_f8(p.push_r + base, th);
-  } else {
-    st_f8_v4(p.push_l + base, th);
-    if (p.push_r != nullptr) st_f8_v4(p.push_r + base, th);
-  }
+  st_f8(p.push_l + base, th);
+  if (p.push_r != nullptr) st_f8(p.push_r + base, th);
 }
 #ifdef EG_DBUF
 __device__ __forceinline__ void push_tile_slot(const GossipParams& p, size_t base, const F8& th, int step) {

@@ -1,5 +1,5 @@
-// eventgrad_b200 -- EXPERIMENTAL double-buffered dense gossip step (decent), sm_100a.
+// eventgrad_b200 -- EXPERIMENTAL double-buffered dense gossip step (decent), sm_90a.
 // Same source as the default kernel, compiled with EG_DBUF: inbox slot = step & 1, no WAR ack
-// (see the header comment of gossip.cu and NEXT_STEPS.md item 2).  Opt-in: TrainConfig.double_buffer.
+// (see the header comment of gossip.cu).  TrainConfig.double_buffer selects it.
 #define EG_DBUF 1
 #include "gossip.cu"

@@ -1,4 +1,4 @@
-// eventgrad_b200 -- CUDA-IPC window runtime: the B200-native replacement of the reference's
+// eventgrad_b200 -- CUDA-IPC window runtime: the H100-native replacement of the reference's
 // MPI RMA window (MPI_Alloc_mem + MPI_Win_create, /root/reference/dmnist/event/event.cpp:170-179).
 // Each rank cudaMalloc's one slab, exports a 64-byte IPC handle (exchanged through the process
 // group by Python), and maps every peer's slab into its own address space.  Stores to a mapped

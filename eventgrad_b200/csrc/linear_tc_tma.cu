@@ -1,245 +1,135 @@
-// eventgrad_b200 -- tcgen05 fused Linear+bias(+ReLU): TMA + 128-byte swizzle, persistent CTAs,
-// double-buffered TMEM accumulator.  sm_100a.
+// eventgrad_b200 -- wgmma fused Linear+bias(+ReLU): TMA + 128-byte swizzle, persistent CTAs, warp-specialised
+// (sm_90a).
 //
-// Measured on B200 (benchmarks/linear_tc_bench.py, profiles/linear_tc_bench.json): 29.3 us vs 34.3 us for
-// cuBLAS bf16 + ReLU on 60000x784x128 (411 vs 351 TFLOP/s), 17.0 vs 16.6 us at M=30000, 17.1 vs 15.6 us at
-// M=7500.  It replaced the round-1 cp.async kernel (0.4-0.6x cuBLAS: one CTA per SM latency-bound on its 25
-// k-blocks, tensor pipe 7 %, 64-byte LDGSTS segments with 4-way bank conflicts), which was deleted.  Here a single
-// thread issues `cp.async.bulk.tensor.2d` (TMA) for 128-byte-wide boxes into a 128B-swizzled ring,
-// a single thread issues tcgen05.mma against SWIZZLE_128B descriptors, and four epilogue warps drain
-// one TMEM accumulator while the MMA warp fills the other:
+// A single thread issues `cp.async.bulk.tensor.2d` (TMA) for 128-byte-wide boxes into a 128B-swizzled ring; two MMA
+// warpgroups each own 64 rows of the 128-row tile, run wgmma.mma_async against SWIZZLE_128B descriptors with the
+// accumulator in registers, and apply bias + ReLU in the register epilogue:
 //
-//   warp 0  TMA producer      full[s]  <- expect_tx + 2 bulk tensor loads (A 128x64, B Nx64 bf16)
-//   warp 1  MMA issuer        wait full[s]; 4 x tcgen05.mma (K=16 each, +32 B inside the swizzle atom);
-//                             tcgen05.commit -> empty[s];  per tile: commit -> tmem_full[a]
-//   warp 2-5 epilogue         wait tmem_full[a]; tcgen05.ld; bias + ReLU; 16-byte stores; arrive tmem_empty[a]
+//   warpgroup 0    TMA producer   full[s]  <- expect_tx + 2 bulk tensor loads (A 128x64, B Nx64 bf16)
+//   warpgroup 1-2  MMA            wait full[s]; 4 K steps x NC wgmma (K=16 each, +32 B inside the swizzle atom);
+//                                 keep one k-block in flight, release the previous stage -> empty[s];
+//                                 per tile: bias + ReLU on the registers, stores
+//
+// N is covered by NC wgmma of width CH (N <= 64: one n64; N <= 128: one n128; N <= 256: two n128).  B rows past N are
+// never loaded; the columns they produce are computed from stale shared memory and discarded.
 #include <cuda.h>
 
 #include "api.h"
 #include "common.cuh"
+#include "tc_common.cuh"
 
 namespace egb {
+using namespace tc;
 
 #define TM_ROWS 128
 #define TM_BK 64
 #define TM_STAGES 4
-#define TM_THREADS 192
+#define TM_THREADS 384
+#define TM_CONSUMERS 256
 
-__device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void bar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void bar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void bar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void bar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap* tmap, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// K-major, SWIZZLE_128B canonical layout: rows of 128 bytes, 8-row (1024 B) swizzle atoms.
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);     // start address (16 B units)
-  d |= (uint64_t)1 << 16;                       // LBO field (ignored for swizzled K-major; canonical value 1)
-  d |= (uint64_t)(1024u >> 4) << 32;            // SBO: 8 rows x 128 B
-  d |= 1ull << 46;                              // version = 1 (Blackwell)
-  d |= 2ull << 61;                              // layout_type = SWIZZLE_128B
-  return d;
-}
-__device__ __forceinline__ uint32_t idesc_bf16(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TM_ROWS >> 4) << 24);
-}
-
-template <bool kOutBf16>
+template <int CH, int NC, bool kOutBf16>
 __global__ void __launch_bounds__(TM_THREADS, 1)
 linear_tma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const LinearParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  constexpr uint32_t A_BYTES = TM_ROWS * TM_BK * 2, B_BYTES = CH * NC * TM_BK * 2, STAGE = A_BYTES + B_BYTES;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int N = p.N;
-  const uint32_t a_bytes = TM_ROWS * TM_BK * 2, b_bytes = (uint32_t)N * TM_BK * 2;
-  const uint32_t stage_bytes = a_bytes + b_bytes;              // multiples of 1024 (N % 16 == 0 -> b_bytes % 2048 == 0)
-  // SWIZZLE_128B atoms (TMA destination and UMMA descriptors, base_offset = 0) need 1024-byte aligned tiles;
+  const uint32_t tx_bytes = A_BYTES + (uint32_t)N * TM_BK * 2;
+  // SWIZZLE_128B atoms (TMA destination and wgmma descriptors, base offset 0) need 1024-byte aligned tiles;
   // the dynamic-smem base is only guaranteed 16-byte aligned, so round up (the launcher adds 1 KB of slack)
   const uint32_t smem_unaligned = s_u32(smem_raw);
   const uint32_t smem0 = (smem_unaligned + 1023u) & ~1023u;
   unsigned char* smem_al = smem_raw + (smem0 - smem_unaligned);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_al + TM_STAGES * stage_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_al + TM_STAGES * STAGE);
   const uint32_t full0 = s_u32(bars), empty0 = full0 + 8u * TM_STAGES;
-  const uint32_t tfull0 = empty0 + 8u * TM_STAGES, tempty0 = tfull0 + 16u;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * TM_STAGES + 4);
-  const uint32_t acc_cols = (N <= 32) ? 32u : (N <= 64) ? 64u : (N <= 128) ? 128u : 256u;   // one accumulator
-  const uint32_t ncols = 2u * acc_cols;                                                       // two of them
   const int n_tiles = (p.M + TM_ROWS - 1) / TM_ROWS;
   const int num_kb = (p.K + TM_BK - 1) / TM_BK;
 
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "r"(ncols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   if (tid == 0) {
     for (int i = 0; i < TM_STAGES; ++i) {
-      bar_init(full0 + 8u * i, 1);      // producer's arrive.expect_tx (+ transaction bytes)
-      bar_init(empty0 + 8u * i, 1);     // tcgen05.commit
-    }
-    for (int i = 0; i < 2; ++i) {
-      bar_init(tfull0 + 8u * i, 1);     // tcgen05.commit after the tile's last MMA
-      bar_init(tempty0 + 8u * i, 4);    // one arrive per epilogue warp
+      bar_init(full0 + 8u * i, 1);                 // producer's arrive.expect_tx (+ transaction bytes)
+      bar_init(empty0 + 8u * i, TM_CONSUMERS);     // every MMA thread, once its wgmma reading the stage completed
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA PRODUCER (one thread) =====================
-    if (lane == 0) {
+    if (tid == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const uint32_t s = it % TM_STAGES, ph = (it / TM_STAGES) & 1u;
           bar_wait(empty0 + 8u * s, ph ^ 1u);                   // slot free (fresh barrier: passes at once)
-          bar_expect_tx(full0 + 8u * s, stage_bytes);
-          const uint32_t sa = smem0 + s * stage_bytes;
+          bar_expect_tx(full0 + 8u * s, tx_bytes);
+          const uint32_t sa = smem0 + s * STAGE;
           tma_load_2d(sa, &tmA, full0 + 8u * s, kb * TM_BK, tile * TM_ROWS);   // OOB rows / K tail are zero-filled
-          tma_load_2d(sa + a_bytes, &tmB, full0 + 8u * s, kb * TM_BK, 0);
+          tma_load_2d(sa + A_BYTES, &tmB, full0 + 8u * s, kb * TM_BK, 0);
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA ISSUER (one thread) =====================
-    if (lane == 0) {
-      const uint32_t idesc = idesc_bf16(N);
-      uint32_t it = 0, tl = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tl) {
-        const uint32_t as = tl & 1u, aph = (tl >> 1) & 1u;
-        bar_wait(tempty0 + 8u * as, aph ^ 1u);                  // epilogue has drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + as * acc_cols;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const uint32_t s = it % TM_STAGES, ph = (it / TM_STAGES) & 1u;
-          bar_wait(full0 + 8u * s, ph);                         // TMA bytes have landed
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t sa = smem0 + s * stage_bytes;
-          const uint64_t da0 = desc_sw128(sa), db0 = desc_sw128(sa + a_bytes);
-#pragma unroll
-          for (int k4 = 0; k4 < TM_BK / 16; ++k4) {
-            const uint64_t da = da0 + (uint64_t)(k4 * 2), db = db0 + (uint64_t)(k4 * 2);   // +32 B in the atom
-            const uint32_t accum = (kb > 0 || k4 > 0) ? 1u : 0u;
-            asm volatile(
-                "{\n\t.reg .pred p;\n\t"
-                "setp.ne.b32 p, %4, 0;\n\t"
-                "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-                : "memory");
-          }
-          umma_commit(empty0 + 8u * s);                          // slot reusable when these MMAs are done
-        }
-        umma_commit(tfull0 + 8u * as);                           // accumulator complete
       }
     }
   } else {
-    // ===================== EPILOGUE (4 warps, one TMEM lane quadrant each) =====================
-    const int q = warp & 3;                                      // warps 2,3,4,5 -> quadrants 2,3,0,1
-    uint32_t tl = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tl) {
-      const uint32_t as = tl & 1u, aph = (tl >> 1) & 1u;
-      bar_wait(tfull0 + 8u * as, aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int row = tile * TM_ROWS + q * 32 + lane;
-      for (int cb = 0; cb < N; cb += 32) {
-        uint32_t r[32];
-        const uint32_t taddr = tmem_base + as * acc_cols + (uint32_t)cb + ((uint32_t)(q * 32) << 16);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-              "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-              "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-              "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (row < p.M) {
+    // ===================== MMA + EPILOGUE (rows 64g .. 64g+63 of every tile) =====================
+    const int g = wg - 1, warp = (tid >> 5) & 3, lane = tid & 31;
+    float d[NC][CH / 2];
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      uint32_t prev = 0;
+      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        const uint32_t s = it % TM_STAGES, ph = (it / TM_STAGES) & 1u;
+        bar_wait(full0 + 8u * s, ph);                           // TMA bytes have landed
+        const uint32_t sa = smem0 + s * STAGE;
+        wgmma_fence();
 #pragma unroll
-          for (int g8 = 0; g8 < 4; ++g8) {
-            const int c0 = cb + g8 * 8;
-            if (c0 >= N) break;
-            float v[8];
+        for (int k4 = 0; k4 < TM_BK / 16; ++k4) {
+          const uint64_t da = desc_k_sw128(sa + (uint32_t)g * 8192u) + (uint64_t)(k4 * 2);   // +32 B in the atom
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              v[j] = __uint_as_float(r[g8 * 8 + j]) + (p.bias ? __ldg(p.bias + c0 + j) : 0.f);
-              if (p.relu) v[j] = fmaxf(v[j], 0.f);
-            }
-            if (kOutBf16) {
-              uint4 u;
-              __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
+          for (int c = 0; c < NC; ++c) {
+            const uint64_t db = desc_k_sw128(sa + A_BYTES + (uint32_t)c * CH * 128u) + (uint64_t)(k4 * 2);
+            const uint32_t accum = (kb > 0 || k4 > 0) ? 1u : 0u;
+            if constexpr (CH == 128) wgmma_m64n128<0, 0>(d[c], da, db, accum);
+            else wgmma_m64n64<0, 0>(d[c], da, db, accum);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                        // the k-block before this one has completed
+        if (kb > 0) bar_arrive(empty0 + 8u * prev);
+        prev = s;
+      }
+      wgmma_wait<0>();
 #pragma unroll
-              for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-              *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.y) + (size_t)row * N + c0) = u;
-            } else {
-              float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.y) + (size_t)row * N + c0);
-              dst[0] = make_float4(v[0], v[1], v[2], v[3]);
-              dst[1] = make_float4(v[4], v[5], v[6], v[7]);
-            }
+      for (int c = 0; c < NC; ++c) wgmma_fence_regs(d[c]);
+      bar_arrive(empty0 + 8u * prev);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = tile * TM_ROWS + g * 64 + warp * 16 + (lane >> 2) + h * 8;
+        if (row >= p.M) continue;
+#pragma unroll
+        for (int c = 0; c < NC; ++c) {
+#pragma unroll
+          for (int j = 0; j < CH / 8; ++j) {
+            const int col = c * CH + 8 * j + 2 * (lane & 3);
+            if (col >= N) continue;
+            float v0 = d[c][4 * j + 2 * h], v1 = d[c][4 * j + 2 * h + 1];
+            if (p.bias) { v0 += __ldg(p.bias + col); v1 += __ldg(p.bias + col + 1); }
+            if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (kOutBf16)
+              *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<__nv_bfloat16*>(p.y) + (size_t)row * N + col) =
+                  __floats2bfloat162_rn(v0, v1);
+            else
+              *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.y) + (size_t)row * N + col) = make_float2(v0, v1);
           }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) bar_arrive(tempty0 + 8u * as);              // this warp is done with the accumulator
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols));
   }
 }
 
 // ---------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
 static bool make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t K, uint32_t box_rows) {
-  EncodeTiledFn enc = get_encode();
+  EgEncodeTiledFn enc = eg_get_encode_tiled();
   if (enc == nullptr) return false;
   const cuuint64_t dims[2] = {K, rows};                    // innermost first
   const cuuint64_t strides[1] = {K * 2};                   // bytes, dims 1..rank-1
@@ -250,26 +140,34 @@ static bool make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t K
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+template <int CH, int NC>
+static cudaError_t linear_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const LinearParams& p, int grid,
+                                 cudaStream_t s) {
+  const size_t smem = (size_t)TM_STAGES * ((size_t)TM_ROWS * TM_BK * 2 + (size_t)CH * NC * TM_BK * 2) + 256 + 1024;
+  cudaError_t e;
+  if (p.out_bf16) {
+    e = cudaFuncSetAttribute(linear_tma_kernel<CH, NC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    linear_tma_kernel<CH, NC, true><<<grid, TM_THREADS, smem, s>>>(tmA, tmB, p);
+  } else {
+    e = cudaFuncSetAttribute(linear_tma_kernel<CH, NC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    linear_tma_kernel<CH, NC, false><<<grid, TM_THREADS, smem, s>>>(tmA, tmB, p);
+  }
+  return cudaGetLastError();
+}
+
 cudaError_t launch_linear_tc_tma(const LinearParams& p, int sm_count, cudaStream_t s) {
   if (p.N % 16 != 0 || p.N < 16 || p.N > 256 || p.K % 8 != 0 || p.M < 1) return cudaErrorInvalidValue;
   CUtensorMap tmA, tmB;
   if (!make_map(&tmA, p.x, (uint64_t)p.M, (uint64_t)p.K, TM_ROWS)) return cudaErrorNotSupported;
   if (!make_map(&tmB, p.w, (uint64_t)p.N, (uint64_t)p.K, (uint32_t)p.N)) return cudaErrorNotSupported;
-  const size_t smem = (size_t)TM_STAGES * ((size_t)TM_ROWS * TM_BK * 2 + (size_t)p.N * TM_BK * 2) + 256 + 1024;
   const int n_tiles = (p.M + TM_ROWS - 1) / TM_ROWS;
   const int grid = n_tiles < sm_count ? n_tiles : sm_count;
-  cudaError_t e;
   eg_count_launch(EG_FAM_LINEAR, 1);
-  if (p.out_bf16) {
-    e = cudaFuncSetAttribute(linear_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    linear_tma_kernel<true><<<grid, TM_THREADS, smem, s>>>(tmA, tmB, p);
-  } else {
-    e = cudaFuncSetAttribute(linear_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    linear_tma_kernel<false><<<grid, TM_THREADS, smem, s>>>(tmA, tmB, p);
-  }
-  return cudaGetLastError();
+  if (p.N <= 64) return linear_launch<64, 1>(tmA, tmB, p, grid, s);
+  if (p.N <= 128) return linear_launch<128, 1>(tmA, tmB, p, grid, s);
+  return linear_launch<128, 2>(tmA, tmB, p, grid, s);
 }
 
 }  // namespace egb

@@ -1,4 +1,4 @@
-// eventgrad_b200 -- sparse (top-k) event exchange (K3) for sm_100a.
+// eventgrad_b200 -- sparse (top-k) event exchange (K3) for sm_90a.
 //
 // spevent semantics (/root/reference/dcifar10/spevent/spevent.cpp:342-448): when tensor i
 // fires, the k_i elements with the largest |theta - prev| travel as (value, index) pairs; the

@@ -1,11 +1,11 @@
-// eventgrad_b200 -- tcgen05 / TMA / mbarrier helpers shared by the tensor-core convolution kernels (sm_100a).
+// eventgrad_b200 -- wgmma / TMA / mbarrier helpers shared by the tensor-core kernels (sm_90a).
 //
-// Descriptor bit layouts (checked against the vendored CUTLASS headers cute/arch/mma_sm100_desc.hpp and proven on
-// hardware by csrc/linear_tc_tma.cu):
-//   shared-memory descriptor: [0,14) start address >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte
-//   offset >> 4 | [46,48) version = 1 | [61,64) layout type (2 = SWIZZLE_128B)
-//   instruction descriptor (kind::f16): [4,6) D format (1 = F32) | [7,10) A format (1 = BF16) | [10,13) B format |
-//   bit 15 A major (0 = K, 1 = MN) | bit 16 B major | [17,23) N >> 3 | [24,29) M >> 4
+// Shared-memory matrix descriptor of wgmma (sm_90): [0,14) start address >> 4 | [16,30) leading byte offset >> 4 |
+// [32,46) stride byte offset >> 4 | [49,52) base offset (0: every tile is 1024-byte aligned) | [62,64) layout type
+// (1 = SWIZZLE_128B).  wgmma.mma_async multiplies a 64-row slice of A by an N-column slice of B for one warpgroup
+// (128 threads); the fp32 accumulator lives in registers, N/2 per thread:
+//   d[4j + 0..1] = D[16*warp + lane/4    ][8j + 2*(lane%4) + 0..1]
+//   d[4j + 2..3] = D[16*warp + lane/4 + 8][8j + 2*(lane%4) + 0..1]
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -55,46 +55,6 @@ __device__ __forceinline__ void tma_load_5d(uint32_t smem_dst, const CUtensorMap
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
-// One lane of a fully converged warp (elect.sync).  The MMA warp keeps its control flow warp-uniform and predicates only
-// the issue on this: inside `if (lane == 0)` ptxas cannot prove a single active thread and wraps EVERY tcgen05.mma
-// (a uniform-datapath instruction) in an ELECT / BRA.U.ANY loop with its descriptors rebuilt from vector registers --
-// ~35 cycles of issue per MMA, which capped the tensor pipe at 40 % (N = 64: 32 cycles of work per MMA) / 53-64 % (N = 128).
-__device__ __forceinline__ bool elect_one_sync() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-      "elect.sync rx|px, 0xFFFFFFFF;\n\t"
-      "selp.u32 %0, 1, 0, px;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns of the accumulator -> 32 registers per thread (thread = one row)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
 // K-major operand, SWIZZLE_128B: rows of 128 bytes (64 bf16 of K), 8-row (1024 B) swizzle atoms stacked along M/N.
 // Advancing K by 16 elements inside the 64-wide block = +32 bytes on the start address (+2 in the >>4 field).
@@ -103,11 +63,10 @@ __device__ __forceinline__ uint64_t desc_k_sw128(uint32_t saddr) {
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)1 << 16;                       // LBO: unused for swizzled K-major (canonical value 1)
   d |= (uint64_t)(1024u >> 4) << 32;            // SBO: next 8-row group
-  d |= 1ull << 46;
-  d |= 2ull << 61;
+  d |= 1ull << 62;                              // SWIZZLE_128B
   return d;
 }
-// MN-major operand, SWIZZLE_128B (canonical ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units): every K index is one
+// MN-major operand, SWIZZLE_128B (canonical ((8,8,m),(8,k)):((1,8,LBO),(64,SBO)) in elements): every K index is one
 // 128-byte row holding 64 consecutive M/N elements; 8 K-rows form a 1024-byte swizzle atom (SBO = distance between
 // consecutive 8-row groups along K); the next 64 M/N elements live `lbo_bytes` further (a separate [K][64] block).
 // Advancing K by 16 = 2 atoms = +2048 bytes on the start address.
@@ -116,21 +75,60 @@ __device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t saddr, uint32_t lbo_b
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)(1024u >> 4) << 32;
-  d |= 1ull << 46;
-  d |= 2ull << 61;
+  d |= 1ull << 62;
   return d;
 }
-__device__ __forceinline__ uint32_t idesc_bf16_f32(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(a_mn_major & 1) << 15) | ((uint32_t)(b_mn_major & 1) << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+
+// wgmma ordering: fence before the first MMA that touches registers written by ordinary instructions, commit the
+// issued MMAs as one group, wait until at most N groups are pending.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads/writes across an MMA that is still in flight
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(ncols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 in, fp32 accumulate; TA / TB: 0 = K-major, 1 = MN-major operand;
+// scale_d = 0 overwrites D.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(ncols));
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
 }  // namespace tc

@@ -50,13 +50,13 @@ class Trainer:
             torch.backends.cuda.matmul.allow_tf32 = tf32
             torch.backends.cudnn.allow_tf32 = tf32
             from ..ops import conv_tc as _conv_tc
-            _conv_tc.set_enabled(bool(cfg.conv_tc))       # fp32: eligible 3x3 convs on tcgen05 at fp32 accuracy
+            _conv_tc.set_enabled(bool(cfg.conv_tc))       # fp32: eligible 3x3 convs on wgmma at fp32 accuracy
         if dev.type == "cuda":
             torch.backends.cudnn.benchmark = bool(cfg.cudnn_benchmark)
             if cfg.host_threads > 0:
                 # The host side of a GPU step is a 0.8 MB gather + a few launches.  A 64-thread OpenMP
                 # pool for that costs milliseconds per step (wake-ups contending with the thread that
-                # polls CUDA events): measured 13.1 ms/step vs 4.3 ms with 2 threads (benchmarks/e2e_probe.py).
+                # polls CUDA events; benchmarks/e2e_probe.py isolates it).
                 torch.set_num_threads(cfg.host_threads)
         # identical initial weights on every rank: torch::manual_seed(0) (event.cpp:115)
         torch.manual_seed(cfg.seed)

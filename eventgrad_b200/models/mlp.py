@@ -24,7 +24,7 @@ class MLP(nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         x = x.reshape(x.shape[0], -1)
         if x.is_cuda and torch.is_autocast_enabled():
-            # Linear(784,128)+bias+ReLU over the whole shard: tcgen05 kernel with fused epilogue
+            # Linear(784,128)+bias+ReLU over the whole shard: wgmma kernel with fused epilogue
             from ..ops.linear_tc import linear_act
             w = self.fc1.w16 if self.fc1.w16 is not None else self.fc1.weight
             b = self.fc1.b16 if self.fc1.b16 is not None else self.fc1.bias

@@ -10,7 +10,7 @@ Reference: /root/reference/dcifar10/common/resnet.hpp
     shapes); `variant="canonical"` builds the textbook blocks-per-stage network
     (62 tensors / 11 173 962 elements for ResNet-18).
 BatchNorm layers are ops.bn_act.FusedBNAct (nn.BatchNorm2d subclass: same names/buffers) so that
-bn->relu and bn->(+=skip)->relu run as fused sm_100a kernels on bf16 NHWC activations.
+bn->relu and bn->(+=skip)->relu run as fused sm_90a kernels on bf16 NHWC activations.
 Parameter registration order matches LibTorch's named_parameters() walk
 (conv, bn, layer1..4 [conv1,bn1,conv2,bn2,(conv3,bn3),downsampler], fc) because the
 arena layout (= the reference's running `disp`) is defined by that order.

@@ -1,4 +1,4 @@
-"""Python front-ends of the sm_100a extension (eventgrad_b200/_C*.so, built by build_ext.py).
+"""Python front-ends of the sm_90a extension (eventgrad_b200/_C*.so, built by build_ext.py).
 
 `ext()` returns the compiled module.  On a machine with a GPU a missing / unloadable extension
 is a hard error -- there is deliberately NO silent PyTorch fallback for the fused ops, so a run
@@ -27,7 +27,7 @@ def ext():
             _EXT = importlib.import_module("eventgrad_b200._C")
         except Exception as e2:  # noqa: BLE001
             raise ImportError(
-                "eventgrad_b200._C (sm_100a extension) is not built and could not be built: "
+                "eventgrad_b200._C (sm_90a extension) is not built and could not be built: "
                 f"{e!r} / {e2!r}. Run `python -m eventgrad_b200.build_ext`.") from e2
     return _EXT
 

@@ -36,8 +36,8 @@ def _workspace(device):
               # fp32 NCHW kernels (csrc/bn_nchw.cu): per-channel tickets (forward | backward) + partial pairs
               "nchw_ticket": torch.zeros(2 * 2048, dtype=torch.int32, device=device),
               "nchw_partial": torch.empty(2048 * 64 * 2, dtype=torch.float32, device=device),
-              # single-launch (spin-flag) variant for small tensors: measured SLOWER than the two-launch
-              # split path inside a CUDA graph (1.52 vs 1.42 ms/step at batch 32), so it is opt-in
+              # single-launch (spin-flag) variant for small tensors: slower than the two-launch split path
+              # inside a CUDA graph, so it is opt-in
               "fused": 1 if os.environ.get("EGB_BN_FUSED_SMALL", "0") == "1" else 0}
         _WS[device] = ws
     return ws

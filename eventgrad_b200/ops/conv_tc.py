@@ -1,11 +1,11 @@
-"""Convolutions on the tcgen05 tensor cores at fp32 accuracy: front-end of csrc/conv_tc.cu.
+"""Convolutions on the wgmma tensor cores at fp32 accuracy: front-end of csrc/conv_tc.cu.
 
 The reference's convolutions are fp32 (/root/reference/dcifar10/common/resnet.hpp:3-9, event.cpp:259-276).  fp32 has
-no tensor-core path in cuDNN (SIMT kernels, 74 TFLOP/s peak), so the forward, the data gradient and the weight
+no tensor-core path in cuDNN (SIMT kernels, 67 TFLOP/s peak on an H100 SXM), so the forward, the data gradient and the weight
 gradient of every convolution of the ResNet family run here instead: each fp32 tensor is split into three bf16 planes
 (x = x0+x1+x2, 24 mantissa bits) and every product is rebuilt from six bf16 tensor-core MMAs accumulated in fp32 --
-fp32 storage, fp32 accuracy (measured against fp64 in tests/test_gpu_conv_tc.py: 1e-7 rms, cuDNN's fp32 kernels
-2-4e-7), tensor-core throughput.
+fp32 storage, fp32 accuracy (measured against fp64 in tests/test_gpu_conv_tc.py on an H100: 0.6-1.7e-7 rms, below
+cuDNN's fp32 kernels in every layer shape), tensor-core throughput.
 
 One kernel pair + a tap table (dh, dw, source sub-image, weight slice) serves five kinds of convolution:
     s1    3x3 stride 1 pad 1                     (BasicBlock / BottleNeck body)
@@ -151,7 +151,7 @@ def wprep(w_oti: torch.Tensor, transposed: bool):
 KSPLIT = os.environ.get("EGB_CONV_KSPLIT", "1") != "0"
 # weight gradient on a side stream, concurrent with the data gradient of the same layer (two branches inside the step's
 # CUDA graph): both kernels leave SMs idle at small per-GPU batches
-PAR_BWD = os.environ.get("EGB_CONV_PAR_BWD", "1") != "0"     # A/B on B200: 2.74 -> 2.65 ms at batch 32, 10.09 -> 10.06 at 256
+PAR_BWD = os.environ.get("EGB_CONV_PAR_BWD", "1") != "0"
 _SIDE = {}
 
 

@@ -1,7 +1,7 @@
-"""tcgen05 fused Linear + bias (+ ReLU): front-end of csrc/linear_tc_tma.cu (TMA, SWIZZLE_128B, persistent CTAs).
+"""wgmma fused Linear + bias (+ ReLU): front-end of csrc/linear_tc_tma.cu (TMA, SWIZZLE_128B, persistent CTAs).
 
-Forward runs on the 5th-generation tensor cores (tcgen05.mma, accumulator in TMEM, bias/ReLU fused
-into the TMEM->register epilogue).  Backward uses plain library GEMMs (cuBLAS through torch): it is
+Forward runs on the Hopper tensor cores (wgmma.mma_async, accumulator in registers, bias/ReLU fused
+into the register epilogue).  Backward uses plain library GEMMs (cuBLAS through torch): it is
 the forward of the full-batch MNIST MLP (60000/R x 784 x 128 per step) that is the hot GEMM.
 Eligibility: CUDA, bf16 operands, N % 16 == 0, 16 <= N <= 256, K % 8 == 0; otherwise F.linear.
 """
@@ -68,7 +68,7 @@ class _LinearTcFn(torch.autograd.Function):
 
 
 def linear_act(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], relu: bool) -> torch.Tensor:
-    """act(x @ weight.T + bias); tcgen05 path when eligible, PyTorch otherwise."""
+    """act(x @ weight.T + bias); wgmma path when eligible, PyTorch otherwise."""
     if tc_eligible(x, weight) and (x.dtype == torch.bfloat16 or torch.is_autocast_enabled()):
         return _LinearTcFn.apply(x, weight, bias, relu)
     y = F.linear(x, weight, bias)

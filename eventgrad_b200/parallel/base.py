@@ -4,7 +4,7 @@ A backend owns everything that happens between backward() and the next forward()
 the exchange (all-reduce or neighbour gossip), the consensus average and the optimizer
 update.  Three implementations:
 
-  p2p        fused sm_100a kernels over peer-mapped memory (the product)       parallel/p2p.py
+  p2p        fused sm_90a kernels over peer-mapped memory (the product)       parallel/p2p.py
   nccl/gloo  torch.distributed collectives + eager elementwise ops (baseline /
              GPU-free plumbing)                                                parallel/collective.py
 """

@@ -94,7 +94,7 @@ class P2PBackend(CommBackend):
 
     def __init__(self, cfg, arena: ParamArena, ring, env, group=None, symm=None,
                  grid_cap: int = 0, defer_connect: bool = False, group_iters: int = 2,
-                 timeout_ns: int = 0, vec256_push: bool = True, push_grid: int = 0):
+                 timeout_ns: int = 0, push_grid: int = 0):
         super().__init__(cfg, arena, ring)
         from ..ops import ext
         self.C = ext()
@@ -113,7 +113,7 @@ class P2PBackend(CommBackend):
         # balance: every CTA gets the same number of tiles (+-1 only on the last round)
         rounds = -(-t.n_tiles // self.grid)
         self.grid = -(-t.n_tiles // rounds)
-        self.group_iters, self.timeout_ns, self.vec256_push = group_iters, timeout_ns or default_timeout_ns(cfg), vec256_push
+        self.group_iters, self.timeout_ns = group_iters, timeout_ns or default_timeout_ns(cfg)
         self.sync = cfg.sync_mode == "iter"
         self.gossip = cfg.algo in ("decent", "event", "spevent")
         self.sparse = cfg.algo == "spevent"
@@ -235,7 +235,6 @@ class P2PBackend(CommBackend):
                 "sync": 1 if self.sync else 0,
                 "send_ack": 1 if dense else 0,
                 "zero_grad": 1, "group_iters": int(self.group_iters),
-                "vec256_push": 1 if self.vec256_push else 0,
                 "flag_from_l": win.addr("flag_from_l"), "flag_from_r": win.addr("flag_from_r"),
                 "flag_to_l": win.addr("flag_from_r", L), "flag_to_r": win.addr("flag_from_l", R),
                 "ack_from_l": win.addr("ack_from_l"), "ack_from_r": win.addr("ack_from_r"),

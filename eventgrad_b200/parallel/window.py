@@ -1,11 +1,11 @@
-"""Peer-mapped memory windows -- the B200-native replacement of the reference's MPI RMA window
+"""Peer-mapped memory windows -- the H100-native replacement of the reference's MPI RMA window
 (MPI_Alloc_mem + MPI_Win_create, /root/reference/dmnist/event/event.cpp:170-179).
 
 Every rank owns one device slab with an identical layout on all ranks (so "the same offset in
 my neighbour's slab" is the reference's `target_disp`).  Slabs are exported with CUDA IPC
 (native runtime: csrc/ipc.cu), the 64-byte handles are exchanged once through the process
 group, and each rank maps its peers' slabs.  A kernel-side `st.global` to a mapped address is
-the `MPI_Put`: it crosses NVLink 5 / NVSwitch directly into the peer's HBM.
+the `MPI_Put`: it crosses NVLink 4 / NVSwitch directly into the peer's HBM.
 
 Two bootstraps implement the same interface:
   DistBootstrap   one process per GPU (torchrun); handles travel via all_gather_object

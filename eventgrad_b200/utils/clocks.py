@@ -1,5 +1,5 @@
 """Sample GPU clocks / throttle reasons with nvidia-smi during a timed region
-(B200_PROFILING.md "clocks DURING the timed region")."""
+(the clocks DURING the timed region are part of a number)."""
 from __future__ import annotations
 
 import statistics

@@ -1,14 +1,12 @@
 #!/usr/bin/env python
-"""Write the full SASS listing of every kernel in the built extension to profiles/sass/<kernel>.sass
-(cuobjdump -sass of the sm_100a objects, one file per entry point) plus an index with the mnemonics that prove the
-Blackwell paths: UTCHMMA / UTMALDG / LDTM (tcgen05 + TMA), LDGMC / multimem (NVLS), ENL2.256 (256-bit global access).
-Runs on the CPU box (no GPU needed)."""
+"""Write the full SASS listing of every kernel in the built extension to <out>/<kernel>.sass
+(cuobjdump -sass of the sm_90a objects, one file per entry point) plus an index with the mnemonics that show the
+Hopper paths: HGMMA / WARPGROUP (wgmma), UTMALDG (TMA), SYNCS (mbarrier), LDGMC (multimem, NVLS).
+Needs no GPU.  Usage: python scripts/dump_sass.py [out_dir]   (default: eventgrad_b200/csrc/build/sass)"""
 import os, re, subprocess, sys, collections
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BUILD = os.path.join(ROOT, "eventgrad_b200", "csrc", "build")
-OUT = os.path.join(ROOT, "profiles", "sass")
-KEY = ["UTCHMMA", "UTCBAR", "UTMALDG", "LDTM", "LDGMC", "REDG", "SYNCS", "STG.E.ENL2.256", "LDG.E.ENL2.256",
-       "MEMBAR.SC.SYS", "ATOMS", "HMMA", "FFMA"]
+KEY = ["HGMMA", "WARPGROUP", "UTMALDG", "SYNCS", "LDGMC", "REDG", "MEMBAR.SC.SYS", "ATOMS", "HMMA", "FFMA"]
 
 
 def demangle(n):
@@ -19,6 +17,7 @@ def demangle(n):
 
 
 def main():
+    OUT = os.path.abspath(sys.argv[1]) if len(sys.argv) > 1 else os.path.join(BUILD, "sass")
     os.makedirs(OUT, exist_ok=True)
     for f in os.listdir(OUT):
         os.remove(os.path.join(OUT, f))
@@ -35,7 +34,7 @@ def main():
             short = re.sub(r"[^A-Za-z0-9_]+", "_", dm.split("(")[0].replace("egb::", "").replace("void ", ""))[:80].strip("_")
             path = os.path.join(OUT, f"{obj[:-5]}__{short}.sass")
             with open(path, "w") as fo:
-                fo.write(f"// {dm}\n// object: csrc/build/{obj}  (nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3)\n")
+                fo.write(f"// {dm}\n// object: csrc/build/{obj}  (nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3)\n")
                 # drop the raw 128-bit encodings (hex comments): they triple the size and add nothing to a review
                 lean = re.sub(r"[ \t]*/\* 0x[0-9a-f]{16} \*/", "", body)
                 lean = "\n".join(l.rstrip() for l in lean.split("\n") if l.strip())
@@ -45,7 +44,7 @@ def main():
             hits = {k: sum(v for o, v in ops.items() if o.startswith(k)) for k in KEY}
             index.append((os.path.basename(path), dm, n_ins, {k: v for k, v in hits.items() if v}))
     with open(os.path.join(OUT, "INDEX.md"), "w") as fo:
-        fo.write("# SASS listings (cuobjdump -sass, sm_100a) -- one file per kernel entry point\n\n"
+        fo.write("# SASS listings (cuobjdump -sass, sm_90a) -- one file per kernel entry point\n\n"
                  "| file | kernel | instructions | notable mnemonics |\n|---|---|---|---|\n")
         for f, dm, n, hits in index:
             fo.write(f"| `{f}` | `{dm[:110]}` | {n} | {', '.join(f'{k}x{v}' for k, v in hits.items())} |\n")

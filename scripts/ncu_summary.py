@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Summarise .ncu-rep captures (brought back in gpurun_out/) into tracked markdown under profiles/.
-Usage: python scripts/ncu_summary.py gpurun_out/prof_x.ncu-rep [...] > profiles/x.md"""
+"""Summarise .ncu-rep captures into markdown tables.
+Usage: python scripts/ncu_summary.py prof_x.ncu-rep [...] > x.md"""
 import csv
 import io
 import subprocess

@@ -66,7 +66,7 @@ def main():
         assert torch.isfinite(xa.grad.float()).all()
     _workspace(x.device)["fused"] = 0
     print("ok bn")
-    # tcgen05 linear
+    # wgmma linear
     from eventgrad_b200.ops.linear_tc import linear_tc_forward
     xx = torch.randn(200, 80, device="cuda").to(torch.bfloat16)
     ww = (torch.randn(32, 80, device="cuda") * 0.1).to(torch.bfloat16)
@@ -82,7 +82,7 @@ def main():
     p = draw_augment_params(9, 4, "cuda")
     assert torch.allclose(decode_augment(u, 1.0, 0.0, 1.0, p), decode_augment_torch(u, 1.0, 0.0, 1.0, p))
     print("ok augment")
-    # tcgen05 fp32-accuracy convolutions: every kind (forward, dgrad, wgrad; K-split and un-split grids), the fp32 BN
+    # wgmma fp32-accuracy convolutions: every kind (forward, dgrad, wgrad; K-split and un-split grids), the fp32 BN
     # kernels handing bf16 planes over, against cuDNN fp32
     import torch.nn.functional as F
     from eventgrad_b200.ops import conv_tc

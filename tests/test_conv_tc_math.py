@@ -59,21 +59,21 @@ def test_tile_geometry():
     for s in bad:
         assert not C.conv_tc_supported(*s), s
     # wgrad splits: enough CTAs to fill the GPU, never more splits than 64-pixel K blocks
-    assert C.conv_wgrad_splits(256, 32, 32, 64, 64, 9, 148) == 148 // 5
-    assert C.conv_wgrad_splits(256, 4, 4, 512, 512, 9, 148) == 1
-    assert C.conv_wgrad_splits(1, 8, 8, 64, 64, 9, 148) == 1
-    assert C.conv_wgrad_splits(256, 32, 32, 64, 64, 1, 148) == 148      # stem / 1x1: one unit pair
+    assert C.conv_wgrad_splits(256, 32, 32, 64, 64, 9, 132) == 132 // 5
+    assert C.conv_wgrad_splits(256, 4, 4, 512, 512, 9, 132) == 1
+    assert C.conv_wgrad_splits(1, 8, 8, 64, 64, 9, 132) == 1
+    assert C.conv_wgrad_splits(256, 32, 32, 64, 64, 1, 132) == 132      # stem / 1x1: one unit pair
 
 
 def test_fprop_k_splits_only_for_small_grids():
     C = ext()
-    assert C.conv_fprop_ksplits(256, 32, 32, 64, 64, 9, 148) == 1          # 2048 tiles: no split
-    assert C.conv_fprop_ksplits(256, 4, 4, 512, 512, 9, 148) == 1          # 128 tiles
-    ks = C.conv_fprop_ksplits(32, 4, 4, 512, 512, 9, 148)                  # 16 tiles, 72 k-blocks
-    assert ks == 9 and C.conv_fprop_mtiles(32, 4, 4) == 4
-    ks = C.conv_fprop_ksplits(32, 8, 8, 256, 256, 9, 148)                  # 32 tiles, 36 k-blocks -> 4 splits of 9
-    assert ks == 4
-    assert C.conv_fprop_ksplits(32, 16, 16, 64, 128, 1, 148) == 1          # 1x1 with one k-block: nothing to split
+    assert C.conv_fprop_ksplits(256, 32, 32, 64, 64, 9, 132) == 1          # 2048 tiles: no split
+    assert C.conv_fprop_ksplits(256, 4, 4, 512, 512, 9, 132) == 1          # 256 tiles
+    ks = C.conv_fprop_ksplits(32, 4, 4, 512, 512, 9, 132)                  # 32 tiles, 72 k-blocks -> 4 splits of 18
+    assert ks == 4 and C.conv_fprop_mtiles(32, 4, 4) == 4
+    ks = C.conv_fprop_ksplits(32, 8, 8, 256, 256, 9, 132)                  # 64 tiles, 36 k-blocks -> 2 splits of 18
+    assert ks == 2
+    assert C.conv_fprop_ksplits(32, 16, 16, 64, 128, 1, 132) == 1          # 1x1 with one k-block: nothing to split
 
 
 def test_tap_tables():

@@ -1,4 +1,4 @@
-"""tcgen05 fp32-accuracy 3x3 convolution (csrc/conv_tc.cu) against an fp64 convolution.
+"""wgmma fp32-accuracy 3x3 convolution (csrc/conv_tc.cu) against an fp64 convolution.
 
 The claim under test: the tensor-core path (three bf16 planes per fp32 tensor, six MMAs per product, fp32
 accumulation) is as accurate as cuDNN's native fp32 kernels.  Every case computes the TRUTH in fp64, measures
@@ -154,7 +154,7 @@ def test_wgrad_is_bitwise_reproducible():
 
 
 def test_whole_resnet_runs_on_the_tensor_core_convs_and_is_as_close_to_fp64_as_cudnn():
-    """every conv of the reference ResNet (stem, 3x3 s1/s2, 1x1 s2) takes the tcgen05 path, BN hands the bf16 planes
+    """every conv of the reference ResNet (stem, 3x3 s1/s2, 1x1 s2) takes the wgmma path, BN hands the bf16 planes
     over (no split pass between BN and the next conv), and the gradients of the whole network are as close to an fp64
     run of the same model as the gradients of the cuDNN fp32 run are (a 28-conv BN network amplifies round-off, so
     the two fp32 runs are compared against the TRUTH, not against each other)"""
@@ -194,7 +194,7 @@ def test_whole_resnet_runs_on_the_tensor_core_convs_and_is_as_close_to_fp64_as_c
 
 def test_bottleneck_resnet50_takes_the_tensor_core_path():
     """the BottleNeck family (1x1 stride-1 convs up to 2048 channels, 3x3 stride-2 inside the block, 1x1 stride-1 and
-    stride-2 down-samplers): every conv on the tcgen05 kernels, loss and gradients as close to fp64 as cuDNN's"""
+    stride-2 down-samplers): every conv on the wgmma kernels, loss and gradients as close to fp64 as cuDNN's"""
     import copy
     from eventgrad_b200.models.resnet import make_resnet
     from eventgrad_b200.ops import ext

@@ -1,4 +1,4 @@
-"""tcgen05 fused Linear+bias+ReLU vs a plain PyTorch fp32 reference of the same op."""
+"""wgmma fused Linear+bias+ReLU vs a plain PyTorch fp32 reference of the same op."""
 import pytest
 import torch
 

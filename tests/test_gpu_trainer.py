@@ -121,7 +121,7 @@ def test_p2p_file_write_logs(tmp_path):
 
 def test_gpu_defaults_are_the_fast_path_and_fp32_uses_fused_bn():
     """No execution flags: on a GPU the Trainer runs NHWC + whole-step CUDA graph; the fp32 activations go through
-    the fused BN kernels (csrc/bn_act.cu instantiated for float) and the fp32 convolutions through the tcgen05 kernels
+    the fused BN kernels (csrc/bn_act.cu instantiated for float) and the fp32 convolutions through the wgmma kernels
     (csrc/conv_tc.cu) -- counted through the extension's launch counter."""
     from eventgrad_b200.ops import ext
     C = ext()
