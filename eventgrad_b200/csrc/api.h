@@ -278,6 +278,7 @@ bool conv_tc_supported(int N, int H, int W, int Ca, int Cb);
 int conv_wgrad_splits(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count);
 int conv_fprop_ksplits(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count);
 int conv_fprop_mtiles(int N, int H, int W);   // 128-pixel tiles of the grid (workspace rows = 128 * this)
+int conv_fprop_ntile(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count);   // N tile of the launch: 64 | 128
 cudaError_t launch_conv_fprop(const ConvTcParams& p, int sm_count, cudaStream_t s);
 cudaError_t launch_conv_wgrad(const ConvTcParams& p, float* dw, int splits, cudaStream_t s);
 cudaError_t launch_split3(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t s);   // n % 8 == 0

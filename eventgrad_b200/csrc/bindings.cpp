@@ -281,6 +281,9 @@ PYBIND11_MODULE(_C, m) {
     return conv_fprop_ksplits(N, H, W, Ca, Cb, ntaps, sm);
   });
   m.def("conv_fprop_mtiles", [](int N, int H, int W) { return conv_fprop_mtiles(N, H, W); });
+  m.def("conv_fprop_ntile", [](int N, int H, int W, int Ca, int Cb, int ntaps, int sm) {
+    return conv_fprop_ntile(N, H, W, Ca, Cb, ntaps, sm);
+  });
   m.def("split3", [](uintptr_t src, uintptr_t dst, size_t n, uintptr_t s) {
     check(launch_split3(reinterpret_cast<const float*>(src), reinterpret_cast<__nv_bfloat16*>(dst), n, S(s)), "split3");
   });

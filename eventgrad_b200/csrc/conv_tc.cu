@@ -17,13 +17,14 @@
 //
 //   conv3x3_fprop_kernel   Y[pix, co] = sum_{tap,ci} X[pix+tap, ci] * Wt[co, tap, ci]        (forward; also the data
 //                          gradient: X := dY planes, Wt := flipped/transposed weights [ci][8-tap][co])
-//       persistent CTAs, tile 128 pixels x NT channels, K loop = 9 taps x Cin/64; warpgroup 0 is the TMA producer,
-//       warpgroups 1 and 2 each own 64 rows of the tile: 24 wgmma per stage into five FRESH register accumulators,
-//       each added into the fp32 tile sum (round-to-nearest adds: the tensor core itself truncates).
+//       persistent CTAs, tile 128 pixels x NT channels (NT = 128 or 64: conv_fprop_ntile), K loop = 9 taps x
+//       Cin/64; warpgroup 0 is the TMA producer (at NT = 128 it gives most of its registers to the MMA warpgroups,
+//       setmaxnreg), warpgroups 1 and 2 each own 64 rows of the tile: 24 wgmma per stage into five FRESH register
+//       accumulators, each added into the fp32 tile sum (round-to-nearest adds: the tensor core itself truncates).
 //   conv3x3_wgrad_kernel   dW[tap, ci, co] = sum_pix X[pix+tap, ci] * dY[pix, co]            (weight gradient)
 //       both operands are "MN-major" (the contiguous dimension is the channel, K = pixels), expressed with MN-major
 //       SWIZZLE_128B descriptors over the very same TMA boxes; split over pixel ranges, partial sums in a workspace
-//       (one split: dW is written directly).
+//       (one split: dW is written directly).  N tile 64 (see CV_WGRAD_NT).
 //   conv_wgrad_reduce_kernel   fixed-tree (bitwise reproducible) sum of the partials + transpose to the OHWI layout.
 //   conv_fprop_reduce_kernel   sum of the K-split partial tiles of the forward kernel on small grids (per-GPU batch 32).
 //   split3_kernel          fp32 -> three bf16 planes (flat; "parity" variant: the four (h%2, w%2) sub-images of the
@@ -49,10 +50,19 @@ using namespace tc;
 #define CV_CONSUMERS 256   // threads that arrive on an empty[] barrier (every MMA thread, after its wgmma wait)
 #define CV_APLANE 16384u   // one bf16 plane of an operand tile with 128 rows: 128 x 128 B
 #define CV_SMS 132         // grid cap of the element-wise launches (H100 SXM: 132 SMs)
-// N tile: 64 output channels.  Three register accumulators of NT/2 floats per thread (sum + two in flight) must fit
-// the 168 registers a thread of a 384-thread CTA can hold; NT = 128 would spill.
-#define CV_NT 64
-#define CV_STAGES 3        // 3 x 72 KB operand stages (A 3 x 16 KB + B 3 x 8 KB) of the 227 KB of shared memory
+// N tile of the forward / data-gradient kernel: 128 or 64 output channels, chosen per launch by conv_fprop_ntile.
+// An MMA warpgroup holds three accumulator sets of NT/2 floats per thread (the sum + two in flight): 192 registers
+// at NT = 128, more than the 168 a thread of a 384-thread CTA launches with.  So at NT = 128 the producer warpgroup,
+// whose one working thread only issues TMA, drops to CV_PRODUCER_REGS and the MMA warpgroups rise to CV_MMA_REGS
+// (128 x 40 + 256 x 232 = 64512 = 384 x 168).  The wider tile reads A from shared memory once per 128
+// output channels instead of 64, and spreads the per-k-block barriers and descriptors over twice the MMA work.
+#define CV_PRODUCER_REGS 40
+#define CV_MMA_REGS 232
+// N tile of the weight-gradient kernel: 64.  At 128 its MMA warpgroups need more than 232 registers (ptxas spills
+// about 400 bytes per thread, also at a 24 / 240 split), so it stays at 64.
+#define CV_WGRAD_NT 64
+// operand stages in the 227 KB of shared memory: NT = 64: 3 x 72 KB (A 3 x 16 KB + B 3 x 8 KB); NT = 128: 2 x 96 KB
+#define CV_STAGES(NT) ((NT) == 128 ? 2 : 3)
 
 // the six cross terms (plane of A, plane of B), largest last so that the small corrections are summed first
 #define CV_TERM_A(t) ((t) == 0 ? 2 : ((t) == 2 || (t) == 3) ? 1 : 0)
@@ -60,8 +70,10 @@ using namespace tc;
 
 template <int NT, int TA, int TB>
 __device__ __forceinline__ void mma_nt(float (&d)[NT / 2], uint64_t da, uint64_t db, uint32_t acc) {
-  static_assert(NT == 64, "N tile");
-  wgmma_m64n64<TA, TB>(d, da, db, acc);
+  if constexpr (NT == 128)
+    wgmma_m64n128<TA, TB>(d, da, db, acc);
+  else
+    wgmma_m64n64<TA, TB>(d, da, db, acc);
 }
 
 // One k-block of the six-term product for this warpgroup's 64 rows.  The tensor core TRUNCATES every accumulation
@@ -161,6 +173,7 @@ conv3x3_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
 
   if (wg == 0) {
     // ===================== TMA PRODUCER (one thread) =====================
+    if constexpr (NT == 128) setmaxnreg_dec<CV_PRODUCER_REGS>();
     if (tid == 0) {
       uint32_t it = 0;
       for (int work = blockIdx.x; work < total; work += gridDim.x) {
@@ -185,6 +198,7 @@ conv3x3_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     }
   } else {
     // ===================== MMA + EPILOGUE (rows 64g .. 64g+63 of every tile) =====================
+    if constexpr (NT == 128) setmaxnreg_inc<CV_MMA_REGS>();
     const int g = wg - 1, warp = (tid >> 5) & 3, lane = tid & 31;
     const long long M = (long long)p.N * p.H * p.W;
     float d[NT / 2], e[NT / 2];
@@ -559,7 +573,7 @@ bool conv_tc_supported(int N, int H, int W, int Ca, int Cb) {
 int conv_wgrad_splits(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count) {
   int bh, bn, kblocks;
   if (!tile_geometry(N, H, W, 64, &bh, &bn, &kblocks)) return 0;
-  const int NT = CV_NT;
+  const int NT = CV_WGRAD_NT;
   const int U = ntaps * (Ca / 64);
   const int work = ((U + 1) / 2) * (Cb / NT);
   int s = sm_count / work;
@@ -575,11 +589,12 @@ static bool taps_ok(const ConvTcParams& p) {
   return true;
 }
 
-// K-loop splits of the forward kernel: only when the tiles alone leave most SMs idle (small per-GPU batch)
+// K-loop splits of the forward kernel: only when the tiles alone leave most SMs idle (small per-GPU batch).  Counted
+// at the 64-wide N tile, which is the one a split launch runs.
 int conv_fprop_ksplits(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count) {
   int bh, bn, m_tiles;
   if (!tile_geometry(N, H, W, 128, &bh, &bn, &m_tiles)) return 0;
-  const int NT = CV_NT;
+  const int NT = 64;
   const int tiles = m_tiles * (Cb / NT), num_kb = ntaps * (Ca / 64);
   if (tiles * 2 > sm_count || num_kb < 4) return 1;
   int ks = sm_count / tiles;
@@ -592,6 +607,19 @@ int conv_fprop_ksplits(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_co
 int conv_fprop_mtiles(int N, int H, int W) {
   int bh, bn, m_tiles;
   return tile_geometry(N, H, W, 128, &bh, &bn, &m_tiles) ? m_tiles : 0;
+}
+
+// N tile of the forward / data-gradient launch.  128 needs Cb % 128 == 0 and an un-split K loop, and the busiest SM
+// of the persistent grid must get no more MMA work than at 64: 2 * waves(t) <= waves(2t), t = 128-wide tiles.  A
+// 128 x 128 tile does twice the work of a 128 x 64 one at about 1.15x the rate (H100 SXM at 700 W, batch 256:
+// 82-84 -> 94-97 fp32-equivalent TFLOP/s), so when the 128-wide grid fills fewer SMs, 64 is faster.  That happens
+// to the small grids of the multi-GPU per-GPU batches, e.g. 16x16x128 at batch 32: 64 tiles at 128 vs 128 at 64 on
+// 132 SMs, 40 against 64 TFLOP/s measured at 400 W (DESIGN.md section 5a).
+int conv_fprop_ntile(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count) {
+  if (Cb % 128 != 0 || sm_count < 1 || conv_fprop_ksplits(N, H, W, Ca, Cb, ntaps, sm_count) != 1) return 64;
+  const int t = conv_fprop_mtiles(N, H, W) * (Cb / 128);
+  const int waves128 = (t + sm_count - 1) / sm_count, waves64 = (2 * t + sm_count - 1) / sm_count;
+  return 2 * waves128 <= waves64 ? 128 : 64;
 }
 
 template <int NT, int STAGES>
@@ -617,13 +645,14 @@ cudaError_t launch_conv_fprop(const ConvTcParams& p0, int sm_count, cudaStream_t
     if (p.ksplits != want) return cudaErrorInvalidValue;
   }
   CUtensorMap tmA, tmB;
-  const int NT = CV_NT;
+  const int NT = conv_fprop_ntile(p.N, p.H, p.W, p.Ca, p.Cb, p.ntaps, sm_count);
   if (!make_map_w(&tmB, p.b, (uint64_t)p.wtaps * p.Ca, (uint64_t)3 * p.Cb, (uint32_t)NT)) return cudaErrorNotSupported;
   const int total = p.m_tiles * (p.Cb / NT) * p.ksplits;
   const int grid = total < sm_count ? total : sm_count;
   if (!make_map_act(&tmA, p.a, p.Ca, p.W, p.H, p.N, 3 * p.nsrc, p.W, p.bh, p.bn)) return cudaErrorNotSupported;
   eg_count_launch(EG_FAM_CONV, p.ksplits > 1 ? 2 : 1);
-  cudaError_t e = fprop_launch<CV_NT, CV_STAGES>(tmA, tmB, p, grid, s);
+  cudaError_t e = NT == 128 ? fprop_launch<128, CV_STAGES(128)>(tmA, tmB, p, grid, s)
+                            : fprop_launch<64, CV_STAGES(64)>(tmA, tmB, p, grid, s);
   if (e != cudaSuccess || p.ksplits == 1) return e;
   const long long n4 = (long long)p.N * p.H * p.W * (p.Cb / 4);
   long long blocks = (n4 + 255) / 256;
@@ -650,14 +679,14 @@ cudaError_t launch_conv_wgrad(const ConvTcParams& p0, float* dw, int splits, cud
   tile_geometry(p.N, p.H, p.W, 64, &p.bh, &p.bn, &p.k_blocks);
   if (splits > p.k_blocks) splits = p.k_blocks;
   CUtensorMap tmX, tmG;
-  const int NT = CV_NT;
+  const int NT = CV_WGRAD_NT;
   if (!make_map_act(&tmX, p.a, p.Ca, p.W, p.H, p.N, 3 * p.nsrc, p.W, p.bh, p.bn)) return cudaErrorNotSupported;
   if (!make_map_act(&tmG, p.b, p.Cb, p.W, p.H, p.N, 3, p.W, p.bh, p.bn)) return cudaErrorNotSupported;
   const int U = p.ntaps * (p.Ca / 64);
   const dim3 grid((U + 1) / 2, p.Cb / NT, splits);
   p.dwout = dw;
   eg_count_launch(EG_FAM_CONV, splits > 1 ? 2 : 1);
-  cudaError_t e = wgrad_launch<CV_NT, CV_STAGES>(tmX, tmG, p, grid, s);
+  cudaError_t e = wgrad_launch<CV_WGRAD_NT, CV_STAGES(CV_WGRAD_NT)>(tmX, tmG, p, grid, s);
   if (e != cudaSuccess || splits == 1) return e;
   const int rows = p.ntaps * p.Ca;
   conv_wgrad_reduce_kernel<<<dim3((rows + 31) / 32, p.Cb / 32), 256, 0, s>>>(p.out, dw, rows, p.Cb, splits);

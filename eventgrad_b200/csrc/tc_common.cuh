@@ -85,6 +85,14 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Warp-specialised register split: every warp of a warpgroup calls the same one.  The CTA launches with the register
+// count of its launch bounds; a producer warpgroup that only issues TMA hands registers back (dec) and the MMA
+// warpgroups take them (inc), so their accumulators may exceed the launch-bounds limit.  N: multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // keeps the compiler from moving accumulator reads/writes across an MMA that is still in flight
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
