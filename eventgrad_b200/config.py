@@ -17,7 +17,7 @@ from __future__ import annotations
 import argparse
 import dataclasses
 from dataclasses import dataclass
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 ALGOS = ("cent", "decent", "event", "spevent")
 DATASETS = ("mnist", "cifar10")
@@ -37,6 +37,16 @@ class TrainConfig:
     lr: float = 1e-2
     momentum: float = 0.9
     seed: int = 0
+    # torch.optim.SGD options and learning-rate schedule, applied inside the fused step kernels (absent in the
+    # reference: the defaults reproduce its constant-lr heavy-ball SGD).  See engine/lr_schedule.py.
+    weight_decay: float = 0.0        # L2 on every arena tensor (BN included), as SGD without parameter groups
+    nesterov: bool = False           # needs momentum > 0
+    lr_schedule: str = "constant"    # constant | step | multistep | cosine
+    lr_step_epochs: int = 30         # step: multiply by lr_gamma every this many epochs
+    lr_milestones: Tuple[int, ...] = ()   # multistep: epochs at which lr is multiplied by lr_gamma
+    lr_gamma: float = 0.1
+    lr_min: float = 0.0              # cosine: final learning rate
+    lr_warmup_epochs: float = 0.0    # linear warm-up, stepped per step (0: none)
     # ---- event trigger (SURVEY.md A.1) -------------------------------------
     thres_type: int = 1              # 1 adaptive (horizon), 0 constant
     horizon: float = 1.0
@@ -106,6 +116,19 @@ class TrainConfig:
             raise ValueError("topk_percent must be in (0, 100]")
         if self.dtype not in ("fp32", "tf32", "bf16"):
             raise ValueError("dtype must be fp32|tf32|bf16")
+        if not self.weight_decay >= 0.0:
+            raise ValueError(f"weight_decay must be >= 0, got {self.weight_decay}")
+        if self.nesterov and self.momentum == 0.0:
+            raise ValueError("nesterov requires momentum > 0")
+        if self.lr_schedule not in ("constant", "step", "multistep", "cosine"):
+            raise ValueError(f"lr_schedule must be constant|step|multistep|cosine, got {self.lr_schedule!r}")
+        if self.lr_schedule == "step" and self.lr_step_epochs < 1:
+            raise ValueError("lr_step_epochs must be >= 1")
+        ms = list(self.lr_milestones)
+        if any(b <= a for a, b in zip(ms, ms[1:])) or any(m < 0 for m in ms):
+            raise ValueError(f"lr_milestones must be non-negative and strictly increasing, got {ms}")
+        if not self.lr_warmup_epochs >= 0.0:
+            raise ValueError("lr_warmup_epochs must be >= 0")
         return self
 
     def resolved(self, device_type: str, world: int) -> "TrainConfig":
@@ -173,6 +196,16 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--batch-mode", default=None, choices=["global", "per_rank", "full"])
     p.add_argument("--lr", type=float, default=None)
     p.add_argument("--momentum", type=float, default=None)
+    p.add_argument("--weight-decay", type=float, default=None, help="L2 weight decay on every parameter (default 0)")
+    p.add_argument("--nesterov", action=argparse.BooleanOptionalAction, default=None,
+                   help="Nesterov momentum (needs --momentum > 0)")
+    p.add_argument("--lr-schedule", default=None, choices=["constant", "step", "multistep", "cosine"])
+    p.add_argument("--lr-step-epochs", type=int, default=None, help="step schedule: period in epochs")
+    p.add_argument("--lr-milestones", type=lambda s: tuple(int(x) for x in s.split(",") if x.strip()), default=None,
+                   metavar="E1,E2,...", help="multistep schedule: epochs at which lr is multiplied by --lr-gamma")
+    p.add_argument("--lr-gamma", type=float, default=None)
+    p.add_argument("--lr-min", type=float, default=None, help="cosine schedule: final learning rate")
+    p.add_argument("--lr-warmup-epochs", type=float, default=None, help="linear warm-up, stepped per step")
     p.add_argument("--seed", type=int, default=None)
     p.add_argument("--sent-history", type=int, default=None)
     p.add_argument("--initial-comm-passes", type=int, default=None)

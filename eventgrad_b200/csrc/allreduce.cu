@@ -45,20 +45,13 @@ __device__ __forceinline__ void cta_barrier_all_ranks(const AllReduceParams& p, 
 }
 
 template <bool kMom>
-__device__ __forceinline__ void sgd_tile(const AllReduceParams& p, size_t base, const F8& g) {
+__device__ __forceinline__ void sgd_tile(const AllReduceParams& p, size_t base, const F8& g, float lr) {
   F8 th = ld_f8(p.theta + base);
-  if (kMom) {
-    F8 m = ld_f8(p.mom + base);
+  F8 m;
+  if (kMom) m = ld_f8(p.mom + base);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      m.v[e] = __fadd_rn(__fmul_rn(m.v[e], p.mu), g.v[e]);
-      th.v[e] = __fmaf_rn(m.v[e], -p.lr, th.v[e]);
-    }
-    st_f8(p.mom + base, m);
-  } else {
-#pragma unroll
-    for (int e = 0; e < 8; ++e) th.v[e] = __fmaf_rn(g.v[e], -p.lr, th.v[e]);
-  }
+  for (int e = 0; e < 8; ++e) th.v[e] = sgd_elem<kMom>(th.v[e], g.v[e], m.v[e], lr, p.mu, p.wd, p.nesterov);
+  if (kMom) st_f8(p.mom + base, m);
   st_f8(p.theta + base, th);
   if (p.shadow != nullptr) st_bf16x8(p.shadow + base, th);
 }
@@ -107,6 +100,9 @@ template <bool kMom>
 __global__ void __launch_bounds__(EG_THREADS, 4) EG_AR_SYM(allreduce_kernel)(const AllReduceParams p) {
   const int b = blockIdx.x, G = gridDim.x, tid = threadIdx.x;
   const uint32_t seq = (uint32_t)(*p.step_ctr) + 1u;
+  // SGD mode: training step of this launch (the rank's device pass counter, advanced in the tail below)
+  const int step = (p.pass_num != nullptr) ? *p.pass_num + 1 : 0;
+  const float lr = sched_lr(p.lr_table, p.lr_len, p.lr, step);
   F8 zero;
 #pragma unroll
   for (int e = 0; e < 8; ++e) zero.v[e] = 0.f;
@@ -118,7 +114,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_AR_SYM(allreduce_kernel)(con
     for (int t = b; t < p.n_tiles; t += G) {
       const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
       const F8 g = reduce_tile(p, base);
-      if (p.mode == 1) sgd_tile<kMom>(p, base, g);
+      if (p.mode == 1) sgd_tile<kMom>(p, base, g, lr);
     }
     // nobody may overwrite (or zero) its buffer while a peer is still reading it
     cta_barrier_all_ranks(p, 2, b, G, seq);
@@ -142,12 +138,13 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_AR_SYM(allreduce_kernel)(con
       for (int t = b; t < p.n_tiles; t += G) {
         const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
         const F8 g = ld_f8_cg(p.local + base);
-        sgd_tile<kMom>(p, base, g);
+        sgd_tile<kMom>(p, base, g, lr);
         if (p.zero_after) st_f8(p.local + base, zero);
       }
     }
   }
-  // bump the launch counter once per grid
+  // bump the launch counter (and, in SGD mode, the pass counter) once per grid: every CTA has read both before
+  // its ticket
   __syncthreads();
   if (tid == 0) {
     __threadfence();
@@ -155,6 +152,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_AR_SYM(allreduce_kernel)(con
     if (prev == gridDim.x - 1) {
       *p.ticket = 0u;
       *p.step_ctr = (int)seq;
+      if (p.pass_num != nullptr) *p.pass_num = step;
     }
   }
 }

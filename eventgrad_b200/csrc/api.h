@@ -101,6 +101,11 @@ struct GossipParams {
                             // the arrived (value, index) records into inbox_l / inbox_r (the replicas) first
   int need_norm;            // 0: skip norm-on-write + trigger entirely (decent/cent without logs)
   int phase;                // 0 fused step | 1 push only (side stream, overlaps backward) | 2 wait+mix+SGD
+  // optimizer options (torch.optim.SGD semantics, applied after the mix; see sgd_elem in common.cuh)
+  float wd;                 // weight decay, every arena tensor (0: off)
+  int nesterov;             // 1: Nesterov momentum (needs mu > 0)
+  const float* lr_table;    // optional [lr_len]: lr of step s is lr_table[min(s-1, lr_len-1)]; null: the scalar lr
+  int lr_len;
 };
 
 int gossip_max_grid(int device);  // co-resident CTAs (persistent grid upper bound)
@@ -139,6 +144,13 @@ struct AllReduceParams {
   int two_shot;             // 0: every rank reads all peers   1: reduce-scatter + broadcast
   int zero_after;
   float* mc_local;          // NVLS variant only: multicast (NVSwitch) mapping of `local`; null otherwise
+  // SGD mode: optimizer options as in GossipParams, and the rank's device pass counter (the step index into
+  // lr_table), advanced once per launch in the tail.  pass_num null: not advanced (averaging mode).
+  float wd;
+  int nesterov;
+  const float* lr_table;
+  int lr_len;
+  int* pass_num;
 };
 cudaError_t launch_allreduce(const AllReduceParams& p, int grid, cudaStream_t s);
 // experimental NVLink-SHARP variant (csrc/allreduce_nvls.cu): multimem.ld_reduce + multimem.st, two-shot only

@@ -52,6 +52,7 @@ static const std::unordered_map<std::string, Setter<GossipParams>> kGossip = {
     NUMF(GossipParams, do_mix), NUMF(GossipParams, do_push), NUMF(GossipParams, sync),
     NUMF(GossipParams, send_ack), NUMF(GossipParams, zero_grad), NUMF(GossipParams, group_iters),
     PTRF(GossipParams, sparse), NUMF(GossipParams, need_norm), NUMF(GossipParams, phase), TAB_FIELDS(GossipParams),
+    NUMF(GossipParams, wd), NUMF(GossipParams, nesterov), PTRF(GossipParams, lr_table), NUMF(GossipParams, lr_len),
     PTRF2(GossipParams, fsm, thres), PTRF2(GossipParams, fsm, last_norm), PTRF2(GossipParams, fsm, last_iter),
     PTRF2(GossipParams, fsm, slopes), PTRF2(GossipParams, fsm, fire), PTRF2(GossipParams, fsm, cur_norm),
     PTRF2(GossipParams, fsm, counters), PTRF2(GossipParams, fsm, pass_num), PTRF2(GossipParams, fsm, log_ring),
@@ -68,6 +69,8 @@ static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce
     NUMF(AllReduceParams, rank), NUMF(AllReduceParams, world), NUMF(AllReduceParams, lr),
     NUMF(AllReduceParams, mu), NUMF(AllReduceParams, mode), NUMF(AllReduceParams, two_shot),
     NUMF(AllReduceParams, zero_after), PTRF(AllReduceParams, mc_local),
+    NUMF(AllReduceParams, wd), NUMF(AllReduceParams, nesterov), PTRF(AllReduceParams, lr_table),
+    NUMF(AllReduceParams, lr_len), PTRF(AllReduceParams, pass_num),
 };
 
 static const std::unordered_map<std::string, Setter<SparseParams>> kSparse = {

@@ -118,4 +118,27 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   return v;
 }
 
+// ---------------------------------------------------------------- optimizer (torch.optim.SGD, dampening 0)
+// Learning rate of training step `step` (1-based): table[min(step-1, len-1)] (engine/lr_schedule.py), or the
+// scalar lr when no table is set.  `step` comes from the device-resident pass counter, so a captured CUDA graph
+// follows the schedule on every replay.
+__device__ __forceinline__ float sched_lr(const float* table, int len, float lr, int step) {
+  if (table == nullptr || len <= 0) return lr;
+  const int i = step < 1 ? 0 : (step > len ? len - 1 : step - 1);
+  return __ldg(table + i);
+}
+
+// One element of the update, rounded as torch.optim.SGD rounds it (parallel/trigger.py:sgd_ is the oracle):
+//   d = wd != 0 ? fma(theta, wd, g) : g;   m = m*mu + d;   d = nesterov ? fma(m, mu, d) : m;   theta = fma(d, -lr, theta)
+// wd == 0 and nesterov == 0 give exactly the plain heavy-ball step.  All branches are uniform across the grid.
+template <bool kMom>
+__device__ __forceinline__ float sgd_elem(float th, float g, float& m, float lr, float mu, float wd, int nesterov) {
+  float d = (wd != 0.f) ? __fmaf_rn(th, wd, g) : g;
+  if (kMom) {
+    m = __fadd_rn(__fmul_rn(m, mu), d);
+    d = nesterov ? __fmaf_rn(m, mu, d) : m;
+  }
+  return __fmaf_rn(d, -lr, th);
+}
+
 }  // namespace egb

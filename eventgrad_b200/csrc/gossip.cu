@@ -12,7 +12,9 @@
 //               async mode reads whatever the inboxes hold (reference: unsynchronised window
 //               reads, event.cpp:372-374).
 //   3. mix+opt: theta <- ((theta+L)+R)/3 ; m <- mu*m+g ; theta <- theta - lr*m   (event.cpp:
-//               459-461, :479), rounding identical to add_/add_/div_/SGD.
+//               459-461, :479), rounding identical to add_/add_/div_/SGD.  Optionally with weight decay,
+//               Nesterov momentum and a per-step learning rate read from a device table (sgd_elem/sched_lr,
+//               common.cuh; off by default).
 //   4. norm-on-write: per-warp sum theta_new^2 partials; the last CTA reduces them per tensor
 //               in fixed order and runs the trigger FSM for the NEXT step (event.cpp:300-355),
 //               so the step needs no extra pass over theta, no grid sync and no host sync.
@@ -278,22 +280,15 @@ __device__ __forceinline__ void mix_tile(const GossipParams& p, int t, const Til
       }
     }
   }
+  // learning rate of this step, looked up per tile (an L1 hit) rather than held in a register across the loop
+  const float lr = sched_lr(p.lr_table, p.lr_len, p.lr, step);
   float ss = 0.f;
-  if (kMom) {
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      m.v[e] = __fadd_rn(__fmul_rn(m.v[e], p.mu), g.v[e]);
-      th.v[e] = __fmaf_rn(m.v[e], -p.lr, th.v[e]);
-      ss = __fmaf_rn(th.v[e], th.v[e], ss);
-    }
-    st_f8(p.mom + base, m);
-  } else {
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      th.v[e] = __fmaf_rn(g.v[e], -p.lr, th.v[e]);
-      ss = __fmaf_rn(th.v[e], th.v[e], ss);
-    }
+  for (int e = 0; e < 8; ++e) {
+    th.v[e] = sgd_elem<kMom>(th.v[e], g.v[e], m.v[e], lr, p.mu, p.wd, p.nesterov);
+    ss = __fmaf_rn(th.v[e], th.v[e], ss);
   }
+  if (kMom) st_f8(p.mom + base, m);
   st_f8(p.theta + base, th);
   if (p.shadow != nullptr) st_bf16x8(p.shadow + base, th);
   if (p.zero_grad && ti.gptr == nullptr) {
@@ -308,7 +303,6 @@ __device__ __forceinline__ void mix_tile(const GossipParams& p, int t, const Til
     ssr = warp_sum(ssr);
   }
   if (!p.need_norm) return;
-  (void)step;
   if (lane == 0) {
     p.tile_ss[(size_t)t * EG_WARPS + warp] = ss;
     if (logrecv) {

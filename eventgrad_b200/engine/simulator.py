@@ -14,16 +14,21 @@ import torch
 from ..parallel.arena import TensorTable
 from ..parallel.trigger import (TriggerConfig, TriggerState, mix3_, sgd_, topk_select,
                                 trigger_step)
+from .lr_schedule import lr_at
 
 
 class RingSimulator:
     def __init__(self, world: int, theta0: torch.Tensor, table: TensorTable, algo: str,
                  tcfg: Optional[TriggerConfig] = None, lr: float = 1e-2, momentum: float = 0.0,
-                 topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None):
+                 topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
+                 weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None):
+        """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
+        None = the constant `lr`."""
         assert algo in ("cent", "decent", "event", "spevent")
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
+        self.wd, self.nesterov, self.lr_table = weight_decay, nesterov, lr_table
         self.serial_skip = serial_skip
         self.theta = [theta0.clone() for _ in range(world)]
         self.mom = [torch.zeros_like(theta0) for _ in range(world)]
@@ -53,6 +58,10 @@ class RingSimulator:
         return torch.stack([torch.linalg.vector_norm(self._flat(buf, i))
                             for i in range(self.table.n_tensors)]).float()
 
+    def _sgd(self, r, grad):
+        lr = lr_at(self.lr_table, self.pass_num, self.lr)
+        sgd_(self.theta[r], grad, self.mom[r], lr, self.mu, self.wd, self.nesterov)
+
     def left(self, r):
         return (r - 1) % self.R
 
@@ -71,11 +80,11 @@ class RingSimulator:
         if self.algo == "cent":
             g = torch.stack(list(grads)).sum(0) / R if R > 1 else grads[0]
             for r in range(R):
-                sgd_(self.theta[r], g, self.mom[r], self.lr, self.mu)
+                self._sgd(r, g)
                 self.bytes[r] += t.n_elems * 4 if R > 1 else 0
             return
         if R == 1 and self.serial_skip:
-            sgd_(self.theta[0], grads[0], self.mom[0], self.lr, self.mu)
+            self._sgd(0, grads[0])
             return
         # ---- phase 1: every rank decides and "Puts" (uses pre-mix theta_k) --------------
         if self.algo == "decent":
@@ -114,7 +123,7 @@ class RingSimulator:
                 mix3_(self.theta[r], self.rep_l[r], self.rep_r[r])
             else:
                 mix3_(self.theta[r], self.inbox_l[r], self.inbox_r[r])
-            sgd_(self.theta[r], grads[r], self.mom[r], self.lr, self.mu)
+            self._sgd(r, grads[r])
 
     def final_average(self) -> torch.Tensor:
         return torch.stack(self.theta).sum(0) / self.R

@@ -29,6 +29,7 @@ from ..utils.ckpt import ckpt_path, load_checkpoint, save_checkpoint
 from ..utils.dist import DistEnv, barrier
 from ..utils.logfiles import RefLogWriter
 from ..utils.timers import PhaseTimer
+from . import lr_schedule
 
 
 def _compute_dtype(cfg: TrainConfig):
@@ -93,6 +94,9 @@ class Trainer:
                                   augment=cfg.augment and cfg.dataset == "cifar10",
                                   out_dtype=torch.float32, channels_last=cfg.channels_last,
                                   seed=cfg.seed, native=cfg.native_loader)
+        if not lr_schedule.is_constant(cfg):
+            # one lr per step of the run, indexed by the backend's (device) pass counter -- also after a resume
+            self.backend.set_lr_table(lr_schedule.lr_table(cfg, len(self.loader)))
         self.logw = RefLogWriter(cfg.log_dir, env.rank, cfg.algo, cfg.dataset, bool(cfg.file_write))
         self.timer = PhaseTimer(dev, enabled=bool(cfg.phase_timers))
         self.correct = torch.zeros((), dtype=torch.int64, device=dev)

@@ -39,6 +39,18 @@ class CommBackend:
         self.pass_num = 0
         self.logs: List[StepLog] = []
         self.want_logs = bool(cfg.file_write)
+        self.lr_table: Optional[torch.Tensor] = None
+
+    # -- learning-rate schedule (engine/lr_schedule.py) ------------------------------------
+    def set_lr_table(self, table: Optional[torch.Tensor]) -> None:
+        """Per-step learning rates of the run (fp32, step s uses table[min(s-1, len-1)]); None = constant cfg.lr.
+        The step index is the backend's pass counter, so a restored checkpoint resumes mid-schedule."""
+        self.lr_table = None if table is None else table.detach().to("cpu", torch.float32).contiguous()
+
+    def step_lr(self, step: int) -> float:
+        """Learning rate of 1-based training step `step`."""
+        from ..engine.lr_schedule import lr_at
+        return lr_at(self.lr_table, step, self.cfg.lr)
 
     # -- one training step (after backward) -------------------------------------------
     def step(self) -> None:

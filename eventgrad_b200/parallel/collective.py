@@ -99,8 +99,8 @@ class CollectiveBackend(CommBackend):
                 w.wait()
 
     def _opt(self) -> None:
-        a = self.arena
-        sgd_(a.theta, a.grad, a.mom, self.cfg.lr, self.cfg.momentum)
+        a, cfg = self.arena, self.cfg
+        sgd_(a.theta, a.grad, a.mom, self.step_lr(self.pass_num), cfg.momentum, cfg.weight_decay, cfg.nesterov)
 
     # ------------------------------------------------------------------ step
     @torch.no_grad()

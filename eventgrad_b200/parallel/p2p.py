@@ -192,6 +192,7 @@ class P2PBackend(CommBackend):
         self.host_bytes = 0
         self._connected = False
         self.gp = self.ap = self.ap_avg = self.sp = None
+        self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
             self.boot.publish("grid", self.grid)
@@ -229,6 +230,7 @@ class P2PBackend(CommBackend):
                 "ticket": P(self.ticket), "tensor_done": P(self.tensor_done), "status": P(self.status),
                 "timeout_ns": int(self.timeout_ns),
                 "lr": float(cfg.lr), "mu": float(cfg.momentum),
+                "wd": float(cfg.weight_decay), "nesterov": 1 if cfg.nesterov else 0,
                 "need_norm": 1 if (cfg.algo in ("event", "spevent") or self.log_ring is not None) else 0,
                 "do_mix": 1 if self.do_comm else 0,
                 "do_push": 1 if (self.do_comm and dense) else 0,
@@ -311,6 +313,8 @@ class P2PBackend(CommBackend):
         ap.update(common)
         ap.update({"peer_bufs": P(self.d_peer_grad), "local": P(a.grad), "theta": P(a.theta),
                    "mom": P(a.mom) if cfg.momentum != 0 else 0, "mode": 1, "zero_after": 1,
+                   "wd": float(cfg.weight_decay), "nesterov": 1 if cfg.nesterov else 0,
+                   "pass_num": P(self.d_pass),      # cent's device step index: the all-reduce advances it
                    "two_shot": 1 if t.n_padded * 4 > ONE_SHOT_MAX_BYTES else 0})
         self.ap = ap
         av = C.AllReduceParams()
@@ -328,12 +332,29 @@ class P2PBackend(CommBackend):
             av.update({"mc_local": mc_theta})
         self.nvls_step = self.nvls and t.n_padded * 4 > ONE_SHOT_MAX_BYTES
         self._connected = True
+        self._apply_lr_table()
         if self.gossip or self.table_mode:
             self._init_norms(run_fsm=self.gossip)
         boot.barrier()
 
     def _stream(self) -> int:
         return torch.cuda.current_stream(self.dev).cuda_stream
+
+    # ------------------------------------------------------------------ learning-rate schedule
+    def set_lr_table(self, table) -> None:
+        """Upload the per-step learning rates once; the step kernels index them with the device pass counter
+        (d_pass), so eager steps and every replay of a captured graph read the lr of their own step.  Call before
+        the first step (a graph captured earlier keeps the parameters it was captured with)."""
+        super().set_lr_table(table)
+        self.d_lr = None if self.lr_table is None else self.lr_table.to(self.dev)
+        if self._connected:
+            self._apply_lr_table()
+
+    def _apply_lr_table(self) -> None:
+        upd = {"lr_table": 0 if self.d_lr is None else self.d_lr.data_ptr(),
+               "lr_len": 0 if self.d_lr is None else int(self.d_lr.numel())}
+        self.gp.update(upd)
+        self.ap.update(upd)
 
     def _init_norms(self, run_fsm: bool) -> None:
         with torch.cuda.device(self.dev):

@@ -20,7 +20,6 @@ import torch
 import torch.distributed as dist
 
 from .collective import CollectiveBackend
-from .trigger import sgd_
 
 
 class ReferenceStyleBackend(CollectiveBackend):
@@ -99,7 +98,7 @@ class ReferenceStyleBackend(CollectiveBackend):
             _ = torch.linalg.vector_norm(il).item(), torch.linalg.vector_norm(ir).item()   # receive-side norms (:379,:423)
             self.host_syncs += 2
             flat.add_(il).add_(ir).div_(3)                         # event.cpp:459-461
-        sgd_(a.theta, a.grad, a.mom, cfg.lr, cfg.momentum)
+        self._opt()
 
     @torch.no_grad()
     def _step_decent(self) -> None:
@@ -110,7 +109,7 @@ class ReferenceStyleBackend(CollectiveBackend):
             self._send_recv_tensor(True, flat.clone(), il, ir)
             flat.add_(il).add_(ir).div_(3)
         self.bytes += 2 * t.n_elems * 4
-        sgd_(a.theta, a.grad, a.mom, cfg.lr, cfg.momentum)
+        self._opt()
 
     def _step_cent(self) -> None:
         a, t = self.arena, self.arena.table

@@ -95,14 +95,17 @@ def mix3_(theta: torch.Tensor, left: torch.Tensor, right: torch.Tensor) -> torch
 
 
 @torch.no_grad()
-def sgd_(theta: torch.Tensor, grad: torch.Tensor, mom, lr: float, mu: float) -> None:
-    """torch::optim::SGD step, dampening 0, no nesterov, no weight decay
-    (dcifar10/event/event.cpp:196-200; zero momentum buffer == first-step clone)."""
+def sgd_(theta: torch.Tensor, grad: torch.Tensor, mom, lr: float, mu: float, wd: float = 0.0,
+         nesterov: bool = False) -> None:
+    """torch.optim.SGD step with dampening 0 (dcifar10/event/event.cpp:196-200; zero momentum buffer ==
+    first-step clone), op for op as torch's single-tensor path, so the rounding is the same:
+        d = grad + wd*theta  (wd != 0) ;  m = mu*m + d ;  d = d + mu*m (nesterov) or m ;  theta -= lr*d
+    `grad` is not modified.  The reference uses wd = 0, nesterov = False (the defaults)."""
+    d = grad.add(theta, alpha=wd) if wd != 0.0 else grad
     if mu != 0.0:
-        mom.mul_(mu).add_(grad)
-        theta.add_(mom, alpha=-lr)
-    else:
-        theta.add_(grad, alpha=-lr)
+        mom.mul_(mu).add_(d)
+        d = d.add(mom, alpha=mu) if nesterov else mom
+    theta.add_(d, alpha=-lr)
 
 
 @torch.no_grad()
