@@ -71,6 +71,8 @@ class TrainConfig:
                                      # WAR ack (csrc/gossip_dbuf.cu).  None = on where it applies
     peer_timeout_s: float = 30.0     # bound of every device-side peer wait (sticky status instead of a hang);
                                      # EGB_PEER_TIMEOUT_S overrides
+    topology: str = "ring"           # gossip graph (parallel/topology.py): ring | exp (offsets 1,2,4,...) | "o1,o2,..."
+                                     # (circulant offsets, at most 4); decent/event only beyond the ring
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -129,29 +131,63 @@ class TrainConfig:
             raise ValueError(f"lr_milestones must be non-negative and strictly increasing, got {ms}")
         if not self.lr_warmup_epochs >= 0.0:
             raise ValueError("lr_warmup_epochs must be >= 0")
+        from .parallel.topology import check_topology_name
+        check_topology_name(self.topology)
+        if not self.ring_topology:
+            # a graph beyond the ring runs on the fused single-kernel step (csrc/gossip_graph.cu) and the
+            # torch.distributed backends; the split step, the double-buffered inbox, copy-engine pushes, spevent and the
+            # reference-structured backend exist for the ring only
+            if self.algo not in ("decent", "event"):
+                raise ValueError(f"topology {self.topology!r} needs algo decent or event, got {self.algo!r}")
+            if self.backend == "refport":
+                raise ValueError(f"topology {self.topology!r} is not supported by --backend refport (ring only)")
+            for name in ("overlap_push", "double_buffer", "ce_push"):
+                if getattr(self, name):
+                    raise ValueError(f"topology {self.topology!r} does not support {name} (ring only)")
+            if self.file_write:
+                raise ValueError(f"topology {self.topology!r} does not support file_write: the reference's log format "
+                                 "has exactly one left and one right receive column")
         return self
+
+    @property
+    def ring_topology(self) -> bool:
+        """True when `topology` names the ring (ring or the single offset 1).  The restrictions of validate() apply by
+        this name, independent of the world size; a name that resolves to the ring for the actual world (exp at
+        R <= 3) becomes "ring" in resolved() / for_world(), and then gets the ring's code path AND defaults."""
+        return str(self.topology).strip().lower() in ("ring", "1")
+
+    def for_world(self, world: int) -> "TrainConfig":
+        """This config with `topology` resolved for `world` ranks: a graph whose offsets are {1} is the ring (named
+        "ring", so the ring defaults -- double-buffered inbox, overlapped pushes -- apply).  Raises ValueError for
+        offsets out of range for `world`."""
+        if self.ring_topology:
+            return self
+        from .parallel.topology import parse_topology
+        return dataclasses.replace(self, topology="ring") if parse_topology(self.topology, world) == (1,) else self
 
     def resolved(self, device_type: str, world: int) -> "TrainConfig":
         """Fill the auto (None) execution switches for the device the job actually runs on: on a GPU the fast path
-        (NHWC + fused BN kernels, whole-step CUDA graph, pushes overlapped with backward) IS the default path."""
+        (NHWC + fused BN kernels, whole-step CUDA graph, pushes overlapped with backward) IS the default path.
+        The topology is resolved for `world` first (for_world): a graph that is the ring there gets the ring defaults."""
+        c = self.for_world(world)
         cuda = device_type == "cuda"
-        p2p = self.backend == "p2p" or (self.backend == "auto" and cuda)
+        p2p = c.backend == "p2p" or (c.backend == "auto" and cuda)
         kw = {}
-        conv_tc = self.conv_tc
+        conv_tc = c.conv_tc
         if conv_tc is None:
             import os
-            conv_tc = kw["conv_tc"] = bool(cuda and self.dtype == "fp32" and os.environ.get("EGB_CONV_TC", "1") != "0")
-        if self.channels_last is None:
+            conv_tc = kw["conv_tc"] = bool(cuda and c.dtype == "fp32" and os.environ.get("EGB_CONV_TC", "1") != "0")
+        if c.channels_last is None:
             # bf16 / tf32 / fp32 on our tensor-core convolutions: NHWC.  fp32 on cuDNN (conv_tc off): its IEEE-fp32
             # convolutions are NCHW kernels -- fed NHWC they transpose around every conv -- so that path stays NCHW;
             # the fused BN kernels exist for both layouts
-            kw["channels_last"] = cuda and (self.dtype != "fp32" or conv_tc)
-        if self.cuda_graph is None:
+            kw["channels_last"] = cuda and (c.dtype != "fp32" or conv_tc)
+        if c.cuda_graph is None:
             kw["cuda_graph"] = cuda
-        if self.overlap_push is None:
-            kw["overlap_push"] = bool(cuda and p2p and world >= 2 and self.algo in ("decent", "event")
-                                      and not bool(self.double_buffer))
-        return dataclasses.replace(self, **kw) if kw else self
+        if c.overlap_push is None:
+            kw["overlap_push"] = bool(cuda and p2p and world >= 2 and c.algo in ("decent", "event")
+                                      and not bool(c.double_buffer) and c.ring_topology)
+        return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
         return dataclasses.replace(self, **kw)
@@ -216,6 +252,8 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--double-buffer", action=argparse.BooleanOptionalAction, default=None)
     p.add_argument("--peer-timeout-s", type=float, default=None)
     p.add_argument("--ce-push", action="store_true", default=None)
+    p.add_argument("--topology", default=None, metavar="ring|exp|O1,O2,...",
+                   help="gossip graph: ring (default), exp (offsets 1,2,4,... up to R/2) or explicit circulant offsets")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

@@ -7,6 +7,7 @@
 
 #define EG_TILE 2048     // fp32 elements per tile == parallel/arena.py:TILE
 #define EG_THREADS 256
+#define EG_MAX_SLOTS 8   // inbox slots of a circulant gossip graph: 2 per offset, <= 4 offsets (parallel/topology.py)
 
 namespace egb {
 
@@ -108,6 +109,20 @@ struct GossipParams {
   int lr_len;
 };
 
+// Circulant gossip graph beyond the ring (csrc/gossip_graph.cu): the 2|O| inbox slots that replace the ring's
+// left/right pointers.  A separate block, passed to the graph kernel next to GossipParams, so the ring kernels'
+// parameters are untouched.  Slot s of this rank receives from peer Graph.slots()[s]; out-slot j pushes into slot j of
+// peer Graph.out_slots()[j] (parallel/topology.py).  mix: theta <- (((theta + in_0) + in_1) + ...) / (n_slots + 1)
+struct GraphSlots {
+  int n_slots;                          // 2|O|: even, 2..EG_MAX_SLOTS
+  const float* inbox[EG_MAX_SLOTS];     // local: what the sender of slot s last pushed
+  float* push[EG_MAX_SLOTS];            // peer-mapped: slot j's inbox of my j-th out peer
+  uint32_t* flag_from[EG_MAX_SLOTS];    // local [n_tiles * 8] (tile, warp), written by the sender of slot s
+  uint32_t* flag_to[EG_MAX_SLOTS];      // peer-mapped: flag_from[j] of my j-th out peer
+  uint32_t* ack_from[EG_MAX_SLOTS];     // local: my j-th out peer finished reading what I pushed at step k
+  uint32_t* ack_to[EG_MAX_SLOTS];       // peer-mapped: ack_from[s] of the sender of slot s
+};
+
 int gossip_max_grid(int device);  // co-resident CTAs (persistent grid upper bound)
 cudaError_t launch_gossip_step(const GossipParams& p, int grid, cudaStream_t s);
 // experimental double-buffered dense variant (csrc/gossip_dbuf.cu): inbox_l/inbox_r/push_l/push_r address
@@ -116,6 +131,10 @@ cudaError_t launch_gossip_step(const GossipParams& p, int grid, cudaStream_t s);
 cudaError_t launch_ce_push(const GossipParams& p, cudaStream_t s);
 int gossip_dbuf_max_grid(int device);
 cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_t s);
+// circulant-graph step (csrc/gossip_graph.cu): the fused single-kernel step over the slots of `g`; requires phase 0,
+// no sparse block, do_push and do_mix, and an even n_slots in [2, EG_MAX_SLOTS]
+int gossip_graph_max_grid(int device);
+cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g, int grid, cudaStream_t s);
 // (re)compute tile_ss (+ shadow) from theta and evaluate the trigger for step pass_num+1.
 cudaError_t launch_gossip_init(const GossipParams& p, int grid, int run_fsm, cudaStream_t s);
 // Trigger FSM alone with externally supplied norms (unit tests against the oracle).

@@ -9,6 +9,7 @@
 #include <stdexcept>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 #include <unordered_map>
 
@@ -33,6 +34,17 @@ using Setter = std::function<void(S&, py::object)>;
   { #sub "." #f, [](S& p, py::object v) { p.sub.f = reinterpret_cast<decltype(p.sub.f)>(v.cast<uintptr_t>()); } }
 #define NUMF2(S, sub, f) \
   { #sub "." #f, [](S& p, py::object v) { p.sub.f = v.cast<decltype(p.sub.f)>(); } }
+
+// pointer array of EG_MAX_SLOTS entries from a Python list (missing entries are null)
+#define ARRF(S, f)                                                                                       \
+  {                                                                                                      \
+    #f, [](S& p, py::object v) {                                                                         \
+      const auto l = v.cast<std::vector<uintptr_t>>();                                                   \
+      if (l.size() > EG_MAX_SLOTS) throw std::invalid_argument(#f ": more than EG_MAX_SLOTS entries");   \
+      for (size_t i = 0; i < EG_MAX_SLOTS; ++i)                                                          \
+        p.f[i] = reinterpret_cast<std::remove_reference_t<decltype(p.f[0])>>(i < l.size() ? l[i] : 0);   \
+    }                                                                                                    \
+  }
 
 #define TAB_FIELDS(S)                                                                              \
   PTRF2(S, tab, tile_tensor), PTRF2(S, tab, t_tile_start), PTRF2(S, tab, t_tile_count),            \
@@ -59,6 +71,11 @@ static const std::unordered_map<std::string, Setter<GossipParams>> kGossip = {
     NUMF2(GossipParams, fsm, log_cap), NUMF2(GossipParams, fsm, horizon), NUMF2(GossipParams, fsm, constant),
     NUMF2(GossipParams, fsm, thres_type), NUMF2(GossipParams, fsm, history),
     NUMF2(GossipParams, fsm, initial_comm_passes), NUMF2(GossipParams, fsm, enabled),
+};
+
+static const std::unordered_map<std::string, Setter<GraphSlots>> kGraph = {
+    NUMF(GraphSlots, n_slots), ARRF(GraphSlots, inbox), ARRF(GraphSlots, push), ARRF(GraphSlots, flag_from),
+    ARRF(GraphSlots, flag_to), ARRF(GraphSlots, ack_from), ARRF(GraphSlots, ack_to),
 };
 
 static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce = {
@@ -145,6 +162,7 @@ PYBIND11_MODULE(_C, m) {
   m.attr("TILE") = EG_TILE;
   m.attr("arch") = "sm_90a";
   bind_params<GossipParams>(m, "GossipParams", kGossip);
+  bind_params<GraphSlots>(m, "GraphSlots", kGraph);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
   bind_params<SparseParams>(m, "SparseParams", kSparse);
   bind_params<BnParams>(m, "BnParams", kBn);
@@ -161,6 +179,11 @@ PYBIND11_MODULE(_C, m) {
   m.def("gossip_dbuf_max_grid", &gossip_dbuf_max_grid);
   m.def("gossip_step_dbuf", [](const GossipParams& p, int grid, uintptr_t s) {
     check(launch_gossip_step_dbuf(p, grid, S(s)), "gossip_step_dbuf");
+  });
+  m.attr("MAX_SLOTS") = EG_MAX_SLOTS;
+  m.def("gossip_graph_max_grid", &gossip_graph_max_grid);
+  m.def("gossip_step_graph", [](const GossipParams& p, const GraphSlots& g, int grid, uintptr_t s) {
+    check(launch_gossip_step_graph(p, g, grid, S(s)), "gossip_step_graph");
   });
   m.def("gossip_init", [](const GossipParams& p, int grid, int run_fsm, uintptr_t s) {
     check(launch_gossip_init(p, grid, run_fsm, S(s)), "gossip_init");

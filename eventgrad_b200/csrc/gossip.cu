@@ -19,21 +19,47 @@
 //               in fixed order and runs the trigger FSM for the NEXT step (event.cpp:300-355),
 //               so the step needs no extra pass over theta, no grid sync and no host sync.
 //
-// This file is compiled twice.  As gossip.cu it is the default kernel described above.  csrc/gossip_dbuf.cu
+// This file is compiled three times.  As gossip.cu it is the default kernel described above.  csrc/gossip_dbuf.cu
 // defines EG_DBUF and includes it again to build the EXPERIMENTAL double-buffered dense variant
 // (`gossip_step_kernel_dbuf`, decent only): the inbox has two slots, slot = step & 1, and the WAR ack
 // (PROTOCOL.md 1.3) disappears -- a sender can be at most one step ahead of a receiver's reads because
 // finishing step k+1 needs the receiver's flags of step k+1 (model-checked: tests/test_protocol_model.py).
+// csrc/gossip_graph.cu defines EG_GRAPH and includes it a third time for circulant gossip graphs beyond the ring
+// (`gossip_step_kernel_graph`, decent/event, fused step only): the two neighbours become the 2|O| inbox slots of a
+// GraphSlots block that the graph kernel receives next to GossipParams (parallel/topology.py).  Each fired tile is
+// pushed into every out-slot, iter mode publishes and waits for one flag per slot per (tile, warp), the tail acks
+// every slot, and the mix adds the slots in slot order, two at a time, before one true division by 2|O|+1.
+// GossipParams is unchanged, so the ring kernels compile exactly as before.
 #include "api.h"
 #include "common.cuh"
 #include "sparse_apply.cuh"
 
-#ifdef EG_DBUF
+namespace egb {
+#ifdef EG_GRAPH
+struct GraphStepParams : GossipParams {   // kernel parameter of the graph build: the ring block + the slots
+  GraphSlots g;
+};
+using StepParams = GraphStepParams;
+#else
+using StepParams = GossipParams;
+#endif
+}  // namespace egb
+
+#if defined(EG_DBUF)
 #define EG_SYM(name) name##_dbuf
 #define EG_SLOT_OFF(p, step) ((size_t)((step) & 1) * ((size_t)(p).tab.n_tiles * EG_TILE))
+#elif defined(EG_GRAPH)
+#define EG_SYM(name) name##_graph
+#define EG_SLOT_OFF(p, step) ((size_t)0)
 #else
 #define EG_SYM(name) name
 #define EG_SLOT_OFF(p, step) ((size_t)0)
+#endif
+// messages one fired tensor costs: one per inbox slot it lands in (the reference's logical count)
+#ifdef EG_GRAPH
+#define EG_NMSG(p) ((unsigned long long)(p).g.n_slots)
+#else
+#define EG_NMSG(p) 2ull
 #endif
 
 namespace egb {
@@ -55,7 +81,7 @@ struct TileInfo {
 // -------------------------------------------------------------------------------------------
 __device__ __forceinline__ void fsm_update_tensor(const FsmDev& f, const TableDev& tab, int i, float norm,
                                                   float lnorm, float rnorm, bool have_recv, int next_step,
-                                                  bool count) {
+                                                  bool count, unsigned long long nmsg) {
   const int sz = tab.n_tensors;
   float* row_next = nullptr;   // log row of the decision (step next_step)
   float* row_cur = nullptr;    // log row of the step that just ran (receive-side norms)
@@ -69,9 +95,9 @@ __device__ __forceinline__ void fsm_update_tensor(const FsmDev& f, const TableDe
   }
   f.cur_norm[i] = norm;
   if (!f.enabled) return;
-  if (count && f.fire[i]) {   // +2 events per fired tensor, one per ring neighbour (event.cpp:319)
-    atomicAdd(f.counters + 0, 2ull);
-    atomicAdd(f.counters + 1, 2ull * (unsigned long long)tab.t_msg_bytes[i]);
+  if (count && f.fire[i]) {   // +2 events per fired tensor, one per ring neighbour (event.cpp:319); graph: one per slot
+    atomicAdd(f.counters + 0, nmsg);
+    atomicAdd(f.counters + 1, nmsg * (unsigned long long)tab.t_msg_bytes[i]);
     atomicAdd(f.counters + 2, 1ull);
   }
   const float value_diff = fabsf(__fsub_rn(norm, f.last_norm[i]));
@@ -128,7 +154,7 @@ __device__ __forceinline__ double reduce_partials(const float* part, int n4, int
 // completes a tensor reduces that tensor's per-warp partials in fixed order (one warp per tensor)
 // and runs the trigger FSM for it.  Tiles of a CTA ascend, so equal tensors are consecutive.
 #define EG_MAX_OWN 1024   // >= number of parameter tensors (asserted host-side)
-__device__ __forceinline__ void cta_finish_tensors(const GossipParams& p, const TileInfo* s_ti, int next_step,
+__device__ __forceinline__ void cta_finish_tensors(const StepParams& p, const TileInfo* s_ti, int next_step,
                                                    bool count, bool recv_ok) {
   __shared__ int s_own[EG_MAX_OWN];
   __shared__ int s_nown;
@@ -170,24 +196,35 @@ __device__ __forceinline__ void cta_finish_tensors(const GossipParams& p, const 
     }
     if (lane == 0) {
       p.tensor_done[i] = 0u;
-      fsm_update_tensor(p.fsm, p.tab, i, (float)sqrt(ss), (float)sqrt(sl), (float)sqrt(sr), recv, next_step, count);
+      fsm_update_tensor(p.fsm, p.tab, i, (float)sqrt(ss), (float)sqrt(sl), (float)sqrt(sr), recv, next_step, count,
+                        EG_NMSG(p));
     }
   }
 }
 
 // -------------------------------------------------------------------------------------------
-__device__ __forceinline__ void push_tile(const GossipParams& p, size_t base, const F8& th) {
+#ifdef EG_GRAPH
+// Slot loops run over EG_MAX_SLOTS with constant indices (unrolled, predicated on n_slots), so every slot pointer
+// is read straight from the kernel's parameter bank.
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th) {
+#pragma unroll
+  for (int k = 0; k < EG_MAX_SLOTS; ++k)
+    if (k < p.g.n_slots) st_f8(p.g.push[k] + base, th);
+}
+#else
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th) {
   // push_r == nullptr: 2-rank ring, the one neighbour is both left and right and reads the single copy twice
   st_f8(p.push_l + base, th);
   if (p.push_r != nullptr) st_f8(p.push_r + base, th);
 }
+#endif
 #ifdef EG_DBUF
-__device__ __forceinline__ void push_tile_slot(const GossipParams& p, size_t base, const F8& th, int step) {
+__device__ __forceinline__ void push_tile_slot(const StepParams& p, size_t base, const F8& th, int step) {
   push_tile(p, EG_SLOT_OFF(p, step) + base, th);
 }
 #endif
 
-__device__ __forceinline__ TileInfo resolve_tile(const GossipParams& p, int t) {
+__device__ __forceinline__ TileInfo resolve_tile(const StepParams& p, int t) {
   TileInfo ti;
   const int i = p.tab.tile_tensor[t];
   const int first = (t - p.tab.t_tile_start[i]) * EG_TILE;
@@ -203,7 +240,7 @@ __device__ __forceinline__ TileInfo resolve_tile(const GossipParams& p, int t) {
   return ti;
 }
 
-__device__ __forceinline__ void fill_tile_cache(const GossipParams& p, TileInfo* s_ti) {
+__device__ __forceinline__ void fill_tile_cache(const StepParams& p, TileInfo* s_ti) {
   const int j = threadIdx.x;
   if (j < EG_TI_CACHE) {
     const int t = blockIdx.x + j * gridDim.x;
@@ -211,14 +248,14 @@ __device__ __forceinline__ void fill_tile_cache(const GossipParams& p, TileInfo*
   }
   __syncthreads();
 }
-__device__ __forceinline__ TileInfo tile_info(const GossipParams& p, const TileInfo* s_ti, int j, int t) {
+__device__ __forceinline__ TileInfo tile_info(const StepParams& p, const TileInfo* s_ti, int j, int t) {
   return (j < EG_TI_CACHE) ? s_ti[j] : resolve_tile(p, t);
 }
 
 // Gradient of this thread's 8 elements.  Flat mode: the fp32 grad arena.  Table mode: autograd's
 // own gradient tensors are read in place (bf16 or fp32, exactly numel elements each) -- no
 // AccumulateGrad kernels, no grad arena traffic, no zeroing.
-__device__ __forceinline__ F8 load_grad(const GossipParams& p, const TileInfo& ti, size_t base, int tid) {
+__device__ __forceinline__ F8 load_grad(const StepParams& p, const TileInfo& ti, size_t base, int tid) {
   if (ti.gptr == nullptr) return ld_f8(p.grad + base);
   const int off = tid * EG_VEC;
   F8 g;
@@ -253,8 +290,30 @@ __device__ __forceinline__ F8 load_grad(const GossipParams& p, const TileInfo& t
 
 // mix + SGD + norm-on-write for one tile. `th` already holds theta_k for this thread's 8 floats.
 template <bool kMom>
-__device__ __forceinline__ void mix_tile(const GossipParams& p, int t, const TileInfo& ti, size_t base, F8 th,
+__device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileInfo& ti, size_t base, F8 th,
                                          int lane, int warp, int step) {
+#ifdef EG_GRAPH
+  // no receive-norm logging on graphs (file_write is ring only); slots are loaded two at a time after the gradient
+  // and momentum, which keeps the kernel at 64 registers whatever the degree
+  constexpr bool logrecv = false;
+  float ssl = 0.f, ssr = 0.f;
+  F8 m;
+  const F8 g = load_grad(p, ti, base, threadIdx.x);
+  if (kMom) m = ld_f8(p.mom + base);
+  if (p.do_mix) {
+#pragma unroll
+    for (int s = 0; s < EG_MAX_SLOTS; s += 2) {
+      if (s < p.g.n_slots) {
+        const F8 A = ld_f8_cg(p.g.inbox[s] + base), B = ld_f8_cg(p.g.inbox[s + 1] + base);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) th.v[e] = __fadd_rn(__fadd_rn(th.v[e], A.v[e]), B.v[e]);
+      }
+    }
+    const float k = (float)(p.g.n_slots + 1);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(th.v[e], k);
+  }
+#else
   const bool logrecv = (p.tile_ss_l != nullptr);
   float ssl = 0.f, ssr = 0.f;
   // issue every load of the tile before the first dependent FP op (5 x 32 B in flight per lane)
@@ -280,6 +339,7 @@ __device__ __forceinline__ void mix_tile(const GossipParams& p, int t, const Til
       }
     }
   }
+#endif
   // learning rate of this step, looked up per tile (an L1 hit) rather than held in a register across the loop
   const float lr = sched_lr(p.lr_table, p.lr_len, p.lr, step);
   float ss = 0.f;
@@ -314,7 +374,7 @@ __device__ __forceinline__ void mix_tile(const GossipParams& p, int t, const Til
 
 // Elect the last CTA of the grid; it acks and bumps the step counter (the trigger FSM itself is
 // run per tensor by whichever warp completes that tensor, see cta_finish_tensors).
-__device__ __forceinline__ void grid_tail(const GossipParams& p, int step) {
+__device__ __forceinline__ void grid_tail(const StepParams& p, int step) {
   __shared__ int s_last;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -327,7 +387,15 @@ __device__ __forceinline__ void grid_tail(const GossipParams& p, int step) {
   if (threadIdx.x == 0) {
     *p.ticket = 0u;
     *p.fsm.pass_num = step;
-#ifndef EG_DBUF
+#if defined(EG_GRAPH)
+    if (p.sync && p.send_ack) {
+      // every CTA of this rank has finished reading its inboxes for `step`: ack every slot's sender
+      fence_sys();
+#pragma unroll
+      for (int s = 0; s < EG_MAX_SLOTS; ++s)
+        if (s < p.g.n_slots) st_release_sys(p.g.ack_to[s], (uint32_t)step);
+    }
+#elif !defined(EG_DBUF)
     if (p.sync && p.send_ack) {
       // every CTA of this rank has finished reading its inboxes for `step`
       fence_sys();
@@ -341,7 +409,7 @@ __device__ __forceinline__ void grid_tail(const GossipParams& p, int step) {
 // phase 1 of the split step: push only.  Depends on theta_k and the trigger decisions alone, so
 // it is launched on a side stream at the START of step k and its NVLink traffic hides behind the
 // forward/backward pass.  Publishes ONE "all pushed" flag per neighbour when every CTA is done.
-__device__ __forceinline__ void push_phase(const GossipParams& p, int step) {
+__device__ __forceinline__ void push_phase(const StepParams& p, int step) {
   __shared__ int s_last;
   const int b = blockIdx.x, G = gridDim.x, tid = threadIdx.x;
   if (p.sync) {
@@ -378,7 +446,7 @@ __device__ __forceinline__ void push_phase(const GossipParams& p, int step) {
 }
 
 template <bool kMom>
-__global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(const GossipParams p) {
+__global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(const StepParams p) {
   const int b = blockIdx.x, G = gridDim.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int step = *p.fsm.pass_num + 1;
@@ -389,8 +457,10 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   // when it reads the status word.  (Uniform per CTA; the run is over, so a partial step does not matter.)
   if (p.do_push && *reinterpret_cast<volatile int*>(p.status) != EG_OK) return;
 
-#ifdef EG_DBUF
+#if defined(EG_DBUF)
   if (p.phase != 0 || !(p.sync && push)) return;   // the launcher rejects these; never reached
+#elif defined(EG_GRAPH)
+  if (p.phase != 0) return;                        // fused step only (the launcher rejects the rest)
 #else
   if (p.phase == 1) {
     push_phase(p, step);
@@ -399,7 +469,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #endif
   __shared__ TileInfo s_ti[EG_TI_CACHE];
   fill_tile_cache(p, s_ti);
-#ifndef EG_DBUF
+#if !defined(EG_DBUF) && !defined(EG_GRAPH)
   // spevent: receive side first -- scatter the records that arrived for this step into the replicas
   // (inbox_l / inbox_r point at them), grid barrier, then the dense mix below reads them tile by tile
   if (p.sparse != nullptr) sparse_apply_prologue(*p.sparse, p.sparse->bar);
@@ -433,7 +503,19 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
     // neighbours' flags of that slice (normally long set -- the ring is symmetric) and mixes it.
     // Warps never wait for each other, so flag latency and the sys-scope fence of one warp hide
     // behind the streaming of the other 31 warps on the SM.
-#ifndef EG_DBUF
+#if defined(EG_GRAPH)
+    __shared__ int s_ok;
+    if (tid == 0) {
+      // WAR guard: every peer I push into must have consumed what I pushed at step-1 before I overwrite it
+      bool ok = true;
+#pragma unroll
+      for (int k = 0; k < EG_MAX_SLOTS; ++k)
+        if (k < p.g.n_slots) ok = wait_ge(p.g.ack_from[k], (uint32_t)(step - 1), p.status, p.timeout_ns) && ok;
+      s_ok = ok;
+    }
+    __syncthreads();
+    if (!s_ok) return;
+#elif !defined(EG_DBUF)
     __shared__ int s_ok;
     if (tid == 0) {
       // WAR guard: neighbours must have consumed what I pushed at step-1 before I overwrite it
@@ -463,15 +545,28 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         __syncwarp();
         if (lane == 0) {
           if (fired) fence_sys();                  // my warp's stores are performed before the flag
+#ifdef EG_GRAPH
+#pragma unroll
+          for (int k = 0; k < EG_MAX_SLOTS; ++k)   // (k: out-slot; j is the tile loop's index)
+            if (k < p.g.n_slots) st_release_sys(p.g.flag_to[k] + (size_t)t * EG_WARPS + warp, (uint32_t)step);
+#else
           st_release_sys(p.flag_to_l + (size_t)t * EG_WARPS + warp, (uint32_t)step);
           st_release_sys(p.flag_to_r + (size_t)t * EG_WARPS + warp, (uint32_t)step);
+#endif
         }
       }
       const int t2 = b + (j - D) * G;
       if (j >= D && t2 < n_tiles) {
         if (lane == 0) {
+#ifdef EG_GRAPH
+#pragma unroll
+          for (int s = 0; s < EG_MAX_SLOTS; ++s)
+            if (s < p.g.n_slots)
+              wait_ge(p.g.flag_from[s] + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
+#else
           wait_ge(p.flag_from_l + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
           wait_ge(p.flag_from_r + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
+#endif
         }
         __syncwarp();
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
@@ -483,7 +578,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   grid_tail(p, step);
 }
 
-#ifndef EG_DBUF
+#if !defined(EG_DBUF) && !defined(EG_GRAPH)
 // (Re)compute tile partials (+ bf16 shadow) from theta; optionally evaluate the trigger for the
 // first step.  Used once at start-up and after theta is modified outside the step kernel
 // (checkpoint restore).
@@ -515,7 +610,7 @@ __global__ void __launch_bounds__(EG_THREADS) fsm_decide_kernel(const FsmDev f, 
                                                                const float* ext_norm) {
   const int next_step = *f.pass_num + 1;
   for (int i = threadIdx.x; i < t.n_tensors; i += EG_THREADS)
-    fsm_update_tensor(f, t, i, ext_norm[i], 0.f, 0.f, false, next_step, false);
+    fsm_update_tensor(f, t, i, ext_norm[i], 0.f, 0.f, false, next_step, false, 2ull);
   __syncthreads();
   if (threadIdx.x == 0) *f.pass_num += 1;
 }
@@ -550,6 +645,33 @@ cudaError_t launch_gossip_init(const GossipParams& p, int grid, int run_fsm, cud
 cudaError_t launch_fsm_decide(const FsmDev& f, const TableDev& t, const float* ext_norm, cudaStream_t s) {
   eg_count_launch(EG_FAM_GOSSIP, 1);
   fsm_decide_kernel<<<1, EG_THREADS, 0, s>>>(f, t, ext_norm);
+  return cudaGetLastError();
+}
+
+#elif defined(EG_GRAPH)   // only the step kernel + its launcher exist in this translation unit
+int gossip_graph_max_grid(int device) {
+  int sms = 0, a = 0, b = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_graph<true>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_graph<false>, EG_THREADS, 0);
+  if (b < a) a = b;
+  if (a < 1) a = 1;
+  return sms * a;
+}
+
+// Fused decent/event step on a circulant graph: iter-sync (flags + acks per slot) or async (single pass, no flags).
+cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g, int grid, cudaStream_t s) {
+  if (p.phase != 0 || p.sparse != nullptr || !p.do_push || !p.do_mix || g.n_slots < 2 || g.n_slots > EG_MAX_SLOTS ||
+      (g.n_slots & 1))
+    return cudaErrorInvalidValue;
+  GraphStepParams q;
+  static_cast<GossipParams&>(q) = p;
+  q.g = g;
+  eg_count_launch(EG_FAM_GOSSIP, 1);
+  if (p.mu != 0.f && p.mom != nullptr)
+    gossip_step_kernel_graph<true><<<grid, EG_THREADS, 0, s>>>(q);
+  else
+    gossip_step_kernel_graph<false><<<grid, EG_THREADS, 0, s>>>(q);
   return cudaGetLastError();
 }
 

@@ -12,7 +12,8 @@ from typing import List, Optional, Sequence
 import torch
 
 from ..parallel.arena import TensorTable
-from ..parallel.trigger import (TriggerConfig, TriggerState, mix3_, sgd_, topk_select,
+from ..parallel.topology import Graph
+from ..parallel.trigger import (TriggerConfig, TriggerState, mix3_, mixk_, sgd_, topk_select,
                                 trigger_step)
 from .lr_schedule import lr_at
 
@@ -21,10 +22,17 @@ class RingSimulator:
     def __init__(self, world: int, theta0: torch.Tensor, table: TensorTable, algo: str,
                  tcfg: Optional[TriggerConfig] = None, lr: float = 1e-2, momentum: float = 0.0,
                  topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
-                 weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None):
+                 weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
+                 offsets=(1,)):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
-        None = the constant `lr`."""
+        None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
+        resolved for `world`); the default (1,) is the ring."""
         assert algo in ("cent", "decent", "event", "spevent")
+        self.graphs = [Graph.build(r, world, offsets) for r in range(world)]
+        self.offsets = self.graphs[0].offsets
+        self.n_slots = self.graphs[0].n_slots
+        if self.offsets != (1,) and algo not in ("decent", "event"):
+            raise ValueError(f"offsets {self.offsets}: only decent and event gossip beyond the ring")
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -46,8 +54,11 @@ class RingSimulator:
             self.rep_l = [l0.clone() for _ in range(world)]
             self.rep_r = [r0.clone() for _ in range(world)]
         elif algo in ("decent", "event"):
-            self.inbox_l = [torch.zeros_like(theta0) for _ in range(world)]
-            self.inbox_r = [torch.zeros_like(theta0) for _ in range(world)]
+            # inbox[r][s]: what rank r last received in slot s (zero-initialised RMA window, event.cpp:144-147)
+            self.inbox = [[torch.zeros_like(theta0) for _ in range(self.n_slots)] for _ in range(world)]
+            if self.n_slots == 2:
+                self.inbox_l = [ib[0] for ib in self.inbox]       # ring: slot 0 = from left, slot 1 = from right
+                self.inbox_r = [ib[1] for ib in self.inbox]
 
     # ------------------------------------------------------------------
     def _flat(self, buf, i):
@@ -98,13 +109,14 @@ class RingSimulator:
                      for r in range(R)]
         self.fire_history.append([f.clone() for f in fires])
         snap = [th.clone() for th in self.theta]
+        n = self.n_slots
         for r in range(R):
             L, Rn = self.left(r), self.right(r)
             for i in range(t.n_tensors):
                 if not fires[r][i]:
                     continue
                 if self.algo != "decent":
-                    self.events[r] += 2
+                    self.events[r] += n
                 src = self._flat(snap[r], i)
                 if self.algo == "spevent":
                     pv = self._flat(self.prev[r], i)
@@ -114,15 +126,17 @@ class RingSimulator:
                     self._flat(self.rep_l[Rn], i)[ix] = v    # and my right neighbour's left
                     self.bytes[r] += 2 * 2 * self.k[i] * 4
                 else:
-                    self._flat(self.inbox_r[L], i).copy_(src)
-                    self._flat(self.inbox_l[Rn], i).copy_(src)
-                    self.bytes[r] += 2 * t.numels[i] * 4
+                    for p, j in self.graphs[r].out_slots():    # a fired tensor goes into every slot I feed
+                        self._flat(self.inbox[p][j], i).copy_(src)
+                    self.bytes[r] += n * t.numels[i] * 4
         # ---- phase 2: mix with whatever the inboxes hold, then SGD -----------------------
         for r in range(R):
             if self.algo == "spevent":
                 mix3_(self.theta[r], self.rep_l[r], self.rep_r[r])
+            elif n == 2:
+                mix3_(self.theta[r], self.inbox[r][0], self.inbox[r][1])
             else:
-                mix3_(self.theta[r], self.inbox_l[r], self.inbox_r[r])
+                mixk_(self.theta[r], self.inbox[r])
             self._sgd(r, grads[r])
 
     def final_average(self) -> torch.Tensor:
@@ -132,5 +146,9 @@ class RingSimulator:
         return int(sum(self.events))
 
     def dense_messages(self) -> int:
-        """Denominator of 'messages saved': 2 * sz * passes * R (BASELINE.md)."""
-        return 2 * self.table.n_tensors * self.pass_num * self.R
+        """Denominator of 'messages saved': 2|O| * sz * passes * R (BASELINE.md; 2 on the ring)."""
+        return self.n_slots * self.table.n_tensors * self.pass_num * self.R
+
+    def mixing_matrix(self) -> torch.Tensor:
+        """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD."""
+        return torch.tensor([g.mixing_row() for g in self.graphs], dtype=torch.float64)

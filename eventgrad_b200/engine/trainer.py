@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from ..config import TrainConfig
 from ..data import BatchLoader, ShardSampler, eval_batches, load_source, per_rank_batch
 from ..models import build_model
-from ..parallel import ParamArena, Ring, make_backend
+from ..parallel import Graph, ParamArena, Ring, make_backend
 from ..utils.ckpt import ckpt_path, load_checkpoint, save_checkpoint
 from ..utils.dist import DistEnv, barrier
 from ..utils.logfiles import RefLogWriter
@@ -41,7 +41,8 @@ class Trainer:
                  test_source=None):
         cfg = cfg.validate().resolved(env.device.type, env.world)
         self.cfg, self.env = cfg, env
-        self.ring = Ring(env.rank, env.world)
+        graph = Graph.build(env.rank, env.world, cfg.topology)    # ValueError: offsets out of range for this world
+        self.ring = Ring(env.rank, env.world) if graph.is_ring else graph
         dev = env.device
         self.device = dev
         if dev.type == "cuda":
@@ -326,7 +327,7 @@ class Trainer:
         res["events_total"] = self.backend.total_events() if gossip else 0
         if gossip and env.rank == 0 and not cfg.quiet:
             print(f"Total number of events - {res['events_total']}", flush=True)
-        dense = 2 * self.arena.table.n_tensors * self.backend.pass_num * env.world
+        dense = self.ring.n_slots * self.arena.table.n_tensors * self.backend.pass_num * env.world
         res["dense_messages"] = dense
         res["messages_saved"] = (1.0 - res["events_total"] / dense) if (gossip and dense) else 0.0
         if evaluate and env.rank == 0:

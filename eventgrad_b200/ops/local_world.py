@@ -18,14 +18,24 @@ import torch
 from ..config import TrainConfig
 from ..parallel.arena import ParamArena
 from ..parallel.p2p import P2PBackend, preallocate_arena_buffers
-from ..parallel.topology import Ring
+from ..parallel.topology import Graph, Ring
 from ..parallel.window import LocalBootstrap
 
 
 class LocalWorld:
     def __init__(self, cfg: TrainConfig, world: int, model_fn, device="cuda:0", grid_cap: int = 8,
-                 **backend_kw):
+                 topology=None, table_mode: bool = False, **backend_kw):
+        """`topology`: gossip graph name or offsets (default cfg.topology, parallel/topology.py).  `table_mode`: the
+        step kernel reads per-tensor gradient tensors in place (P2PBackend.update_grad_table) instead of the grad
+        arena; step() then hands each rank's flat gradient to the kernel as per-tensor views."""
+        if topology is not None:
+            if isinstance(topology, (tuple, list)):
+                topology = ",".join(str(int(o)) for o in topology)
+            cfg = cfg.replace(topology=str(topology)).validate()
+        cfg = cfg.for_world(world)          # a name that resolves to {1} is the ring, with the ring's defaults
+        topology = cfg.topology
         self.cfg, self.world = cfg, world
+        self.table_mode = table_mode
         self.device = torch.device(device)
         self.boot = LocalBootstrap(world)
         self.models, self.arenas, self.backends, self.streams = [], [], [], []
@@ -35,7 +45,10 @@ class LocalWorld:
             model = model_fn()
             theta, grad, symm = preallocate_arena_buffers(model, cfg, env, bootstrap=self.boot.for_rank(r))
             arena = ParamArena(model, self.device, theta=theta, grad=grad)
-            be = P2PBackend(cfg, arena, Ring(r, world), env, symm=symm, grid_cap=grid_cap,
+            if table_mode:
+                arena.enable_table_mode(shadow=False)
+            g = Graph.build(r, world, topology)
+            be = P2PBackend(cfg, arena, Ring(r, world) if g.is_ring else g, env, symm=symm, grid_cap=grid_cap,
                             defer_connect=True, **backend_kw)
             self.models.append(model)
             self.arenas.append(arena)
@@ -50,7 +63,13 @@ class LocalWorld:
         """One synchronous training step with externally supplied flat gradients."""
         cur = torch.cuda.current_stream(self.device)
         for r in range(self.world):
-            self.arenas[r].grad.copy_(grads[r])
+            if self.table_mode:
+                a = self.arenas[r]
+                for i, c in enumerate(a.compute):
+                    c.grad = a.flat(grads[r], i).reshape(c.shape).clone()
+                self.backends[r].update_grad_table(a.compute)
+            else:
+                self.arenas[r].grad.copy_(grads[r])
         for st in self.streams:
             st.wait_stream(cur)
         for r in range(self.world):

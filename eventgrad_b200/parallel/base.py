@@ -29,6 +29,18 @@ class StepLog:
     right_new: Optional[torch.Tensor] = None
 
 
+def check_topology_state(sd: Dict, ring, algo: str) -> None:
+    """Refuse to resume gossip state saved under a different graph: the inbox slots would mean other peers.  Ring
+    checkpoints carry no `topology_offsets` key (their format predates graphs)."""
+    if algo not in ("decent", "event"):
+        return
+    saved = tuple(sd.get("topology_offsets", (1,)))
+    now = tuple(getattr(ring, "offsets", (1,)))
+    if saved != now:
+        raise ValueError(f"checkpoint was written with topology offsets {saved}, this run uses {now}; "
+                         "resume with the same --topology")
+
+
 class CommBackend:
     name = "base"
 

@@ -24,8 +24,8 @@ from typing import List
 import torch
 import torch.distributed as dist
 
-from .base import CommBackend, StepLog
-from .trigger import TriggerConfig, TriggerState, mix3_, sgd_, topk_select, trigger_step
+from .base import CommBackend, StepLog, check_topology_state
+from .trigger import TriggerConfig, TriggerState, mix3_, mixk_, sgd_, topk_select, trigger_step
 
 
 class CollectiveBackend(CommBackend):
@@ -50,10 +50,13 @@ class CollectiveBackend(CommBackend):
                 self.rep_l = arena.theta.clone()
                 self.rep_r = arena.theta.clone()
                 self.k = t.topk_counts(cfg.topk_percent)
-            else:
+            elif getattr(ring, "is_ring", True):
                 # RMA window halves, zero-initialised (event.cpp:144-147)
                 self.inbox_l = torch.zeros_like(arena.theta)
                 self.inbox_r = torch.zeros_like(arena.theta)
+            else:
+                # circulant graph (parallel/topology.py): one zero-initialised inbox per slot
+                self.inbox = [torch.zeros_like(arena.theta) for _ in range(ring.n_slots)]
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
             self.last_recv_norm_l, self.last_recv_norm_r = z(), z()
@@ -98,6 +101,15 @@ class CollectiveBackend(CommBackend):
             for w in dist.batch_isend_irecv(ops):
                 w.wait()
 
+    def _exchange_slots(self, payload: torch.Tensor, recv: List[torch.Tensor]) -> None:
+        """Graph rendezvous: `payload` goes into every slot I feed (out-slot j = slot j of its peer), recv[s] receives
+        slot s.  The tag is the slot index, so two slots fed by the same peer (offset R/2) cannot cross."""
+        g = self.ring
+        ops = [dist.P2POp(dist.isend, payload, p, self.group, tag=j) for p, j in g.out_slots()]
+        ops += [dist.P2POp(dist.irecv, d, p, self.group, tag=s) for s, (p, d) in enumerate(zip(g.slots(), recv))]
+        for w in dist.batch_isend_irecv(ops):
+            w.wait()
+
     def _opt(self) -> None:
         a, cfg = self.arena, self.cfg
         sgd_(a.theta, a.grad, a.mom, self.step_lr(self.pass_num), cfg.momentum, cfg.weight_decay, cfg.nesterov)
@@ -128,6 +140,12 @@ class CollectiveBackend(CommBackend):
 
     def _step_decent(self) -> None:
         a = self.arena
+        if hasattr(self, "inbox"):
+            self._exchange_slots(a.theta, self.inbox)
+            self.bytes += len(self.inbox) * a.table.n_elems * 4
+            mixk_(a.theta, self.inbox)
+            self._opt()
+            return
         self._exchange([a.theta], [a.theta], [self.inbox_l], [self.inbox_r])
         self.bytes += 2 * a.table.n_elems * 4
         mix3_(a.theta, self.inbox_l, self.inbox_r)
@@ -147,7 +165,35 @@ class CollectiveBackend(CommBackend):
         self._exchange([m], [m], [ml], [mr])
         return fire.tolist(), ml.bool().tolist(), mr.bool().tolist()
 
+    def _step_event_graph(self) -> None:
+        """event on a circulant graph: fire masks per slot, then one payload of my fired tensors into every slot."""
+        a, t = self.arena, self.arena.table
+        n = len(self.inbox)
+        _, fire = self._fire()
+        m = fire.to(torch.uint8)
+        masks = [torch.empty_like(m) for _ in range(n)]
+        self._exchange_slots(m, masks)
+        mine = fire.tolist()
+        self.events += n * sum(mine)
+        sent = [self._flat(a.theta, i) for i in range(t.n_tensors) if mine[i]]
+        payload = torch.cat(sent) if sent else a.theta.new_empty(0)
+        self.bytes += n * payload.numel() * 4
+        masks = [mk.bool().tolist() for mk in masks]
+        bufs = [a.theta.new_empty(sum(t.numels[i] for i in range(t.n_tensors) if mk[i])) for mk in masks]
+        self._exchange_slots(payload, bufs)
+        for mask, buf, inbox in zip(masks, bufs, self.inbox):
+            off = 0
+            for i in range(t.n_tensors):
+                if mask[i]:
+                    k = t.numels[i]
+                    self._flat(inbox, i).copy_(buf[off:off + k])
+                    off += k
+        mixk_(a.theta, self.inbox)
+        self._opt()
+
     def _step_event(self) -> None:
+        if hasattr(self, "inbox"):
+            return self._step_event_graph()
         a, t = self.arena, self.arena.table
         thres_used = None
         if self.want_logs:
@@ -268,13 +314,21 @@ class CollectiveBackend(CommBackend):
         for k in ("inbox_l", "inbox_r", "prev", "rep_l", "rep_r"):
             if hasattr(self, k):
                 sd[k] = getattr(self, k).cpu().clone()
+        if hasattr(self, "inbox"):
+            sd["topology_offsets"] = list(self.ring.offsets)
+            for s, ib in enumerate(self.inbox):
+                sd[f"inbox_{s}"] = ib.cpu().clone()
         return sd
 
     def load_state_dict(self, sd):
         self.pass_num = int(sd["pass_num"])
         self.events = int(sd["events"])
         self.bytes = int(sd.get("bytes", 0))
+        check_topology_state(sd, self.ring, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
+        if hasattr(self, "inbox"):
+            for s, ib in enumerate(self.inbox):
+                ib.copy_(sd[f"inbox_{s}"].to(ib.device))
         for k in ("inbox_l", "inbox_r", "prev", "rep_l", "rep_r"):
             if hasattr(self, k) and k in sd:
                 getattr(self, k).copy_(sd[k].to(getattr(self, k).device))

@@ -3,6 +3,8 @@
 Per training step, after backward():
   cent     ONE launch: one-/two-shot all-reduce over peer-mapped gradients fused with 1/R and SGD
   decent   ONE launch: push theta to both ring neighbours -> flag handshake -> (t+L+R)/3 -> SGD
+           (circulant graph: push into all 2|O| slots I feed -> flags per slot -> (t+s_0+...)/(2|O|+1) -> SGD,
+           csrc/gossip_graph.cu)
   event    ONE launch: as decent, but a tensor is pushed only if its device-resident trigger fired;
            the same kernel accumulates the norms and runs the trigger FSM for the next step
   spevent  batched segmented radix-select top-k + compaction straight into the neighbours'
@@ -17,7 +19,8 @@ from typing import List
 import torch
 
 from .arena import TILE, ParamArena, TensorTable
-from .base import CommBackend, StepLog
+from .base import CommBackend, StepLog, check_topology_state
+from .topology import Graph
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
 
 ONE_SHOT_MAX_BYTES = 512 * 1024        # above this the all-reduce switches to two-shot
@@ -40,14 +43,30 @@ def _wants_dbuf(cfg) -> bool:
     only; there it is the default (double_buffer=None), `--no-double-buffer` selects the single-slot + ack protocol."""
     db = getattr(cfg, "double_buffer", None)
     return ((db is None or bool(db)) and cfg.algo == "decent" and cfg.sync_mode == "iter"
-            and not getattr(cfg, "overlap_push", False))
+            and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True))
 
 
-def build_layout(table: TensorTable, cfg, world: int, max_grid: int) -> Layout:
+def _graph_of(cfg, rank: int, world: int):
+    """The circulant graph of a non-ring topology, or None when the topology resolves to the ring."""
+    g = Graph.build(rank, world, getattr(cfg, "topology", "ring"))
+    return None if g.is_ring else g
+
+
+def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None) -> Layout:
     lay = Layout()
     n = table.n_padded * 4
     lay.add("theta", n)
     lay.add("grad", n)
+    nflag = (table.n_tiles * 8 + 64) * 4      # one flag per (tile, warp)
+    if graph is not None:
+        # circulant graph: one inbox, one flag block and one ack word per slot (csrc/gossip_graph.cu)
+        for k in range(graph.n_slots):
+            lay.add(f"inbox_{k}", n)
+        for k in range(graph.n_slots):
+            lay.add(f"flag_from_{k}", nflag)
+            lay.add(f"ack_from_{k}", 256)
+        lay.add("ar_flags", 3 * max_grid * world * 4)
+        return lay
     if cfg.algo in ("decent", "event"):
         slots = 2 if _wants_dbuf(cfg) else 1      # double-buffered decent: slot = step & 1
         lay.add("inbox_l", n * slots)
@@ -60,7 +79,6 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int) -> Layout:
         lay.add("seq_from_r", table.n_tensors * 4)
         lay.add("done_from_l", 256)
         lay.add("done_from_r", 256)
-    nflag = (table.n_tiles * 8 + 64) * 4      # one flag per (tile, warp)
     lay.add("flag_from_l", nflag)
     lay.add("flag_from_r", nflag)
     lay.add("ack_from_l", 256)
@@ -78,9 +96,12 @@ def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
     C = ext()
     table = _table_of(model)
     max_grid = C.gossip_max_grid(env.device.index or 0)
+    graph = _graph_of(cfg, env.rank, env.world) if cfg.algo in ("decent", "event") else None
     if _wants_dbuf(cfg):
         max_grid = min(max_grid, C.gossip_dbuf_max_grid(env.device.index or 0))
-    lay = build_layout(table, cfg, env.world, max_grid)
+    if graph is not None:
+        max_grid = min(max_grid, C.gossip_graph_max_grid(env.device.index or 0))
+    lay = build_layout(table, cfg, env.world, max_grid, graph)
     symm = wants_symm_window(env) and bootstrap is None      # NVLS path: torch symmetric memory + multicast mapping
     win = (SymmWindow if symm else Window)(lay, env.rank, env.world, env.device)
     theta = win.view("theta", torch.float32)
@@ -118,6 +139,11 @@ class P2PBackend(CommBackend):
         self.gossip = cfg.algo in ("decent", "event", "spevent")
         self.sparse = cfg.algo == "spevent"
         self.do_comm = self.comm_enabled and self.gossip
+        # circulant graph beyond the ring (parallel/topology.py): the fused single-kernel step of csrc/gossip_graph.cu
+        self.graph = None if getattr(ring, "is_ring", True) else ring
+        if self.graph is not None and (cfg.algo not in ("decent", "event") or getattr(cfg, "overlap_push", False)
+                                       or getattr(cfg, "ce_push", False) or self.want_logs):
+            raise ValueError("p2p backend: a non-ring topology runs decent/event on the fused step only")
         # split step: everything that depends only on theta_k (pushes / top-k records) is launched on a
         # side stream at the start of the step and overlaps forward+backward
         self.overlap = bool(getattr(cfg, "overlap_push", False)) and self.do_comm
@@ -191,7 +217,7 @@ class P2PBackend(CommBackend):
         self._grads_alive = None
         self.host_bytes = 0
         self._connected = False
-        self.gp = self.ap = self.ap_avg = self.sp = None
+        self.gp = self.ap = self.ap_avg = self.sp = self.gs = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
@@ -210,7 +236,7 @@ class P2PBackend(CommBackend):
             grids = boot.all_gather_object(self.grid)
         self.grid = int(min(grids))          # identical persistent grid on every rank
         boot.connect(win)
-        L, R = ring.left, ring.right
+        L, R = (ring.left, ring.right) if self.graph is None else (None, None)
         C, t, cfg = self.C, self.table, self.cfg
         a = self.arena
         P = lambda x: 0 if x is None else x.data_ptr()
@@ -237,12 +263,6 @@ class P2PBackend(CommBackend):
                 "sync": 1 if self.sync else 0,
                 "send_ack": 1 if dense else 0,
                 "zero_grad": 1, "group_iters": int(self.group_iters),
-                "flag_from_l": win.addr("flag_from_l"), "flag_from_r": win.addr("flag_from_r"),
-                "flag_to_l": win.addr("flag_from_r", L), "flag_to_r": win.addr("flag_from_l", R),
-                "ack_from_l": win.addr("ack_from_l"), "ack_from_r": win.addr("ack_from_r"),
-                "ack_to_l": win.addr("ack_from_r", L), "ack_to_r": win.addr("ack_from_l", R),
-                "pushed_from_l": win.addr("pushed_from_l"), "pushed_from_r": win.addr("pushed_from_r"),
-                "pushed_to_l": win.addr("pushed_from_r", L), "pushed_to_r": win.addr("pushed_from_l", R),
                 "phase": 0,
                 "fsm.thres": P(self.thres), "fsm.last_norm": P(self.last_norm),
                 "fsm.last_iter": P(self.last_iter), "fsm.slopes": P(self.slopes),
@@ -254,7 +274,32 @@ class P2PBackend(CommBackend):
                 "fsm.initial_comm_passes": int(cfg.initial_comm_passes),
                 "fsm.enabled": 1 if (cfg.algo in ("event", "spevent") and self.do_comm) else 0,
             })
-            if dense:
+            if self.graph is None:
+                gp.update({
+                    "flag_from_l": win.addr("flag_from_l"), "flag_from_r": win.addr("flag_from_r"),
+                    "flag_to_l": win.addr("flag_from_r", L), "flag_to_r": win.addr("flag_from_l", R),
+                    "ack_from_l": win.addr("ack_from_l"), "ack_from_r": win.addr("ack_from_r"),
+                    "ack_to_l": win.addr("ack_from_r", L), "ack_to_r": win.addr("ack_from_l", R),
+                    "pushed_from_l": win.addr("pushed_from_l"), "pushed_from_r": win.addr("pushed_from_r"),
+                    "pushed_to_l": win.addr("pushed_from_r", L), "pushed_to_r": win.addr("pushed_from_l", R),
+                })
+            else:
+                # slot s receives from g.slots()[s]; out-slot j writes slot j of its peer (inbox, flags) and the
+                # receiver acks slot s into its sender's ack word of the same index
+                g, n = self.graph, self.graph.n_slots
+                outs, ins = g.out_slots(), g.slots()
+                gs = C.GraphSlots()
+                gs.update({
+                    "n_slots": n,
+                    "inbox": [win.addr(f"inbox_{s}") for s in range(n)],
+                    "push": [win.addr(f"inbox_{k}", p) for p, k in outs],
+                    "flag_from": [win.addr(f"flag_from_{s}") for s in range(n)],
+                    "flag_to": [win.addr(f"flag_from_{k}", p) for p, k in outs],
+                    "ack_from": [win.addr(f"ack_from_{j}") for j in range(n)],
+                    "ack_to": [win.addr(f"ack_from_{s}", ins[s]) for s in range(n)],
+                })
+                self.gs = gs
+            if dense and self.graph is None:
                 gp.update({"inbox_l": win.addr("inbox_l"), "inbox_r": win.addr("inbox_r"),
                            "push_l": win.addr("inbox_r", L), "push_r": win.addr("inbox_l", R)})
                 # 2-rank ring: left == right.  Push theta ONCE (into the peer's inbox_r) and let the peer read that
@@ -436,6 +481,8 @@ class P2PBackend(CommBackend):
                 C.gossip_step_phase(self.gp, 2, self.grid, s)
             elif self.dbuf:
                 C.gossip_step_dbuf(self.gp, self.grid, s)
+            elif self.graph is not None and self.do_comm:
+                C.gossip_step_graph(self.gp, self.gs, self.grid, s)
             else:
                 C.gossip_step(self.gp, self.grid, s)
 
@@ -445,7 +492,7 @@ class P2PBackend(CommBackend):
         if self.cfg.algo == "cent" and self.ring.world > 1:
             self.host_bytes += self.table.n_elems * 4
         elif self.cfg.algo == "decent" and self.do_comm:
-            self.host_bytes += 2 * self.table.n_elems * 4
+            self.host_bytes += getattr(self.ring, "n_slots", 2) * self.table.n_elems * 4
 
     def step(self) -> None:
         if self.overlap:        # no compute to hide behind when called stand-alone: run both halves in order
@@ -516,7 +563,11 @@ class P2PBackend(CommBackend):
         sd = {"pass_num": self.pass_num, "host_bytes": self.host_bytes}
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
             sd[k] = getattr(self, k).cpu().clone()
-        if self.cfg.algo in ("decent", "event"):
+        if self.cfg.algo in ("decent", "event") and self.graph is not None:
+            sd["topology_offsets"] = list(self.graph.offsets)
+            for k in range(self.graph.n_slots):
+                sd[f"inbox_{k}"] = self.win.view(f"inbox_{k}", torch.float32).cpu().clone()
+        elif self.cfg.algo in ("decent", "event"):
             sd["inbox_l"] = self.win.view("inbox_l", torch.float32).cpu().clone()
             sd["inbox_r"] = self.win.view("inbox_r", torch.float32).cpu().clone()
         if self.sparse:
@@ -525,11 +576,15 @@ class P2PBackend(CommBackend):
         return sd
 
     def load_state_dict(self, sd):
+        check_topology_state(sd, self.ring, self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
             getattr(self, k).copy_(sd[k].to(self.dev))
-        if "inbox_l" in sd and self.cfg.algo in ("decent", "event"):
+        if self.graph is not None:
+            for k in range(self.graph.n_slots):
+                self.win.view(f"inbox_{k}", torch.float32).copy_(sd[f"inbox_{k}"].to(self.dev))
+        elif "inbox_l" in sd and self.cfg.algo in ("decent", "event"):
             self.win.view("inbox_l", torch.float32).copy_(sd["inbox_l"].to(self.dev))
             self.win.view("inbox_r", torch.float32).copy_(sd["inbox_r"].to(self.dev))
         if self.sparse:
@@ -544,6 +599,11 @@ class P2PBackend(CommBackend):
         torch.cuda.synchronize(self.dev)
 
     def _reset_handshake(self, step: int) -> None:
+        if self.graph is not None:
+            for k in range(self.graph.n_slots):
+                self.win.view(f"flag_from_{k}", torch.int32).fill_(step)
+                self.win.view(f"ack_from_{k}", torch.int32).fill_(step)
+            return
         for name in ("flag_from_l", "flag_from_r", "ack_from_l", "ack_from_r", "pushed_from_l", "pushed_from_r"):
             self.win.view(name, torch.int32).fill_(step)
         if self.sparse:

@@ -95,6 +95,15 @@ def mix3_(theta: torch.Tensor, left: torch.Tensor, right: torch.Tensor) -> torch
 
 
 @torch.no_grad()
+def mixk_(theta: torch.Tensor, slots) -> torch.Tensor:
+    """theta <- (((theta + s_0) + s_1) + ... + s_{n-1}) / (n+1): the circulant-graph mix (parallel/topology.py), one
+    rounded add per inbox slot in slot order, then a true division.  mixk_(theta, [L, R]) == mix3_(theta, L, R)."""
+    for s in slots:
+        theta.add_(s)
+    return theta.div_(len(slots) + 1)
+
+
+@torch.no_grad()
 def sgd_(theta: torch.Tensor, grad: torch.Tensor, mom, lr: float, mu: float, wd: float = 0.0,
          nesterov: bool = False) -> None:
     """torch.optim.SGD step with dampening 0 (dcifar10/event/event.cpp:196-200; zero momentum buffer ==

@@ -1,0 +1,159 @@
+"""Multi-process worker for circulant gossip graphs (parallel/topology.py) on a real process group.
+
+    torchrun --nproc-per-node R tests/topology_worker.py --mode sim --algo decent|event --topology exp|2 \
+        [--backend gloo|nccl|p2p]
+        every rank's parameters, event and byte counters equal the single-process simulator's bit for bit
+        (iter-sync; momentum, weight decay, Nesterov and a multistep lr schedule whose milestone falls in the run;
+        p2p: the simulator takes the kernel's own trigger decisions)
+    torchrun --nproc-per-node R tests/topology_worker.py --mode resume --topology exp --ckpt-dir DIR
+        a Trainer resumed from a mid-run checkpoint equals an uninterrupted run, and resuming it under the ring raises
+Used by tests/test_topology_cpu.py (gloo) and tests/test_gpu_topology.py (one process per GPU: nccl, p2p).
+"""
+import argparse
+import os
+import sys
+
+import torch
+import torch.distributed as dist
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from eventgrad_b200.config import TrainConfig, preset  # noqa: E402
+from eventgrad_b200.engine.lr_schedule import lr_table  # noqa: E402
+from eventgrad_b200.engine.simulator import RingSimulator  # noqa: E402
+from eventgrad_b200.models import build_model  # noqa: E402
+from eventgrad_b200.parallel import Graph, ParamArena, make_backend  # noqa: E402
+from eventgrad_b200.parallel.trigger import TriggerConfig  # noqa: E402
+from eventgrad_b200.utils.dist import init_distributed, shutdown  # noqa: E402
+
+STEPS_PER_EPOCH = 4
+
+
+def run_sim(a, env):
+    cfg = TrainConfig(algo=a.algo, dataset="mnist", model="cnn2", lr=0.05, momentum=0.9, weight_decay=5e-4,
+                      nesterov=True, lr_schedule="multistep", lr_milestones=(1,), lr_gamma=0.1,
+                      lr_warmup_epochs=0.5, epochs=3, horizon=1.0, thres_type=1, initial_comm_passes=4,
+                      backend=a.backend, sync_mode="iter", topology=a.topology).validate()
+    table = lr_table(cfg, STEPS_PER_EPOCH)
+    torch.manual_seed(0)
+    model = build_model(cfg.model)
+    graph = Graph.build(env.rank, env.world, cfg.topology)
+    assert not graph.is_ring, graph
+    if a.backend == "p2p":
+        from eventgrad_b200.parallel.p2p import P2PBackend, preallocate_arena_buffers
+        theta, grad, symm = preallocate_arena_buffers(model, cfg, env)
+        arena = ParamArena(model, env.device, theta=theta, grad=grad)
+        be = P2PBackend(cfg, arena, graph, env, symm=symm, timeout_ns=10_000_000_000)
+    else:
+        arena = ParamArena(model, env.device)
+        be = make_backend(cfg, arena, graph, env)
+    be.set_lr_table(table)
+    t = arena.table
+    theta0 = arena.theta.detach().cpu().clone()
+    mask = torch.zeros(t.n_padded)
+    for o, n in zip(t.offsets, t.numels):
+        mask[o:o + n] = 1
+
+    def grad_of(step, rank):
+        g = torch.Generator().manual_seed(step * 1000 + rank)
+        return torch.randn(t.n_padded, generator=g) * 0.05 * mask
+
+    fires = []
+    for s in range(a.steps):
+        if a.backend == "p2p" and a.algo == "event":
+            fires.append(be.fire.clone().bool().cpu())
+        arena.grad.copy_(grad_of(s, env.rank))
+        be.step()
+    if hasattr(be, "check_status"):
+        be.check_status()
+    W = env.world
+    allfires = [None] * W
+    dist.all_gather_object(allfires, fires)
+    mine = arena.theta.detach().clone()
+    allth = [torch.empty_like(mine) for _ in range(W)]
+    dist.all_gather(allth, mine)
+    cnt = torch.tensor([be.num_events(), be.bytes_sent()], dtype=torch.int64, device=mine.device)
+    allcnt = [torch.empty_like(cnt) for _ in range(W)]
+    dist.all_gather(allcnt, cnt)
+    ok = True
+    if env.rank == 0:
+        sim = RingSimulator(W, theta0, t, a.algo, TriggerConfig.from_train(cfg), lr=cfg.lr, momentum=cfg.momentum,
+                            serial_skip=False, weight_decay=cfg.weight_decay, nesterov=cfg.nesterov,
+                            lr_table=table, offsets=graph.offsets)
+        for s in range(a.steps):
+            sim.step([grad_of(s, r) for r in range(W)], fires=[allfires[r][s] for r in range(W)] if fires else None)
+        for r in range(W):
+            th = allth[r].cpu()
+            if not torch.equal(th, sim.theta[r]):
+                ok = False
+                print(f"MISMATCH rank {r}: max abs diff {(th - sim.theta[r]).abs().max().item():.3e}")
+            want_ev = sim.events[r] if a.algo == "event" else 0
+            if int(allcnt[r][0]) != want_ev or int(allcnt[r][1]) != sim.bytes[r]:
+                ok = False
+                print(f"COUNTERS rank {r}: {allcnt[r].tolist()} vs events {want_ev} bytes {sim.bytes[r]}")
+        if a.algo == "event" and sum(sim.events) == graph.n_slots * t.n_tensors * a.steps * W:
+            print("note: every tensor fired at every step")
+        print("WORKER_OK" if ok else "WORKER_FAIL",
+              f"mode=sim algo={a.algo} topology={a.topology} offsets={graph.offsets} world={W}", flush=True)
+    be.close()
+    return ok
+
+
+def run_resume(a, env):
+    from eventgrad_b200.data import synthetic_source
+    from eventgrad_b200.engine.trainer import Trainer
+    from eventgrad_b200.utils.ckpt import ckpt_path
+
+    def trainer(**kw):
+        base = dict(device="cpu", backend="gloo", model="cnn2", train_samples=128 * env.world, test_samples=64,
+                    batch_size=32, epochs=3, quiet=True, momentum=0.9, weight_decay=5e-4, nesterov=True,
+                    lr_schedule="multistep", lr_milestones=(2,), lr_gamma=0.1, topology=a.topology)
+        base.update(kw)
+        torch.manual_seed(0)
+        return Trainer(preset("mnist_event", **base), env,
+                       train_source=synthetic_source("mnist", 128 * env.world),
+                       test_source=synthetic_source("mnist", 64, train=False))
+
+    full = trainer()
+    full.fit()
+    th_full = full.arena.theta.clone()
+    ev_full = full.backend.num_events()
+    part = trainer(ckpt_dir=a.ckpt_dir, ckpt_every=1, max_steps=STEPS_PER_EPOCH)      # stops after epoch 1
+    part.fit()
+    assert part.epoch == 1 and part.backend.pass_num == STEPS_PER_EPOCH
+    res = trainer(resume=ckpt_path(a.ckpt_dir, env.rank))
+    assert res.backend.pass_num == STEPS_PER_EPOCH
+    res.fit()
+    ok = torch.equal(res.arena.theta, th_full) and res.backend.num_events() == ev_full
+    ok = ok and not torch.equal(part.arena.theta, th_full)
+    try:
+        trainer(resume=ckpt_path(a.ckpt_dir, env.rank), topology="ring")
+        ok = False
+        print(f"rank {env.rank}: resuming a graph checkpoint under the ring did not raise")
+    except ValueError as e:
+        ok = ok and "topology" in str(e)
+    flags = [None] * env.world
+    dist.all_gather_object(flags, ok)
+    if env.rank == 0:
+        print("WORKER_OK" if all(flags) else "WORKER_FAIL", f"mode=resume topology={a.topology} world={env.world}",
+              flush=True)
+    return all(flags)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--mode", default="sim", choices=["sim", "resume"])
+    ap.add_argument("--algo", default="event")
+    ap.add_argument("--topology", default="exp")
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--ckpt-dir", default="")
+    ap.add_argument("--backend", default="gloo", choices=["gloo", "nccl", "p2p"])
+    a = ap.parse_args()
+    env = init_distributed("cpu" if a.backend == "gloo" else "cuda")
+    ok = run_sim(a, env) if a.mode == "sim" else run_resume(a, env)
+    shutdown()
+    sys.exit(0 if ok else 1)
+
+
+if __name__ == "__main__":
+    main()
