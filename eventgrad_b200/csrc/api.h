@@ -266,6 +266,12 @@ struct BnParams {
   // the tensor-core convolutions (csrc/conv_tc.cu), so the consumer conv needs no separate split pass
   __nv_bfloat16* y_planes;    // forward: planes of y
   __nv_bfloat16* dx_planes;   // backward: planes of dx (= dY of the convolution that produced x)
+  // ReLU mask of the backward (split kernels; BN_MASK_* in bn_common.cuh): 0 = y > 0 read from p.y; 1 = recomputed
+  // from x as fmaf(x, sc, sh) > 0, bit for bit what the apply kernel decided (no residual only); 2 = the bit mask p.mask.
+  // p.mask [M*C/8]: bit e of byte (row*C + c)/8 is the mask of channel c+e (c a multiple of 8); the forward apply
+  // kernel writes it when non-null.  The backward skips the fp32 dx store when p.dx is null (planes only).
+  int mask_mode;
+  unsigned char* mask;
 };
 int bn_partial_rows(int sm_count);
 // fp32 NCHW variant (csrc/bn_nchw.cu): `hw` = H*W (multiple of 4), p.M = N*H*W.  Workspace: p.partial >= C*64*2
@@ -304,6 +310,11 @@ struct ConvTcParams {
   float* ws;                // fprop: workspace [ksplits][m_tiles*128][Cb] when ksplits > 1
   int ksplits;              // fprop: K-loop splits (conv_fprop_ksplits(); 1 = none)
   int bh, bn, m_tiles, k_blocks;   // filled in by the launchers
+  // fprop/dgrad, optional: out = acc + (mask bit ? addend : 0.f), addend [N][OH][OW][Cb] fp32 and addmask one bit per
+  // element in the BnParams::mask layout -- the skip-connection gradient of an identity block, added in the epilogue
+  // of its first convolution's data gradient
+  const float* addend;
+  const unsigned char* addmask;
 };
 bool conv_tc_supported(int N, int H, int W, int Ca, int Cb);
 int conv_wgrad_splits(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_count);

@@ -231,7 +231,7 @@ PYBIND11_MODULE(_C, m) {
                          uintptr_t invstd, uintptr_t run_mean, uintptr_t run_var, uintptr_t nbt, uintptr_t partial,
                          uintptr_t ticket, uintptr_t flag, uintptr_t epoch, uintptr_t status, long long M, int C,
                          float eps, float momentum, int relu, int training, int fused_ok, int sm_count, int fp32,
-                         int nchw_hw, uintptr_t s, uintptr_t y_planes) {
+                         int nchw_hw, uintptr_t s, uintptr_t y_planes, uintptr_t mask) {
     BnParams p;
     std::memset(&p, 0, sizeof(p));
     p.fp32 = fp32;
@@ -253,16 +253,20 @@ PYBIND11_MODULE(_C, m) {
     p.M = M; p.C = C; p.eps = eps; p.momentum = momentum; p.relu = relu; p.fused_ok = fused_ok;
     if (y_planes != 0 && (!fp32 || nchw_hw > 0)) throw std::invalid_argument("bn_forward: planes need the fp32 NHWC path");
     p.y_planes = reinterpret_cast<__nv_bfloat16*>(y_planes);
+    if (mask != 0 && (nchw_hw > 0 || !training)) throw std::invalid_argument("bn_forward: the bit mask needs the NHWC training path");
+    p.mask = reinterpret_cast<unsigned char*>(mask);
     if (nchw_hw > 0)
       check(launch_bn_nchw(p, nchw_hw, training ? 0 : 1, sm_count, S(s)), "bn_forward (nchw)");
     else
       check(launch_bn(p, training ? 0 : 1, sm_count, S(s)), "bn_forward");
   });
+  // mask_mode: BN_MASK_Y (read y) | BN_MASK_X (recompute from x, needs beta) | BN_MASK_BITS (read `mask`); dx may be 0
+  // when dx_planes is given
   m.def("bn_backward", [](uintptr_t x, uintptr_t y, uintptr_t dy, uintptr_t dx, uintptr_t dres, uintptr_t gamma,
                           uintptr_t mean, uintptr_t invstd, uintptr_t dgamma, uintptr_t dbeta, uintptr_t partial,
                           uintptr_t ticket, uintptr_t flag, uintptr_t epoch, uintptr_t status, long long M, int C,
                           int relu, int fused_ok, int sm_count, int fp32, int nchw_hw, uintptr_t s,
-                          uintptr_t dx_planes) {
+                          uintptr_t dx_planes, uintptr_t beta, int mask_mode, uintptr_t mask) {
     BnParams p;
     std::memset(&p, 0, sizeof(p));
     p.fp32 = fp32;
@@ -284,6 +288,12 @@ PYBIND11_MODULE(_C, m) {
     p.M = M; p.C = C; p.relu = relu; p.fused_ok = fused_ok;
     if (dx_planes != 0 && (!fp32 || nchw_hw > 0)) throw std::invalid_argument("bn_backward: planes need the fp32 NHWC path");
     p.dx_planes = reinterpret_cast<__nv_bfloat16*>(dx_planes);
+    p.beta = reinterpret_cast<const float*>(beta);
+    p.mask_mode = mask_mode;
+    p.mask = reinterpret_cast<unsigned char*>(mask);
+    if (mask_mode < 0 || mask_mode > 2 || (mask_mode == 1 && beta == 0) || (mask_mode == 2 && mask == 0) ||
+        (mask_mode != 0 && (nchw_hw > 0 || !fp32)) || (dx == 0 && dx_planes == 0))
+      throw std::invalid_argument("bn_backward: bad mask source / outputs");
     if (nchw_hw > 0)
       check(launch_bn_nchw(p, nchw_hw, 2, sm_count, S(s)), "bn_backward (nchw)");
     else
@@ -338,7 +348,8 @@ PYBIND11_MODULE(_C, m) {
   };
   m.def("conv_fprop", [fill](uintptr_t a, uintptr_t b, uintptr_t out, int N, int H, int W, int Ca, int Cb,
                              std::vector<std::tuple<int, int, int, int>> taps, int nsrc, int wtaps, int OH, int OW, int os,
-                             int op, int oq, int sm_count, uintptr_t s, uintptr_t ws, int ksplits) {
+                             int op, int oq, int sm_count, uintptr_t s, uintptr_t ws, int ksplits, uintptr_t addend,
+                             uintptr_t addmask) {
     ConvTcParams p{};
     p.a = reinterpret_cast<const __nv_bfloat16*>(a);
     p.b = reinterpret_cast<const __nv_bfloat16*>(b);
@@ -346,6 +357,9 @@ PYBIND11_MODULE(_C, m) {
     p.N = N; p.H = H; p.W = W; p.Ca = Ca; p.Cb = Cb; p.nsrc = nsrc; p.wtaps = wtaps;
     p.OH = OH; p.OW = OW; p.os = os; p.op = op; p.oq = oq;
     p.ws = reinterpret_cast<float*>(ws); p.ksplits = ksplits;
+    if ((addend == 0) != (addmask == 0)) throw std::invalid_argument("conv_fprop: addend and addmask go together");
+    p.addend = reinterpret_cast<const float*>(addend);
+    p.addmask = reinterpret_cast<const unsigned char*>(addmask);
     fill(p, taps);
     check(launch_conv_fprop(p, sm_count, S(s)), "conv_fprop");
   });

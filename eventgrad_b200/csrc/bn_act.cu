@@ -253,11 +253,7 @@ __global__ void __launch_bounds__(BN_THREADS, 3) bn_fwd_apply_kernel(const BnPar
   const size_t coff = (size_t)slice * BN_SLICE + tx * 8;
   float sc[8], sh[8];
 #pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const int c = slice * BN_SLICE + tx * 8 + e;
-    sc[e] = p.gamma[c] * p.invstd[c];
-    sh[e] = p.beta[c] - p.mean[c] * sc[e];
-  }
+  for (int e = 0; e < 8; ++e) bn_affine(p, slice * BN_SLICE + tx * 8 + e, sc[e], sh[e]);
   const long long stride = (long long)RS * BN_RPP;
   const bool has_res = pres != nullptr;
   for (long long row = (long long)rs * BN_RPP + ty; row < p.M; row += BN_APPLY_UNROLL(T) * stride) {
@@ -277,15 +273,18 @@ __global__ void __launch_bounds__(BN_THREADS, 3) bn_fwd_apply_kernel(const BnPar
       V8 x = unpack8(xr[u]);
       V8 r;
       if (has_res) r = unpack8(rr[u]);
+      unsigned m = 0u;
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         float v = fmaf(x.v[e], sc[e], sh[e]);
         if (has_res) v += r.v[e];
+        m |= (v > 0.f ? 1u : 0u) << e;
         x.v[e] = p.relu ? fmaxf(v, 0.f) : v;
       }
       Raw8<T> o;
       pack8(x, o);
       st8(py + r2 * p.C + coff, o);
+      if (p.mask != nullptr) p.mask[(r2 * p.C + coff) >> 3] = (unsigned char)m;
       if (p.y_planes != nullptr) store_planes8(x, p.y_planes + r2 * p.C + coff, (size_t)p.M * p.C);
     }
   }
@@ -298,34 +297,36 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_reduce_kernel(const BnPa
   const int slice = blockIdx.x, rs = blockIdx.y, RS = gridDim.y;   // slice fastest: CTAs scheduled together read adjacent 128 B of the same rows
   const int tx = threadIdx.x & 7, ty = threadIdx.x >> 3;
   const size_t coff = (size_t)slice * BN_SLICE + tx * 8;
-  float mu[8], is[8], s1[8], s2[8];
+  float mu[8], is[8], s1[8], s2[8], sc[8], sh[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     mu[e] = p.mean[slice * BN_SLICE + tx * 8 + e];
     is[e] = p.invstd[slice * BN_SLICE + tx * 8 + e];
     s1[e] = s2[e] = 0.f;
+    if (p.mask_mode == BN_MASK_X) bn_affine(p, slice * BN_SLICE + tx * 8 + e, sc[e], sh[e]);
   }
   const long long stride = (long long)RS * BN_RPP;
   for (long long row = (long long)rs * BN_RPP + ty; row < p.M; row += BN_RED_UNROLL(T) * stride) {
     Raw8<T> dr[BN_RED_UNROLL(T)], xr[BN_RED_UNROLL(T)], yr[BN_RED_UNROLL(T)];
+    unsigned char mb[BN_RED_UNROLL(T)];
 #pragma unroll
     for (int u = 0; u < BN_RED_UNROLL(T); ++u) {
       const long long r2 = row + u * stride;
       if (r2 < p.M) {
         dr[u] = ld8(pdy + r2 * p.C + coff);
         xr[u] = ld8(px + r2 * p.C + coff);
-        if (p.relu) yr[u] = ld8(py + r2 * p.C + coff);
+        if (p.relu && p.mask_mode == BN_MASK_Y) yr[u] = ld8(py + r2 * p.C + coff);
+        if (p.relu && p.mask_mode == BN_MASK_BITS) mb[u] = p.mask[(r2 * p.C + coff) >> 3];
       }
     }
 #pragma unroll
     for (int u = 0; u < BN_RED_UNROLL(T); ++u) {
       if (row + u * stride >= p.M) continue;
       const V8 d = unpack8(dr[u]), x = unpack8(xr[u]);
-      V8 y;
-      if (p.relu) y = unpack8(yr[u]);
+      const unsigned m = p.relu ? relu_bits<T>(p, yr[u], mb[u], x, sc, sh) : 0xffu;
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        const float dz = (p.relu && !(y.v[e] > 0.f)) ? 0.f : d.v[e];
+        const float dz = ((m >> e) & 1u) ? d.v[e] : 0.f;
         s1[e] += dz;
         s2[e] = fmaf(dz, (x.v[e] - mu[e]) * is[e], s2[e]);
       }
@@ -347,7 +348,7 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_dx_kernel(const BnParams
   const int slice = blockIdx.x, rs = blockIdx.y, RS = gridDim.y;   // slice fastest: CTAs scheduled together read adjacent 128 B of the same rows
   const int tx = threadIdx.x & 7, ty = threadIdx.x >> 3;
   const size_t coff = (size_t)slice * BN_SLICE + tx * 8;
-  float mu[8], is[8], k0[8], k1[8], k2[8];
+  float mu[8], is[8], k0[8], k1[8], k2[8], sc[8], sh[8];
   const float invM = 1.f / (float)p.M;
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
@@ -357,35 +358,38 @@ __global__ void __launch_bounds__(BN_THREADS, 2) bn_bwd_dx_kernel(const BnParams
     k0[e] = p.gamma[c] * is[e];              // dx = k0*(dz - k1 - xhat*k2)
     k1[e] = p.dbeta[c] * invM;
     k2[e] = p.dgamma[c] * invM;
+    if (p.mask_mode == BN_MASK_X) bn_affine(p, c, sc[e], sh[e]);
   }
   const long long stride = (long long)RS * BN_RPP;
   const bool want_dres = pdres != nullptr;
   for (long long row = (long long)rs * BN_RPP + ty; row < p.M; row += BN_DX_UNROLL(T) * stride) {
     Raw8<T> dr[BN_DX_UNROLL(T)], xr[BN_DX_UNROLL(T)], yr[BN_DX_UNROLL(T)];
+    unsigned char mb[BN_DX_UNROLL(T)];
 #pragma unroll
     for (int u = 0; u < BN_DX_UNROLL(T); ++u) {
       const long long r2 = row + u * stride;
       if (r2 < p.M) {
         dr[u] = ld8(pdy + r2 * p.C + coff);
         xr[u] = ld8(px + r2 * p.C + coff);
-        if (p.relu) yr[u] = ld8(py + r2 * p.C + coff);
+        if (p.relu && p.mask_mode == BN_MASK_Y) yr[u] = ld8(py + r2 * p.C + coff);
+        if (p.relu && p.mask_mode == BN_MASK_BITS) mb[u] = p.mask[(r2 * p.C + coff) >> 3];
       }
     }
 #pragma unroll
     for (int u = 0; u < BN_DX_UNROLL(T); ++u) {
       const long long r2 = row + u * stride;
       if (r2 >= p.M) continue;
-      V8 d = unpack8(dr[u]), x = unpack8(xr[u]), y;
-      if (p.relu) y = unpack8(yr[u]);
+      V8 d = unpack8(dr[u]), x = unpack8(xr[u]);
+      const unsigned m = p.relu ? relu_bits<T>(p, yr[u], mb[u], x, sc, sh) : 0xffu;
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        const float dz = (p.relu && !(y.v[e] > 0.f)) ? 0.f : d.v[e];
+        const float dz = ((m >> e) & 1u) ? d.v[e] : 0.f;
         d.v[e] = dz;
         x.v[e] = k0[e] * (dz - k1[e] - (x.v[e] - mu[e]) * is[e] * k2[e]);
       }
       Raw8<T> o;
       pack8(x, o);
-      st8(pdx + r2 * p.C + coff, o);
+      if (pdx != nullptr) st8(pdx + r2 * p.C + coff, o);
       if (p.dx_planes != nullptr) store_planes8(x, p.dx_planes + r2 * p.C + coff, (size_t)p.M * p.C);
       if (want_dres) {
         pack8(d, o);
@@ -424,7 +428,7 @@ static cudaError_t launch_bn_t(const BnParams& p, int which, int sm_count, cudaS
   };
   if (which == 0) {
     const long long rs_f = ceil_div(passes, BN_FWD_PASSES);
-    if (p.fused_ok && p.y_planes == nullptr && rs_f * slices <= max_ctas) {
+    if (p.fused_ok && p.y_planes == nullptr && p.mask == nullptr && rs_f * slices <= max_ctas) {
       eg_count_launch(EG_FAM_BN, 1);
       bn_fwd_fused_kernel<T><<<dim3((unsigned)slices, (unsigned)rs_f), BN_THREADS, 0, s>>>(p);
     } else {
@@ -437,7 +441,7 @@ static cudaError_t launch_bn_t(const BnParams& p, int which, int sm_count, cudaS
     bn_fwd_apply_kernel<T><<<map_grid(BN_APPLY_UNROLL(T)), BN_THREADS, 0, s>>>(p);
   } else if (which == 2) {
     const long long rs_b = ceil_div(passes, BN_BWD_PASSES);
-    if (p.fused_ok && p.dx_planes == nullptr && rs_b * slices <= max_ctas) {
+    if (p.fused_ok && p.dx_planes == nullptr && p.mask_mode == BN_MASK_Y && rs_b * slices <= max_ctas) {
       eg_count_launch(EG_FAM_BN, 1);
       bn_bwd_fused_kernel<T><<<dim3((unsigned)slices, (unsigned)rs_b), BN_THREADS, 0, s>>>(p);
     } else {

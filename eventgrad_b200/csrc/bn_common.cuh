@@ -105,6 +105,35 @@ __device__ __forceinline__ void mask_le0(Raw8<float>& d, const Raw8<float>& y) {
   if (!(y.b.w > 0.f)) d.b.w = 0.f;
 }
 
+// ReLU mask sources of the split backward kernels (BnParams::mask_mode)
+#define BN_MASK_Y 0
+#define BN_MASK_X 1
+#define BN_MASK_BITS 2
+
+// y = fmaf(x, sc, sh) (+ residual): the forward apply kernel and the "mask from x" backward share this expression, so
+// the backward's fmaf(x, sc, sh) > 0 is bit for bit the forward's decision
+__device__ __forceinline__ void bn_affine(const BnParams& p, int c, float& sc, float& sh) {
+  sc = p.gamma[c] * p.invstd[c];
+  sh = p.beta[c] - p.mean[c] * sc;
+}
+
+// ReLU mask of 8 channels as bits (bit e = channel e), from whichever source p.mask_mode names
+template <typename T>
+__device__ __forceinline__ unsigned relu_bits(const BnParams& p, const Raw8<T>& yr, unsigned char mb, const V8& x,
+                                              const float (&sc)[8], const float (&sh)[8]) {
+  if (p.mask_mode == BN_MASK_BITS) return mb;
+  unsigned m = 0u;
+  if (p.mask_mode == BN_MASK_X) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m |= (fmaf(x.v[e], sc[e], sh[e]) > 0.f ? 1u : 0u) << e;
+  } else {
+    const V8 y = unpack8(yr);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m |= (y.v[e] > 0.f ? 1u : 0u) << e;
+  }
+  return m;
+}
+
 // -------------------------------------------------------------------------------------------
 // Reduce the per-thread 2x8 accumulators over the 32 row lanes, write this CTA's partial row
 // [128] = {sum a[64] | sum b[64]} for its slice.

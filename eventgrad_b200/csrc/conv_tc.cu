@@ -139,7 +139,9 @@ __device__ __forceinline__ void six_term_kblock(float (&acc)[NT / 2], float (&d)
 }
 
 // ------------------------------------------------------------------------------------------------ forward / dgrad
-template <int NT, int STAGES>
+// ADD: the epilogue adds the masked skip-connection gradient (p.addend / p.addmask); only launched un-split.  A separate
+// instantiation, so that the k-loop of the plain kernel is compiled exactly as without the option.
+template <int NT, int STAGES, bool ADD>
 __global__ void __launch_bounds__(CV_THREADS, 1)
 conv3x3_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const ConvTcParams p) {
@@ -237,6 +239,31 @@ conv3x3_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
           continue;
         }
         dst += 2 * (lane & 3);
+        if constexpr (ADD) {                                   // skip-connection gradient: + (mask ? addend : 0.f)
+          // Every load of the row segment is issued before the first store, so the thread waits out one load latency
+          // per row instead of one per 8 channels.  Column j's 2 channels sit in mask byte (off >> 3) + j: the NT/8
+          // bytes are consecutive and NT/8-aligned (Cb and nt*NT are multiples of NT), one vector load.
+          const size_t off = (size_t)(dst - p.out);
+          const float* __restrict__ src = p.addend + off;
+          uint32_t mw[NT / 32];
+          if constexpr (NT == 128) {
+            const uint4 v = __ldg(reinterpret_cast<const uint4*>(p.addmask + (off >> 3)));
+            mw[0] = v.x; mw[1] = v.y; mw[2] = v.z; mw[3] = v.w;
+          } else {
+            const uint2 v = __ldg(reinterpret_cast<const uint2*>(p.addmask + (off >> 3)));
+            mw[0] = v.x; mw[1] = v.y;
+          }
+          float2 a[NT / 8];
+#pragma unroll
+          for (int j = 0; j < NT / 8; ++j) a[j] = __ldg(reinterpret_cast<const float2*>(src + 8 * j));
+#pragma unroll
+          for (int j = 0; j < NT / 8; ++j) {
+            const unsigned m = (mw[j >> 2] >> (8 * (j & 3) + 2 * (lane & 3))) & 3u;
+            *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h] + ((m & 1u) ? a[j].x : 0.f),
+                                                                  acc[4 * j + 2 * h + 1] + ((m & 2u) ? a[j].y : 0.f));
+          }
+          continue;
+        }
 #pragma unroll
         for (int j = 0; j < NT / 8; ++j)
           *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
@@ -264,6 +291,15 @@ __global__ void __launch_bounds__(256) conv_fprop_reduce_kernel(const ConvTcPara
       const int n = (int)(row / hw), rem = (int)(row - (long long)n * hw);
       const int ii = rem / p.W, j = rem - ii * p.W;
       opix = ((long long)n * p.OH + ii * p.os + p.op) * p.OW + j * p.os + p.oq;
+    }
+    if (p.addend != nullptr) {                                 // skip-connection gradient, as in the un-split epilogue
+      const size_t off = (size_t)opix * p.Cb + 4 * c4;
+      const float4 v = __ldg(reinterpret_cast<const float4*>(p.addend + off));
+      const unsigned m = (unsigned)p.addmask[off >> 3] >> (off & 7);
+      a.x += (m & 1u) ? v.x : 0.f;
+      a.y += (m & 2u) ? v.y : 0.f;
+      a.z += (m & 4u) ? v.z : 0.f;
+      a.w += (m & 8u) ? v.w : 0.f;
     }
     reinterpret_cast<float4*>(p.out + (size_t)opix * p.Cb)[c4] = a;
   }
@@ -622,13 +658,13 @@ int conv_fprop_ntile(int N, int H, int W, int Ca, int Cb, int ntaps, int sm_coun
   return 2 * waves128 <= waves64 ? 128 : 64;
 }
 
-template <int NT, int STAGES>
+template <int NT, int STAGES, bool ADD>
 static cudaError_t fprop_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvTcParams& p, int grid,
                                 cudaStream_t s) {
   const size_t smem = (size_t)STAGES * (3 * CV_APLANE + 3 * NT * 128) + 256 + 1024;
-  cudaError_t e = cudaFuncSetAttribute(conv3x3_fprop_kernel<NT, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e = cudaFuncSetAttribute(conv3x3_fprop_kernel<NT, STAGES, ADD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  conv3x3_fprop_kernel<NT, STAGES><<<grid, CV_THREADS, smem, s>>>(tmA, tmB, p);
+  conv3x3_fprop_kernel<NT, STAGES, ADD><<<grid, CV_THREADS, smem, s>>>(tmA, tmB, p);
   return cudaGetLastError();
 }
 
@@ -651,8 +687,12 @@ cudaError_t launch_conv_fprop(const ConvTcParams& p0, int sm_count, cudaStream_t
   const int grid = total < sm_count ? total : sm_count;
   if (!make_map_act(&tmA, p.a, p.Ca, p.W, p.H, p.N, 3 * p.nsrc, p.W, p.bh, p.bn)) return cudaErrorNotSupported;
   eg_count_launch(EG_FAM_CONV, p.ksplits > 1 ? 2 : 1);
-  cudaError_t e = NT == 128 ? fprop_launch<128, CV_STAGES(128)>(tmA, tmB, p, grid, s)
-                            : fprop_launch<64, CV_STAGES(64)>(tmA, tmB, p, grid, s);
+  if ((p.addend == nullptr) != (p.addmask == nullptr)) return cudaErrorInvalidValue;
+  const bool add = p.addend != nullptr && p.ksplits == 1;   // K-split: the reduce kernel adds it
+  cudaError_t e = NT == 128 ? (add ? fprop_launch<128, CV_STAGES(128), true>(tmA, tmB, p, grid, s)
+                                   : fprop_launch<128, CV_STAGES(128), false>(tmA, tmB, p, grid, s))
+                            : (add ? fprop_launch<64, CV_STAGES(64), true>(tmA, tmB, p, grid, s)
+                                   : fprop_launch<64, CV_STAGES(64), false>(tmA, tmB, p, grid, s));
   if (e != cudaSuccess || p.ksplits == 1) return e;
   const long long n4 = (long long)p.N * p.H * p.W * (p.Cb / 4);
   long long blocks = (n4 + 255) / 256;

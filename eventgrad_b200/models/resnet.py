@@ -10,7 +10,8 @@ Reference: /root/reference/dcifar10/common/resnet.hpp
     shapes); `variant="canonical"` builds the textbook blocks-per-stage network
     (62 tensors / 11 173 962 elements for ResNet-18).
 BatchNorm layers are ops.bn_act.FusedBNAct (nn.BatchNorm2d subclass: same names/buffers) so that
-bn->relu and bn->(+=skip)->relu run as fused sm_90a kernels on bf16 NHWC activations.
+bn->relu and bn->(+=skip)->relu run as fused sm_90a kernels on NHWC activations; in fp32 training each conv+bn pair
+runs as one autograd node (ops/conv_bn.py).
 Parameter registration order matches LibTorch's named_parameters() walk
 (conv, bn, layer1..4 [conv1,bn1,conv2,bn2,(conv3,bn3),downsampler], fc) because the
 arena layout (= the reference's running `disp`) is defined by that order.
@@ -24,6 +25,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.bn_act import FusedBNAct
+from ..ops.conv_bn import SkipGrad, conv_bn
 from ..ops.shadow import ShadowConv2d, ShadowLinear
 
 
@@ -43,9 +45,10 @@ class BasicBlock(nn.Module):
         self.downsampler = downsample
 
     def forward(self, x):
-        out = self.bn1(self.conv1(x), relu=True)
+        skip = SkipGrad() if self.downsampler is None else None      # identity block: bn2 hands x's gradient to conv1
+        out = conv_bn(self.conv1, self.bn1, x, relu=True, skip_in=skip)
         residual = self.downsampler(x) if self.downsampler is not None else x
-        return self.bn2(self.conv2(out), residual=residual, relu=True)      # bn -> += skip -> relu, fused
+        return conv_bn(self.conv2, self.bn2, out, residual=residual, relu=True, skip_out=skip)   # bn -> += skip -> relu
 
 
 class BottleNeck(nn.Module):
@@ -62,10 +65,11 @@ class BottleNeck(nn.Module):
         self.downsampler = downsample
 
     def forward(self, x):
-        out = self.bn1(self.conv1(x), relu=True)
-        out = self.bn2(self.conv2(out), relu=True)
+        skip = SkipGrad() if self.downsampler is None else None      # identity block: bn3 hands x's gradient to conv1
+        out = conv_bn(self.conv1, self.bn1, x, relu=True, skip_in=skip)
+        out = conv_bn(self.conv2, self.bn2, out, relu=True)
         residual = self.downsampler(x) if self.downsampler is not None else x
-        return self.bn3(self.conv3(out), residual=residual, relu=True)
+        return conv_bn(self.conv3, self.bn3, out, residual=residual, relu=True, skip_out=skip)
 
 
 class ResNet(nn.Module):
@@ -116,7 +120,7 @@ class ResNet(nn.Module):
         return nn.Sequential(*mods)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        out = self.bn(self.conv(x), relu=True)
+        out = conv_bn(self.conv, self.bn, x, relu=True)
         out = self.layer4(self.layer3(self.layer2(self.layer1(out))))
         out = F.avg_pool2d(out, 4)
         out = out.reshape(out.shape[0], -1)

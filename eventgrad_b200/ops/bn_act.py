@@ -73,38 +73,76 @@ def _eligible(x: torch.Tensor, residual: Optional[torch.Tensor]) -> bool:
     return True
 
 
+# ReLU mask source of the backward (csrc/bn_common.cuh BN_MASK_*): the saved output y, recomputed from the BN input x
+# (no residual: y > 0 <=> fmaf(x, sc, sh) > 0), or the bit mask the forward wrote
+MASK_Y, MASK_X, MASK_BITS = 0, 1, 2
+
+
+def bn_forward(x, weight, bias, running_mean, running_var, nbt, residual, training, momentum, eps, relu,
+               y_planes=None, mask=None):
+    """Launch the forward kernels -> (y, mean, invstd, nchw_hw).  y_planes / mask (uint8 [numel/8]): optional extra
+    outputs of the fp32 NHWC path (bf16 planes of y; the ReLU mask as bits)."""
+    ws = _workspace(x.device)
+    C_ext = ws["C"]
+    N, C, H, W = x.shape
+    M = N * H * W
+    y = torch.empty_like(x)                       # preserves channels_last
+    if training:
+        mean = torch.empty(C, dtype=torch.float32, device=x.device)
+        invstd = torch.empty(C, dtype=torch.float32, device=x.device)
+        rm = running_mean.data_ptr() if running_mean is not None else 0
+        rv = running_var.data_ptr() if running_var is not None else 0
+        nb = nbt.data_ptr() if nbt is not None else 0
+    else:
+        mean = running_mean
+        invstd = torch.rsqrt(running_var + eps)
+        rm = rv = nb = 0
+    stream = torch.cuda.current_stream(x.device).cuda_stream
+    nchw = not _eligible(x, residual)              # caller guarantees one of the two layouts is eligible
+    nchw_hw = H * W if nchw else 0
+    with torch.cuda.device(x.device):
+        C_ext.bn_forward(x.data_ptr(), residual.data_ptr() if residual is not None else 0, y.data_ptr(),
+                         weight.data_ptr(), bias.data_ptr(), mean.data_ptr(), invstd.data_ptr(), rm, rv, nb,
+                         (ws["nchw_partial"] if nchw else ws["partial"]).data_ptr(),
+                         ws["nchw_ticket"].data_ptr() if nchw else ws["f"][0], ws["f"][1], ws["f"][2],
+                         ws["status"], M, C,
+                         float(eps), float(momentum), 1 if relu else 0, 1 if training else 0, ws["fused"],
+                         ws["sm"], 1 if x.dtype == torch.float32 else 0, nchw_hw, stream,
+                         y_planes.data_ptr() if (y_planes is not None and not nchw) else 0,
+                         0 if mask is None else mask.data_ptr())
+    return y, mean, invstd, nchw_hw
+
+
+def bn_backward(x, y, dy, weight, bias, mean, invstd, relu, nchw_hw, dx, dres, dx_planes=None, mask_mode=MASK_Y,
+                mask=None):
+    """Launch the backward kernels into the given outputs (dx may be None when dx_planes is given) -> (dgamma, dbeta).
+    y is read only for mask_mode MASK_Y."""
+    ws = _workspace(x.device)
+    C_ext = ws["C"]
+    N, C, H, W = x.shape
+    M = N * H * W
+    dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
+    dbeta = torch.empty(C, dtype=torch.float32, device=x.device)
+    ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+    stream = torch.cuda.current_stream(x.device).cuda_stream
+    with torch.cuda.device(x.device):
+        C_ext.bn_backward(x.data_ptr(), ptr(y), dy.data_ptr(), ptr(dx), ptr(dres), weight.data_ptr(), mean.data_ptr(),
+                          invstd.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(),
+                          (ws["nchw_partial"] if nchw_hw else ws["partial"]).data_ptr(),
+                          ws["nchw_ticket"][2048:].data_ptr() if nchw_hw else ws["b"][0], ws["b"][1], ws["b"][2],
+                          ws["status"], M, C, 1 if relu else 0,
+                          ws["fused"], ws["sm"], 1 if x.dtype == torch.float32 else 0, nchw_hw, stream,
+                          ptr(dx_planes), ptr(bias), mask_mode, ptr(mask))
+    return dgamma, dbeta
+
+
 class _FusedBNActFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, running_mean, running_var, nbt, residual, training, momentum, eps, relu,
                 y_planes=None, dx_planes_wanted=False):
-        ws = _workspace(x.device)
-        C_ext = ws["C"]
-        N, C, H, W = x.shape
-        M = N * H * W
-        y = torch.empty_like(x)                       # preserves channels_last
-        if training:
-            mean = torch.empty(C, dtype=torch.float32, device=x.device)
-            invstd = torch.empty(C, dtype=torch.float32, device=x.device)
-            rm = running_mean.data_ptr() if running_mean is not None else 0
-            rv = running_var.data_ptr() if running_var is not None else 0
-            nb = nbt.data_ptr() if nbt is not None else 0
-        else:
-            mean = running_mean
-            invstd = torch.rsqrt(running_var + eps)
-            rm = rv = nb = 0
-        stream = torch.cuda.current_stream(x.device).cuda_stream
-        nchw = not _eligible(x, residual)              # caller guarantees one of the two layouts is eligible
-        ctx.nchw_hw = H * W if nchw else 0
-        with torch.cuda.device(x.device):
-            C_ext.bn_forward(x.data_ptr(), residual.data_ptr() if residual is not None else 0, y.data_ptr(),
-                             weight.data_ptr(), bias.data_ptr(), mean.data_ptr(), invstd.data_ptr(), rm, rv, nb,
-                             (ws["nchw_partial"] if nchw else ws["partial"]).data_ptr(),
-                             ws["nchw_ticket"].data_ptr() if nchw else ws["f"][0], ws["f"][1], ws["f"][2],
-                             ws["status"], M, C,
-                             float(eps), float(momentum), 1 if relu else 0, 1 if training else 0, ws["fused"],
-                             ws["sm"], 1 if x.dtype == torch.float32 else 0, ctx.nchw_hw, stream,
-                             y_planes.data_ptr() if (y_planes is not None and not nchw) else 0)
-        ctx.planes_emitted = y_planes is not None and not nchw
+        y, mean, invstd, ctx.nchw_hw = bn_forward(x, weight, bias, running_mean, running_var, nbt, residual, training,
+                                                  momentum, eps, relu, y_planes)
+        nchw = ctx.nchw_hw > 0
         ctx.dx_planes = bool(dx_planes_wanted) and not nchw and x.dtype == torch.float32
         ctx.save_for_backward(x, y, weight, mean, invstd)
         ctx.relu, ctx.has_res, ctx.training = relu, residual is not None, training
@@ -115,10 +153,6 @@ class _FusedBNActFn(torch.autograd.Function):
         x, y, weight, mean, invstd = ctx.saved_tensors
         if not ctx.training:
             raise RuntimeError("FusedBNAct backward is only implemented for training mode")
-        ws = _workspace(x.device)
-        C_ext = ws["C"]
-        N, C, H, W = x.shape
-        M = N * H * W
         if ctx.nchw_hw:
             if dy.dtype != x.dtype or not dy.is_contiguous():
                 dy = dy.to(x.dtype).contiguous()
@@ -126,19 +160,8 @@ class _FusedBNActFn(torch.autograd.Function):
             dy = dy.to(x.dtype).contiguous(memory_format=torch.channels_last)
         dx = torch.empty_like(x)
         dres = torch.empty_like(x) if ctx.has_res else None
-        dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
-        dbeta = torch.empty(C, dtype=torch.float32, device=x.device)
         dxp = torch.empty(3, x.numel(), dtype=torch.bfloat16, device=x.device) if ctx.dx_planes else None
-        stream = torch.cuda.current_stream(x.device).cuda_stream
-        with torch.cuda.device(x.device):
-            C_ext.bn_backward(x.data_ptr(), y.data_ptr(), dy.data_ptr(), dx.data_ptr(),
-                              dres.data_ptr() if dres is not None else 0, weight.data_ptr(), mean.data_ptr(),
-                              invstd.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(),
-                              (ws["nchw_partial"] if ctx.nchw_hw else ws["partial"]).data_ptr(),
-                              ws["nchw_ticket"][2048:].data_ptr() if ctx.nchw_hw else ws["b"][0], ws["b"][1], ws["b"][2],
-                              ws["status"], M, C, 1 if ctx.relu else 0,
-                              ws["fused"], ws["sm"], 1 if x.dtype == torch.float32 else 0, ctx.nchw_hw, stream,
-                              dxp.data_ptr() if dxp is not None else 0)
+        dgamma, dbeta = bn_backward(x, y, dy, weight, None, mean, invstd, ctx.relu, ctx.nchw_hw, dx, dres, dxp)
         if dxp is not None:
             from .conv_tc import planes_put
             planes_put(dx, dxp)                     # the producing conv's backward finds its dY already split

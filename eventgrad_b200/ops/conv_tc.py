@@ -187,8 +187,10 @@ class _fork_wgrad:
                     t.record_stream(self.cur)
 
 
-def fprop(ap, wp, N, H, W, Ca, Cb, taps, nsrc=1, wtaps=9, out=None, OH=None, OW=None, os_=1, op=0, oq=0):
-    """implicit GEMM over the pixel grid (N,H,W): out[n, i*os+op, j*os+oq, :] = sum_taps A_tap[n,i,j,:] @ W_tap^T"""
+def fprop(ap, wp, N, H, W, Ca, Cb, taps, nsrc=1, wtaps=9, out=None, OH=None, OW=None, os_=1, op=0, oq=0,
+          addend=None, addmask=None):
+    """implicit GEMM over the pixel grid (N,H,W): out[n, i*os+op, j*os+oq, :] = sum_taps A_tap[n,i,j,:] @ W_tap^T
+    (+ (addmask bit ? addend : 0) when given: fp32 in out's layout, one mask bit per element)"""
     from . import ext
     C = ext()
     OH, OW = OH or H, OW or W
@@ -201,7 +203,8 @@ def fprop(ap, wp, N, H, W, Ca, Cb, taps, nsrc=1, wtaps=9, out=None, OH=None, OW=
         ws = torch.empty(ks, C.conv_fprop_mtiles(N, H, W) * 128, Cb, dtype=torch.float32, device=ap.device)
     with torch.cuda.device(ap.device):
         C.conv_fprop(ap.data_ptr(), wp.data_ptr(), out.data_ptr(), N, H, W, Ca, Cb, taps, nsrc, wtaps, OH, OW, os_,
-                     op, oq, _sm(ap.device), _stream(ap.device), 0 if ws is None else ws.data_ptr(), ks)
+                     op, oq, _sm(ap.device), _stream(ap.device), 0 if ws is None else ws.data_ptr(), ks,
+                     0 if addend is None else addend.data_ptr(), 0 if addmask is None else addmask.data_ptr())
     return out
 
 
@@ -265,85 +268,101 @@ def _parity_planes(x: torch.Tensor) -> torch.Tensor:
     return planes
 
 
+def conv_forward(x, weight, kind, need_dx):
+    """The forward launches of one convolution -> (y [N,OH,OW,Co] fp32, input planes, transposed weight planes or None),
+    the planes being what the backward needs."""
+    N, Ci, H, W = x.shape
+    Co = weight.shape[0]
+    w_ohwi = weight.permute(0, 2, 3, 1).contiguous()                   # no copy when the weight is channels_last
+    if kind == "stem":
+        xp = split3_stem(x.permute(0, 2, 3, 1))
+        w64 = F.pad(w_ohwi.reshape(Co, 27), (0, 37)).reshape(Co, 1, 64)
+        wp, wtp = wprep(w64, False)
+        y = fprop(xp, wp, N, H, W, 64, Co, TAPS_1X1, 1, 1)
+    elif kind == "s1":
+        xp = planes_get(x)
+        if xp is None:
+            xp = split3(x)
+        wp, wtp = wprep(w_ohwi.reshape(Co, 9, Ci), need_dx)
+        y = fprop(xp, wp, N, H, W, Ci, Co, TAPS_S1, 1, 9)
+    elif kind == "p1":
+        xp = planes_get(x)
+        if xp is None:
+            xp = split3(x)
+        wp, wtp = wprep(w_ohwi.reshape(Co, 1, Ci), need_dx)
+        y = fprop(xp, wp, N, H, W, Ci, Co, TAPS_1X1, 1, 1)
+    else:                                                               # s2 / p2: parity images of the input
+        xp = _parity_planes(x)
+        T = 9 if kind == "s2" else 1
+        wp, wtp = wprep(w_ohwi.reshape(Co, T, Ci), need_dx)
+        y = fprop(xp, wp, N, H // 2, W // 2, Ci, Co, TAPS_S2 if kind == "s2" else TAPS_1X1, 4, T)
+    return y, xp, wtp
+
+
+def conv_backward(xp, wtp, gp, geom, kind, need_dx, need_dw, dev, addend=None, addmask=None):
+    """Weight gradient (side stream) and data gradient of one convolution from the planes of dY -> (dx, dw).
+    addend / addmask (s1 / p1 only): the data gradient becomes dgrad + (mask bit ? addend : 0), in its epilogue."""
+    N, Ci, H, W, Co = geom
+    dx = dw = None
+    if kind == "stem":
+        if need_dw:
+            d = wgrad(xp, gp, N, H, W, 64, Co, TAPS_1X1, 1)                           # [Co, 1, 64]
+            dw = d[:, 0, :27].reshape(Co, 3, 3, 3).permute(0, 3, 1, 2)
+    elif kind in ("s1", "p1"):
+        taps, dtaps, T = (TAPS_S1, TAPS_S1_DGRAD, 9) if kind == "s1" else (TAPS_1X1, TAPS_1X1, 1)
+        fork = _fork_wgrad(dev, PAR_BWD and need_dx and need_dw)
+        if need_dw:
+            k = 3 if kind == "s1" else 1
+            with fork:
+                dwr = wgrad(xp, gp, N, H, W, Ci, Co, taps, 1)
+            dw = dwr.reshape(Co, k, k, Ci).permute(0, 3, 1, 2)
+        if need_dx:
+            skip = {} if addend is None else {"addend": addend, "addmask": addmask}
+            dx = fprop(gp, wtp, N, H, W, Co, Ci, dtaps, 1, T, **skip).permute(0, 3, 1, 2)
+        if need_dw:
+            fork.join(dwr)
+    else:
+        assert addend is None, "the skip-connection gradient is folded into stride-1 data gradients only"
+        Ho, Wo = H // 2, W // 2
+        fork = _fork_wgrad(dev, PAR_BWD and need_dx and need_dw)
+        if need_dw:
+            k = 3 if kind == "s2" else 1
+            with fork:
+                dwr = wgrad(xp, gp, N, Ho, Wo, Ci, Co, TAPS_S2 if kind == "s2" else TAPS_1X1, 4)
+            dw = dwr.reshape(Co, k, k, Ci).permute(0, 3, 1, 2)
+        if need_dx:
+            if kind == "s2":
+                dxn = torch.empty(N, H, W, Ci, dtype=torch.float32, device=dev)
+                for (p, q), taps in TAPS_S2_DGRAD.items():
+                    fprop(gp, wtp, N, Ho, Wo, Co, Ci, taps, 1, 9, out=dxn, OH=H, OW=W, os_=2, op=p, oq=q)
+            else:                                       # 1x1 stride 2: only the even/even pixels receive a gradient
+                dxn = torch.zeros(N, H, W, Ci, dtype=torch.float32, device=dev)
+                fprop(gp, wtp, N, Ho, Wo, Co, Ci, TAPS_1X1, 1, 1, out=dxn, OH=H, OW=W, os_=2, op=0, oq=0)
+            dx = dxn.permute(0, 3, 1, 2)
+        if need_dw:
+            fork.join(dwr)
+    return dx, dw
+
+
 class _ConvTcFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, kind):
         N, Ci, H, W = x.shape
-        Co = weight.shape[0]
-        w_ohwi = weight.permute(0, 2, 3, 1).contiguous()               # no copy when the weight is channels_last
-        ctx.kind, ctx.geom = kind, (N, Ci, H, W, Co)
-        if kind == "stem":
-            xp = split3_stem(x.permute(0, 2, 3, 1))
-            w64 = F.pad(w_ohwi.reshape(Co, 27), (0, 37)).reshape(Co, 1, 64)
-            wp, wtp = wprep(w64, False)
-            y = fprop(xp, wp, N, H, W, 64, Co, TAPS_1X1, 1, 1)
-        elif kind == "s1":
-            xp = planes_get(x)
-            if xp is None:
-                xp = split3(x)
-            wp, wtp = wprep(w_ohwi.reshape(Co, 9, Ci), ctx.needs_input_grad[0])
-            y = fprop(xp, wp, N, H, W, Ci, Co, TAPS_S1, 1, 9)
-        elif kind == "p1":
-            xp = planes_get(x)
-            if xp is None:
-                xp = split3(x)
-            wp, wtp = wprep(w_ohwi.reshape(Co, 1, Ci), ctx.needs_input_grad[0])
-            y = fprop(xp, wp, N, H, W, Ci, Co, TAPS_1X1, 1, 1)
-        else:                                                           # s2 / p2: parity images of the input
-            xp = _parity_planes(x)
-            T = 9 if kind == "s2" else 1
-            wp, wtp = wprep(w_ohwi.reshape(Co, T, Ci), ctx.needs_input_grad[0])
-            y = fprop(xp, wp, N, H // 2, W // 2, Ci, Co, TAPS_S2 if kind == "s2" else TAPS_1X1, 4, T)
+        ctx.kind, ctx.geom = kind, (N, Ci, H, W, weight.shape[0])
+        y, xp, wtp = conv_forward(x, weight, kind, ctx.needs_input_grad[0])
         ctx.save_for_backward(xp, wtp)
         return y.permute(0, 3, 1, 2)                                    # logical NCHW, channels_last memory
 
     @staticmethod
     def backward(ctx, dy):
         xp, wtp = ctx.saved_tensors
-        N, Ci, H, W, Co = ctx.geom
-        kind = ctx.kind
         if dy.dtype != torch.float32 or not dy.is_contiguous(memory_format=torch.channels_last):
             dy = dy.to(torch.float32).contiguous(memory_format=torch.channels_last)
         gp = planes_get(dy)                                             # emitted by the BN backward that produced dy
         if gp is None:
             gp = split3(dy)
-        dx = dw = None
-        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        if kind == "stem":
-            if need_dw:
-                d = wgrad(xp, gp, N, H, W, 64, Co, TAPS_1X1, 1)                       # [Co, 1, 64]
-                dw = d[:, 0, :27].reshape(Co, 3, 3, 3).permute(0, 3, 1, 2)
-        elif kind in ("s1", "p1"):
-            taps, dtaps, T = (TAPS_S1, TAPS_S1_DGRAD, 9) if kind == "s1" else (TAPS_1X1, TAPS_1X1, 1)
-            fork = _fork_wgrad(dy.device, PAR_BWD and need_dx and need_dw)
-            if need_dw:
-                k = 3 if kind == "s1" else 1
-                with fork:
-                    dwr = wgrad(xp, gp, N, H, W, Ci, Co, taps, 1)
-                dw = dwr.reshape(Co, k, k, Ci).permute(0, 3, 1, 2)
-            if need_dx:
-                dx = fprop(gp, wtp, N, H, W, Co, Ci, dtaps, 1, T).permute(0, 3, 1, 2)
-            if need_dw:
-                fork.join(dwr)
-        else:
-            Ho, Wo = H // 2, W // 2
-            fork = _fork_wgrad(dy.device, PAR_BWD and need_dx and need_dw)
-            if need_dw:
-                k = 3 if kind == "s2" else 1
-                with fork:
-                    dwr = wgrad(xp, gp, N, Ho, Wo, Ci, Co, TAPS_S2 if kind == "s2" else TAPS_1X1, 4)
-                dw = dwr.reshape(Co, k, k, Ci).permute(0, 3, 1, 2)
-            if need_dx:
-                if kind == "s2":
-                    dxn = torch.empty(N, H, W, Ci, dtype=torch.float32, device=dy.device)
-                    for (p, q), taps in TAPS_S2_DGRAD.items():
-                        fprop(gp, wtp, N, Ho, Wo, Co, Ci, taps, 1, 9, out=dxn, OH=H, OW=W, os_=2, op=p, oq=q)
-                else:                                   # 1x1 stride 2: only the even/even pixels receive a gradient
-                    dxn = torch.zeros(N, H, W, Ci, dtype=torch.float32, device=dy.device)
-                    fprop(gp, wtp, N, Ho, Wo, Co, Ci, TAPS_1X1, 1, 1, out=dxn, OH=H, OW=W, os_=2, op=0, oq=0)
-                dx = dxn.permute(0, 3, 1, 2)
-            if need_dw:
-                fork.join(dwr)
+        dx, dw = conv_backward(xp, wtp, gp, ctx.geom, ctx.kind, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
+                               dy.device)
         return dx, dw, None
 
 

@@ -17,14 +17,22 @@ class ShadowConv2d(nn.Conv2d):
     w16 = None
     b16 = None
 
+    def tc_kind(self, x: torch.Tensor):
+        """The tensor-core convolution (ops/conv_tc.py kind) this layer runs on x, or None."""
+        if (x.is_cuda and x.dtype == torch.float32 and self.bias is None and self.padding_mode == "zeros"
+                and not torch.is_autocast_enabled() and not torch.backends.cudnn.allow_tf32):
+            # reference precision (fp32): eligible convs run on the tensor cores at fp32 accuracy
+            from .conv_tc import kind_of
+            return kind_of(x, self.weight, self.stride, self.padding, self.dilation, self.groups)
+        return None
+
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.w16 is not None and x.is_cuda and torch.is_autocast_enabled():
             return self._conv_forward(x, self.w16, self.b16)
-        if (x.is_cuda and x.dtype == torch.float32 and self.bias is None and self.padding_mode == "zeros"
-                and not torch.is_autocast_enabled() and not torch.backends.cudnn.allow_tf32):
-            # reference precision (fp32): eligible 3x3 convs run on the tensor cores at fp32 accuracy (ops/conv_tc.py)
-            from .conv_tc import conv2d
-            return conv2d(x, self.weight, None, self.stride, self.padding, self.dilation, self.groups)
+        kind = self.tc_kind(x)
+        if kind is not None:
+            from .conv_tc import conv_tc, mark_tc_output
+            return mark_tc_output(conv_tc(x, self.weight, kind))
         return super().forward(x)
 
 
