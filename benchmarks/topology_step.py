@@ -1,14 +1,16 @@
 #!/usr/bin/env python
 """Step-kernel time of the gossip graphs (parallel/topology.py) with R virtual ranks on ONE GPU.
 
-    python benchmarks/topology_step.py [--worlds 4,8] [--topologies ring,exp,1,2] [--model resnet18] [--out file]
+    python benchmarks/topology_step.py [--worlds 4,8] [--topologies "ring;exp;onepeer-exp;1,2"] [--model resnet18]
+                                       [--out file]
 
 Every virtual rank runs the full decent step (push into every slot it feeds -> per-slot flags -> mix -> SGD with
-momentum) on its own stream, against the other virtual ranks' windows in the same HBM.  The timed region is one step
+momentum; onepeer-exp: push into the step's one out-slot -> its flags -> (theta + slot) / 2 -> SGD) on its own stream, against the other virtual ranks' windows in the same HBM.  The timed region is one step
 of all R ranks (CUDA events around the launches, after warm-up); the median over --steps is reported with the bytes
 the R kernels move:
-    per rank 4 * n_padded * (7 + 2 * slots):  theta read twice (push and mix), grad and momentum read, theta and
-    momentum written, grad zeroed, one push store and one inbox load per slot.
+    per rank 4 * n_padded * (7 + 2 * msgs):  theta read twice (push and mix), grad and momentum read, theta and
+    momentum written, grad zeroed, one push store and one inbox load per message (msgs = 2|O| slots on a static graph,
+    2 on the ring, 1 on onepeer-exp, whose rows average over its period: every step moves the same bytes).
 These are single-GPU, HBM-bound numbers: pushes land in the same GPU's memory, so they say what the slot count costs
 the kernel, not what NVLink would take.  The ring is run with its single-slot + ack protocol (double_buffer off), the
 same protocol the graph kernel uses.  Each row records the SM clock the card reported during the timed steps (NVML,
@@ -28,7 +30,7 @@ from eventgrad_b200.config import TrainConfig  # noqa: E402
 from eventgrad_b200.models import build_model  # noqa: E402
 from eventgrad_b200.ops import ext  # noqa: E402
 from eventgrad_b200.ops.local_world import LocalWorld  # noqa: E402
-from eventgrad_b200.parallel.topology import parse_topology  # noqa: E402
+from eventgrad_b200.parallel.topology import Graph  # noqa: E402
 
 
 def gpu_info() -> str:
@@ -84,11 +86,12 @@ def run(R: int, topology: str, model: str, steps: int, warmup: int) -> dict:
                 clocks.append(clk)
     for be in w.backends:
         be.check_status()
-    slots = 2 * len(parse_topology(topology, R))
-    nbytes = R * 4 * t.n_padded * (7 + 2 * slots)
+    graph = Graph.build(0, R, topology)
+    msgs = graph.fanout
+    nbytes = R * 4 * t.n_padded * (7 + 2 * msgs)
     med = statistics.median(times)
     w.close()
-    return {"world": R, "topology": topology, "offsets": list(parse_topology(topology, R)), "slots": slots,
+    return {"world": R, "topology": topology, "offsets": list(graph.offsets), "slots": graph.n_slots, "msgs": msgs,
             "model": model, "grid_per_rank": w.backends[0].grid, "median_us": round(med, 1),
             "min_us": round(min(times), 1), "max_us": round(max(times), 1), "bytes": nbytes,
             "GBps": round(nbytes / med / 1e3, 1),
@@ -99,7 +102,7 @@ def run(R: int, topology: str, model: str, steps: int, warmup: int) -> dict:
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--worlds", default="4,8")
-    ap.add_argument("--topologies", default="ring;exp;1,2", help="';'-separated topology names")
+    ap.add_argument("--topologies", default="ring;exp;onepeer-exp;1,2", help="';'-separated topology names")
     ap.add_argument("--model", default="resnet18")
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=5)

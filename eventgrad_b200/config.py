@@ -72,6 +72,7 @@ class TrainConfig:
     peer_timeout_s: float = 30.0     # bound of every device-side peer wait (sticky status instead of a hang);
                                      # EGB_PEER_TIMEOUT_S overrides
     topology: str = "ring"           # gossip graph (parallel/topology.py): ring | exp (offsets 1,2,4,...) | "o1,o2,..."
+                                     # | onepeer-exp (time-varying: one peer r + 2^((k-1) mod ceil(log2 R)) per step)
                                      # (circulant offsets, at most 4); decent/event only beyond the ring
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
@@ -162,7 +163,9 @@ class TrainConfig:
         offsets out of range for `world`."""
         if self.ring_topology:
             return self
-        from .parallel.topology import parse_topology
+        from .parallel.topology import is_onepeer, parse_topology
+        if is_onepeer(self.topology):       # time-varying: the ring only when there is no peer at all
+            return dataclasses.replace(self, topology="ring") if world == 1 else self
         return dataclasses.replace(self, topology="ring") if parse_topology(self.topology, world) == (1,) else self
 
     def resolved(self, device_type: str, world: int) -> "TrainConfig":
@@ -252,8 +255,10 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--double-buffer", action=argparse.BooleanOptionalAction, default=None)
     p.add_argument("--peer-timeout-s", type=float, default=None)
     p.add_argument("--ce-push", action="store_true", default=None)
-    p.add_argument("--topology", default=None, metavar="ring|exp|O1,O2,...",
-                   help="gossip graph: ring (default), exp (offsets 1,2,4,... up to R/2) or explicit circulant offsets")
+    p.add_argument("--topology", default=None, metavar="ring|exp|onepeer-exp|O1,O2,...",
+                   help="gossip graph: ring (default), exp (offsets 1,2,4,... up to R/2), explicit circulant offsets, or "
+                        "onepeer-exp (time-varying: at step k push to r + 2^((k-1) mod ceil(log2 R)) only, "
+                        "mix (theta + received) / 2)")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

@@ -113,8 +113,12 @@ struct GossipParams {
 // left/right pointers.  A separate block, passed to the graph kernel next to GossipParams, so the ring kernels'
 // parameters are untouched.  Slot s of this rank receives from peer Graph.slots()[s]; out-slot j pushes into slot j of
 // peer Graph.out_slots()[j] (parallel/topology.py).  mix: theta <- (((theta + in_0) + in_1) + ...) / (n_slots + 1)
+// period > 0: the time-varying one-peer exponential graph (OnePeerExp): slot m receives from r - 2^m, and at step k only
+// slot m = (k-1) % period takes part (push, flag, ack), with the mix theta <- (theta + in_m) / 2.  The kernel derives m
+// from the device step counter, so one captured launch serves every step of the cycle.
 struct GraphSlots {
-  int n_slots;                          // 2|O|: even, 2..EG_MAX_SLOTS
+  int n_slots;                          // static: 2|O|, even, 2..EG_MAX_SLOTS; one-peer: period, 1..EG_MAX_SLOTS
+  int period;                           // 0: static circulant graph; > 0: one-peer graph with n_slots == period
   const float* inbox[EG_MAX_SLOTS];     // local: what the sender of slot s last pushed
   float* push[EG_MAX_SLOTS];            // peer-mapped: slot j's inbox of my j-th out peer
   uint32_t* flag_from[EG_MAX_SLOTS];    // local [n_tiles * 8] (tile, warp), written by the sender of slot s
@@ -132,7 +136,8 @@ cudaError_t launch_ce_push(const GossipParams& p, cudaStream_t s);
 int gossip_dbuf_max_grid(int device);
 cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_t s);
 // circulant-graph step (csrc/gossip_graph.cu): the fused single-kernel step over the slots of `g`; requires phase 0,
-// no sparse block, do_push and do_mix, and an even n_slots in [2, EG_MAX_SLOTS]
+// no sparse block, do_push and do_mix, and an even n_slots in [2, EG_MAX_SLOTS] (static) or n_slots == period in
+// [1, EG_MAX_SLOTS] (one-peer)
 int gossip_graph_max_grid(int device);
 cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g, int grid, cudaStream_t s);
 // (re)compute tile_ss (+ shadow) from theta and evaluate the trigger for step pass_num+1.

@@ -74,7 +74,7 @@ static const std::unordered_map<std::string, Setter<GossipParams>> kGossip = {
 };
 
 static const std::unordered_map<std::string, Setter<GraphSlots>> kGraph = {
-    NUMF(GraphSlots, n_slots), ARRF(GraphSlots, inbox), ARRF(GraphSlots, push), ARRF(GraphSlots, flag_from),
+    NUMF(GraphSlots, n_slots), NUMF(GraphSlots, period), ARRF(GraphSlots, inbox), ARRF(GraphSlots, push), ARRF(GraphSlots, flag_from),
     ARRF(GraphSlots, flag_to), ARRF(GraphSlots, ack_from), ARRF(GraphSlots, ack_to),
 };
 

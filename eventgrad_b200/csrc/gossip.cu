@@ -29,6 +29,10 @@
 // GraphSlots block that the graph kernel receives next to GossipParams (parallel/topology.py).  Each fired tile is
 // pushed into every out-slot, iter mode publishes and waits for one flag per slot per (tile, warp), the tail acks
 // every slot, and the mix adds the slots in slot order, two at a time, before one true division by 2|O|+1.
+// With GraphSlots.period = tau > 0 the same kernel runs the time-varying one-peer exponential graph: at step k only slot
+// m = (k-1) % tau is active (push into out-slot m, publish and wait on slot m's flags, ack slot m's sender, WAR guard on
+// the ack of step k - tau) and the mix is (theta + in_m) / 2.  m comes from the device step counter (a uniform branch,
+// no extra instance), so a captured launch replays every step of the cycle.
 // GossipParams is unchanged, so the ring kernels compile exactly as before.
 #include "api.h"
 #include "common.cuh"
@@ -57,9 +61,12 @@ using StepParams = GossipParams;
 #endif
 // messages one fired tensor costs: one per inbox slot it lands in (the reference's logical count)
 #ifdef EG_GRAPH
-#define EG_NMSG(p) ((unsigned long long)(p).g.n_slots)
+#define EG_NMSG(p) ((p).g.period ? 1ull : (unsigned long long)(p).g.n_slots)
+// one-peer graph: the slot of step `step` (1-based); static graphs and the ring have no active slot
+#define EG_ACTIVE_SLOT(p, step) ((p).g.period ? ((step) - 1) % (p).g.period : -1)
 #else
 #define EG_NMSG(p) 2ull
+#define EG_ACTIVE_SLOT(p, step) (-1)
 #endif
 
 namespace egb {
@@ -204,15 +211,19 @@ __device__ __forceinline__ void cta_finish_tensors(const StepParams& p, const Ti
 
 // -------------------------------------------------------------------------------------------
 #ifdef EG_GRAPH
-// Slot loops run over EG_MAX_SLOTS with constant indices (unrolled, predicated on n_slots), so every slot pointer
+// Slot loops run over EG_MAX_SLOTS with constant indices (unrolled, predicated on slot_on), so every slot pointer
 // is read straight from the kernel's parameter bank.
-__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th) {
+// Slot k takes part in this step: every slot of a static graph, only the active slot of a one-peer graph.
+__device__ __forceinline__ bool slot_on(const StepParams& p, int k, int slot) {
+  return p.g.period ? k == slot : k < p.g.n_slots;
+}
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int slot) {
 #pragma unroll
   for (int k = 0; k < EG_MAX_SLOTS; ++k)
-    if (k < p.g.n_slots) st_f8(p.g.push[k] + base, th);
+    if (slot_on(p, k, slot)) st_f8(p.g.push[k] + base, th);
 }
 #else
-__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th) {
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
   // push_r == nullptr: 2-rank ring, the one neighbour is both left and right and reads the single copy twice
   st_f8(p.push_l + base, th);
   if (p.push_r != nullptr) st_f8(p.push_r + base, th);
@@ -220,7 +231,7 @@ __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, cons
 #endif
 #ifdef EG_DBUF
 __device__ __forceinline__ void push_tile_slot(const StepParams& p, size_t base, const F8& th, int step) {
-  push_tile(p, EG_SLOT_OFF(p, step) + base, th);
+  push_tile(p, EG_SLOT_OFF(p, step) + base, th, -1);
 }
 #endif
 
@@ -291,7 +302,7 @@ __device__ __forceinline__ F8 load_grad(const StepParams& p, const TileInfo& ti,
 // mix + SGD + norm-on-write for one tile. `th` already holds theta_k for this thread's 8 floats.
 template <bool kMom>
 __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileInfo& ti, size_t base, F8 th,
-                                         int lane, int warp, int step) {
+                                         int lane, int warp, int step, int slot) {
 #ifdef EG_GRAPH
   // no receive-norm logging on graphs (file_write is ring only); slots are loaded two at a time after the gradient
   // and momentum, which keeps the kernel at 64 registers whatever the degree
@@ -300,7 +311,16 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
   F8 m;
   const F8 g = load_grad(p, ti, base, threadIdx.x);
   if (kMom) m = ld_f8(p.mom + base);
-  if (p.do_mix) {
+  if (p.do_mix && p.g.period) {
+    // one-peer graph: theta <- (theta + in_slot) / 2
+    const float* in = p.g.inbox[0];
+#pragma unroll
+    for (int s = 1; s < EG_MAX_SLOTS; ++s)
+      if (s == slot) in = p.g.inbox[s];
+    const F8 A = ld_f8_cg(in + base);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(__fadd_rn(th.v[e], A.v[e]), 2.f);
+  } else if (p.do_mix) {
 #pragma unroll
     for (int s = 0; s < EG_MAX_SLOTS; s += 2) {
       if (s < p.g.n_slots) {
@@ -374,7 +394,7 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
 
 // Elect the last CTA of the grid; it acks and bumps the step counter (the trigger FSM itself is
 // run per tensor by whichever warp completes that tensor, see cta_finish_tensors).
-__device__ __forceinline__ void grid_tail(const StepParams& p, int step) {
+__device__ __forceinline__ void grid_tail(const StepParams& p, int step, int slot) {
   __shared__ int s_last;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -389,11 +409,11 @@ __device__ __forceinline__ void grid_tail(const StepParams& p, int step) {
     *p.fsm.pass_num = step;
 #if defined(EG_GRAPH)
     if (p.sync && p.send_ack) {
-      // every CTA of this rank has finished reading its inboxes for `step`: ack every slot's sender
+      // every CTA of this rank has finished reading its inboxes for `step`: ack every active slot's sender
       fence_sys();
 #pragma unroll
       for (int s = 0; s < EG_MAX_SLOTS; ++s)
-        if (s < p.g.n_slots) st_release_sys(p.g.ack_to[s], (uint32_t)step);
+        if (slot_on(p, s, slot)) st_release_sys(p.g.ack_to[s], (uint32_t)step);
     }
 #elif !defined(EG_DBUF)
     if (p.sync && p.send_ack) {
@@ -428,7 +448,7 @@ __device__ __forceinline__ void push_phase(const StepParams& p, int step) {
   for (int t = b; t < p.tab.n_tiles; t += G, ++j) {
     if (!(tile_info(p, s_ti, j, t).flags & 1)) continue;
     const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
-    push_tile(p, base, ld_f8(p.theta + base));
+    push_tile(p, base, ld_f8(p.theta + base), -1);
   }
   __syncthreads();
   if (tid == 0) {
@@ -450,6 +470,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   const int b = blockIdx.x, G = gridDim.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int step = *p.fsm.pass_num + 1;
+  const int slot = EG_ACTIVE_SLOT(p, step);
   const int n_tiles = p.tab.n_tiles;
   const bool push = p.do_push != 0 && p.phase != 2;
   // Sticky failure: once any peer wait has timed out (this or an earlier launch) the step is a no-op on every
@@ -493,8 +514,8 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
       const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
       const TileInfo ti = tile_info(p, s_ti, j, t);
       const F8 th = ld_f8(p.theta + base);
-      if (push && (ti.flags & 1)) push_tile(p, base, th);
-      mix_tile<kMom>(p, t, ti, base, th, lane, warp, step);
+      if (push && (ti.flags & 1)) push_tile(p, base, th, slot);
+      mix_tile<kMom>(p, t, ti, base, th, lane, warp, step, slot);
     }
   } else {
     // ---------------- iter-sync: per-WARP software pipeline, no block barriers ------------------
@@ -506,11 +527,13 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #if defined(EG_GRAPH)
     __shared__ int s_ok;
     if (tid == 0) {
-      // WAR guard: every peer I push into must have consumed what I pushed at step-1 before I overwrite it
+      // WAR guard: every peer I push into must have consumed what I last pushed into its slot before I overwrite
+      // it -- at step-1 on a static graph, at step-period on a one-peer graph (slot m is written every period steps)
       bool ok = true;
+      const int prev = max(step - (p.g.period ? p.g.period : 1), 0);   // the first tau steps wait for nothing
 #pragma unroll
       for (int k = 0; k < EG_MAX_SLOTS; ++k)
-        if (k < p.g.n_slots) ok = wait_ge(p.g.ack_from[k], (uint32_t)(step - 1), p.status, p.timeout_ns) && ok;
+        if (slot_on(p, k, slot)) ok = wait_ge(p.g.ack_from[k], (uint32_t)prev, p.status, p.timeout_ns) && ok;
       s_ok = ok;
     }
     __syncthreads();
@@ -539,7 +562,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #ifdef EG_DBUF
           push_tile_slot(p, base, ld_f8(p.theta + base), step);
 #else
-          push_tile(p, base, ld_f8(p.theta + base));
+          push_tile(p, base, ld_f8(p.theta + base), slot);
 #endif
         }
         __syncwarp();
@@ -548,7 +571,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #ifdef EG_GRAPH
 #pragma unroll
           for (int k = 0; k < EG_MAX_SLOTS; ++k)   // (k: out-slot; j is the tile loop's index)
-            if (k < p.g.n_slots) st_release_sys(p.g.flag_to[k] + (size_t)t * EG_WARPS + warp, (uint32_t)step);
+            if (slot_on(p, k, slot)) st_release_sys(p.g.flag_to[k] + (size_t)t * EG_WARPS + warp, (uint32_t)step);
 #else
           st_release_sys(p.flag_to_l + (size_t)t * EG_WARPS + warp, (uint32_t)step);
           st_release_sys(p.flag_to_r + (size_t)t * EG_WARPS + warp, (uint32_t)step);
@@ -561,7 +584,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #ifdef EG_GRAPH
 #pragma unroll
           for (int s = 0; s < EG_MAX_SLOTS; ++s)
-            if (s < p.g.n_slots)
+            if (slot_on(p, s, slot))
               wait_ge(p.g.flag_from[s] + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
 #else
           wait_ge(p.flag_from_l + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
@@ -570,12 +593,12 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         }
         __syncwarp();
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
-        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step);
+        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, slot);
       }
     }
   }
   if (p.need_norm) cta_finish_tensors(p, s_ti, step + 1, p.do_mix != 0, true);
-  grid_tail(p, step);
+  grid_tail(p, step, slot);
 }
 
 #if !defined(EG_DBUF) && !defined(EG_GRAPH)
@@ -660,10 +683,11 @@ int gossip_graph_max_grid(int device) {
 }
 
 // Fused decent/event step on a circulant graph: iter-sync (flags + acks per slot) or async (single pass, no flags).
+// period > 0: the one-peer exponential graph, one active slot per step.
 cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g, int grid, cudaStream_t s) {
-  if (p.phase != 0 || p.sparse != nullptr || !p.do_push || !p.do_mix || g.n_slots < 2 || g.n_slots > EG_MAX_SLOTS ||
-      (g.n_slots & 1))
-    return cudaErrorInvalidValue;
+  const bool slots_ok = g.period == 0 ? (g.n_slots >= 2 && g.n_slots <= EG_MAX_SLOTS && !(g.n_slots & 1))
+                                      : (g.period >= 1 && g.period <= EG_MAX_SLOTS && g.n_slots == g.period);
+  if (p.phase != 0 || p.sparse != nullptr || !p.do_push || !p.do_mix || !slots_ok) return cudaErrorInvalidValue;
   GraphStepParams q;
   static_cast<GossipParams&>(q) = p;
   q.g = g;

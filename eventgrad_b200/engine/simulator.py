@@ -13,7 +13,7 @@ import torch
 
 from ..parallel.arena import TensorTable
 from ..parallel.topology import Graph
-from ..parallel.trigger import (TriggerConfig, TriggerState, mix3_, mixk_, sgd_, topk_select,
+from ..parallel.trigger import (TriggerConfig, TriggerState, mix2_, mix3_, mixk_, sgd_, topk_select,
                                 trigger_step)
 from .lr_schedule import lr_at
 
@@ -26,13 +26,16 @@ class RingSimulator:
                  offsets=(1,)):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
-        resolved for `world`); the default (1,) is the ring."""
+        resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
+        the ring."""
         assert algo in ("cent", "decent", "event", "spevent")
         self.graphs = [Graph.build(r, world, offsets) for r in range(world)]
         self.offsets = self.graphs[0].offsets
         self.n_slots = self.graphs[0].n_slots
-        if self.offsets != (1,) and algo not in ("decent", "event"):
-            raise ValueError(f"offsets {self.offsets}: only decent and event gossip beyond the ring")
+        self.period = self.graphs[0].period          # 0: static graph; tau: one-peer graph, one active slot per step
+        self.fanout = self.graphs[0].fanout          # messages per fired tensor
+        if not self.graphs[0].is_ring and algo not in ("decent", "event"):
+            raise ValueError(f"topology {offsets!r}: only decent and event gossip beyond the ring")
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -56,7 +59,7 @@ class RingSimulator:
         elif algo in ("decent", "event"):
             # inbox[r][s]: what rank r last received in slot s (zero-initialised RMA window, event.cpp:144-147)
             self.inbox = [[torch.zeros_like(theta0) for _ in range(self.n_slots)] for _ in range(world)]
-            if self.n_slots == 2:
+            if self.n_slots == 2 and not self.period:
                 self.inbox_l = [ib[0] for ib in self.inbox]       # ring: slot 0 = from left, slot 1 = from right
                 self.inbox_r = [ib[1] for ib in self.inbox]
 
@@ -109,7 +112,7 @@ class RingSimulator:
                      for r in range(R)]
         self.fire_history.append([f.clone() for f in fires])
         snap = [th.clone() for th in self.theta]
-        n = self.n_slots
+        n = self.fanout
         for r in range(R):
             L, Rn = self.left(r), self.right(r)
             for i in range(t.n_tensors):
@@ -126,14 +129,19 @@ class RingSimulator:
                     self._flat(self.rep_l[Rn], i)[ix] = v    # and my right neighbour's left
                     self.bytes[r] += 2 * 2 * self.k[i] * 4
                 else:
-                    for p, j in self.graphs[r].out_slots():    # a fired tensor goes into every slot I feed
+                    outs = self.graphs[r].out_slots()
+                    if self.period:                            # one-peer graph: only this step's out-slot
+                        outs = [outs[self.graphs[r].active(self.pass_num)]]
+                    for p, j in outs:                          # a fired tensor goes into every slot I feed
                         self._flat(self.inbox[p][j], i).copy_(src)
                     self.bytes[r] += n * t.numels[i] * 4
         # ---- phase 2: mix with whatever the inboxes hold, then SGD -----------------------
         for r in range(R):
             if self.algo == "spevent":
                 mix3_(self.theta[r], self.rep_l[r], self.rep_r[r])
-            elif n == 2:
+            elif self.period:
+                mix2_(self.theta[r], self.inbox[r][self.graphs[r].active(self.pass_num)])
+            elif self.n_slots == 2:
                 mix3_(self.theta[r], self.inbox[r][0], self.inbox[r][1])
             else:
                 mixk_(self.theta[r], self.inbox[r])
@@ -146,9 +154,14 @@ class RingSimulator:
         return int(sum(self.events))
 
     def dense_messages(self) -> int:
-        """Denominator of 'messages saved': 2|O| * sz * passes * R (BASELINE.md; 2 on the ring)."""
-        return self.n_slots * self.table.n_tensors * self.pass_num * self.R
+        """Denominator of 'messages saved': fanout * sz * passes * R (BASELINE.md; 2 on the ring, 2|O| on a static
+        graph, 1 on the one-peer graph)."""
+        return self.fanout * self.table.n_tensors * self.pass_num * self.R
 
-    def mixing_matrix(self) -> torch.Tensor:
-        """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD."""
+    def mixing_matrix(self, step: Optional[int] = None) -> torch.Tensor:
+        """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD.  The one-peer graph's W depends
+        on the 1-based step (default: the next one)."""
+        if self.period:
+            k = self.pass_num + 1 if step is None else step
+            return torch.tensor([g.mixing_row(k) for g in self.graphs], dtype=torch.float64)
         return torch.tensor([g.mixing_row() for g in self.graphs], dtype=torch.float64)

@@ -327,7 +327,7 @@ class Trainer:
         res["events_total"] = self.backend.total_events() if gossip else 0
         if gossip and env.rank == 0 and not cfg.quiet:
             print(f"Total number of events - {res['events_total']}", flush=True)
-        dense = self.ring.n_slots * self.arena.table.n_tensors * self.backend.pass_num * env.world
+        dense = self.ring.fanout * self.arena.table.n_tensors * self.backend.pass_num * env.world
         res["dense_messages"] = dense
         res["messages_saved"] = (1.0 - res["events_total"] / dense) if (gossip and dense) else 0.0
         if evaluate and env.rank == 0:

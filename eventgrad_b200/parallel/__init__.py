@@ -1,6 +1,6 @@
 from .topology import Graph, Ring, parse_topology  # noqa
 from .arena import ParamArena, TensorTable, TILE  # noqa
-from .trigger import TriggerConfig, TriggerState, trigger_step, mix3_, mixk_, sgd_, topk_select  # noqa
+from .trigger import TriggerConfig, TriggerState, trigger_step, mix2_, mix3_, mixk_, sgd_, topk_select  # noqa
 from .base import CommBackend, StepLog  # noqa
 
 

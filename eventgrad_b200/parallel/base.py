@@ -31,13 +31,15 @@ class StepLog:
 
 def check_topology_state(sd: Dict, ring, algo: str) -> None:
     """Refuse to resume gossip state saved under a different graph: the inbox slots would mean other peers.  Ring
-    checkpoints carry no `topology_offsets` key (their format predates graphs)."""
+    checkpoints carry no `topology_offsets` key (their format predates graphs); static graphs carry no `topology` key,
+    time-varying ones store their name (onepeer-exp), whose offsets can equal a static graph's."""
     if algo not in ("decent", "event"):
         return
-    saved = tuple(sd.get("topology_offsets", (1,)))
-    now = tuple(getattr(ring, "offsets", (1,)))
+    saved = (str(sd.get("topology", "circulant")), tuple(sd.get("topology_offsets", (1,))))
+    now = (getattr(ring, "kind", "circulant"), tuple(getattr(ring, "offsets", (1,))))
     if saved != now:
-        raise ValueError(f"checkpoint was written with topology offsets {saved}, this run uses {now}; "
+        raise ValueError(f"checkpoint was written with topology {saved[0]} offsets {saved[1]}, this run uses "
+                         f"{now[0]} offsets {now[1]}; "
                          "resume with the same --topology")
 
 

@@ -25,7 +25,7 @@ import torch
 import torch.distributed as dist
 
 from .base import CommBackend, StepLog, check_topology_state
-from .trigger import TriggerConfig, TriggerState, mix3_, mixk_, sgd_, topk_select, trigger_step
+from .trigger import TriggerConfig, TriggerState, mix2_, mix3_, mixk_, sgd_, topk_select, trigger_step
 
 
 class CollectiveBackend(CommBackend):
@@ -55,7 +55,7 @@ class CollectiveBackend(CommBackend):
                 self.inbox_l = torch.zeros_like(arena.theta)
                 self.inbox_r = torch.zeros_like(arena.theta)
             else:
-                # circulant graph (parallel/topology.py): one zero-initialised inbox per slot
+                # circulant or one-peer graph (parallel/topology.py): one zero-initialised inbox per slot
                 self.inbox = [torch.zeros_like(arena.theta) for _ in range(ring.n_slots)]
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
@@ -101,14 +101,29 @@ class CollectiveBackend(CommBackend):
             for w in dist.batch_isend_irecv(ops):
                 w.wait()
 
-    def _exchange_slots(self, payload: torch.Tensor, recv: List[torch.Tensor]) -> None:
-        """Graph rendezvous: `payload` goes into every slot I feed (out-slot j = slot j of its peer), recv[s] receives
-        slot s.  The tag is the slot index, so two slots fed by the same peer (offset R/2) cannot cross."""
+    def _active_slots(self) -> List[int]:
+        """Slots that take part in this step: all of a static graph, the one active slot of a one-peer graph."""
         g = self.ring
-        ops = [dist.P2POp(dist.isend, payload, p, self.group, tag=j) for p, j in g.out_slots()]
-        ops += [dist.P2POp(dist.irecv, d, p, self.group, tag=s) for s, (p, d) in enumerate(zip(g.slots(), recv))]
+        return [g.active(self.pass_num)] if g.period else list(range(g.n_slots))
+
+    def _exchange_slots(self, payload: torch.Tensor, recv: List[torch.Tensor]) -> None:
+        """Graph rendezvous over the active slots: `payload` goes into every active slot I feed (out-slot j = slot j of
+        its peer), recv[s] receives active slot s (the other entries are left alone).  The tag is the slot index, so
+        two slots fed by the same peer (offset R/2) cannot cross.  One-peer graph: one isend to the step's out-peer
+        and one irecv from its in-peer."""
+        g = self.ring
+        act, outs, ins = self._active_slots(), g.out_slots(), g.slots()
+        ops = [dist.P2POp(dist.isend, payload, outs[j][0], self.group, tag=outs[j][1]) for j in act]
+        ops += [dist.P2POp(dist.irecv, recv[s], ins[s], self.group, tag=s) for s in act]
         for w in dist.batch_isend_irecv(ops):
             w.wait()
+
+    def _mix_slots(self) -> None:
+        """Static graph: mixk_ over every slot.  One-peer graph: (theta + active slot) / 2."""
+        if self.ring.period:
+            mix2_(self.arena.theta, self.inbox[self.ring.active(self.pass_num)])
+        else:
+            mixk_(self.arena.theta, self.inbox)
 
     def _opt(self) -> None:
         a, cfg = self.arena, self.cfg
@@ -142,8 +157,8 @@ class CollectiveBackend(CommBackend):
         a = self.arena
         if hasattr(self, "inbox"):
             self._exchange_slots(a.theta, self.inbox)
-            self.bytes += len(self.inbox) * a.table.n_elems * 4
-            mixk_(a.theta, self.inbox)
+            self.bytes += self.ring.fanout * a.table.n_elems * 4
+            self._mix_slots()
             self._opt()
             return
         self._exchange([a.theta], [a.theta], [self.inbox_l], [self.inbox_r])
@@ -166,29 +181,33 @@ class CollectiveBackend(CommBackend):
         return fire.tolist(), ml.bool().tolist(), mr.bool().tolist()
 
     def _step_event_graph(self) -> None:
-        """event on a circulant graph: fire masks per slot, then one payload of my fired tensors into every slot."""
+        """event on a graph: fire masks per active slot, then one payload of my fired tensors into every active slot
+        (every slot of a static graph, the step's one slot of a one-peer graph)."""
         a, t = self.arena, self.arena.table
-        n = len(self.inbox)
+        n, fan = len(self.inbox), self.ring.fanout
+        act = self._active_slots()
         _, fire = self._fire()
         m = fire.to(torch.uint8)
         masks = [torch.empty_like(m) for _ in range(n)]
         self._exchange_slots(m, masks)
         mine = fire.tolist()
-        self.events += n * sum(mine)
+        self.events += fan * sum(mine)
         sent = [self._flat(a.theta, i) for i in range(t.n_tensors) if mine[i]]
         payload = torch.cat(sent) if sent else a.theta.new_empty(0)
-        self.bytes += n * payload.numel() * 4
-        masks = [mk.bool().tolist() for mk in masks]
-        bufs = [a.theta.new_empty(sum(t.numels[i] for i in range(t.n_tensors) if mk[i])) for mk in masks]
+        self.bytes += fan * payload.numel() * 4
+        masks = {s: masks[s].bool().tolist() for s in act}
+        bufs = [None] * n
+        for s in act:
+            bufs[s] = a.theta.new_empty(sum(t.numels[i] for i in range(t.n_tensors) if masks[s][i]))
         self._exchange_slots(payload, bufs)
-        for mask, buf, inbox in zip(masks, bufs, self.inbox):
+        for s in act:
             off = 0
             for i in range(t.n_tensors):
-                if mask[i]:
+                if masks[s][i]:
                     k = t.numels[i]
-                    self._flat(inbox, i).copy_(buf[off:off + k])
+                    self._flat(self.inbox[s], i).copy_(bufs[s][off:off + k])
                     off += k
-        mixk_(a.theta, self.inbox)
+        self._mix_slots()
         self._opt()
 
     def _step_event(self) -> None:
@@ -316,6 +335,8 @@ class CollectiveBackend(CommBackend):
                 sd[k] = getattr(self, k).cpu().clone()
         if hasattr(self, "inbox"):
             sd["topology_offsets"] = list(self.ring.offsets)
+            if self.ring.period:
+                sd["topology"] = self.ring.kind
             for s, ib in enumerate(self.inbox):
                 sd[f"inbox_{s}"] = ib.cpu().clone()
         return sd

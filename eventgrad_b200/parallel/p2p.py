@@ -4,7 +4,8 @@ Per training step, after backward():
   cent     ONE launch: one-/two-shot all-reduce over peer-mapped gradients fused with 1/R and SGD
   decent   ONE launch: push theta to both ring neighbours -> flag handshake -> (t+L+R)/3 -> SGD
            (circulant graph: push into all 2|O| slots I feed -> flags per slot -> (t+s_0+...)/(2|O|+1) -> SGD,
-           csrc/gossip_graph.cu)
+           csrc/gossip_graph.cu; one-peer graph: push into the step's single out-slot m -> slot m's flags ->
+           (t+s_m)/2 -> SGD, same kernel)
   event    ONE launch: as decent, but a tensor is pushed only if its device-resident trigger fired;
            the same kernel accumulates the norms and runs the trigger FSM for the next step
   spevent  batched segmented radix-select top-k + compaction straight into the neighbours'
@@ -285,12 +286,13 @@ class P2PBackend(CommBackend):
                 })
             else:
                 # slot s receives from g.slots()[s]; out-slot j writes slot j of its peer (inbox, flags) and the
-                # receiver acks slot s into its sender's ack word of the same index
+                # receiver acks slot s into its sender's ack word of the same index.  One-peer graph (period > 0): the
+                # same wiring, the kernel picks the active slot from its step counter
                 g, n = self.graph, self.graph.n_slots
                 outs, ins = g.out_slots(), g.slots()
                 gs = C.GraphSlots()
                 gs.update({
-                    "n_slots": n,
+                    "n_slots": n, "period": int(g.period),
                     "inbox": [win.addr(f"inbox_{s}") for s in range(n)],
                     "push": [win.addr(f"inbox_{k}", p) for p, k in outs],
                     "flag_from": [win.addr(f"flag_from_{s}") for s in range(n)],
@@ -492,7 +494,7 @@ class P2PBackend(CommBackend):
         if self.cfg.algo == "cent" and self.ring.world > 1:
             self.host_bytes += self.table.n_elems * 4
         elif self.cfg.algo == "decent" and self.do_comm:
-            self.host_bytes += getattr(self.ring, "n_slots", 2) * self.table.n_elems * 4
+            self.host_bytes += getattr(self.ring, "fanout", 2) * self.table.n_elems * 4
 
     def step(self) -> None:
         if self.overlap:        # no compute to hide behind when called stand-alone: run both halves in order
@@ -565,6 +567,8 @@ class P2PBackend(CommBackend):
             sd[k] = getattr(self, k).cpu().clone()
         if self.cfg.algo in ("decent", "event") and self.graph is not None:
             sd["topology_offsets"] = list(self.graph.offsets)
+            if self.graph.period:
+                sd["topology"] = self.graph.kind
             for k in range(self.graph.n_slots):
                 sd[f"inbox_{k}"] = self.win.view(f"inbox_{k}", torch.float32).cpu().clone()
         elif self.cfg.algo in ("decent", "event"):

@@ -14,6 +14,18 @@ each o ascending, "from r-o" (slot 2k), then "from r+o" (slot 2k+1).  The mix is
 so the mixing matrix W = (I + sum_o (S^o + S^-o)) / (2|O|+1) is symmetric and doubly stochastic.
 When o == R/2 both slots of o come from the same peer and that peer counts twice (the rule the
 ring follows at R == 2, quirk Q15).  O == (1,) is the ring, bit for bit.
+
+`OnePeerExp` ("onepeer-exp") is the time-varying one-peer exponential graph (Ying et al., NeurIPS 2021).  For R >= 2
+let tau = ceil(log2 R) and o_m = 2^m, m = 0 .. tau-1 (every o_m < R).  Steps are 1-based (the device step counter
+pass_num + 1); at step k the active index is m = (k-1) mod tau.  Rank r pushes its fired tensors to r + o_m only, and
+mixes with slot m, which holds what it last received from r - o_m:
+    theta' = (theta + s_m) / 2          (one rounded add, one true division)
+so W_k = (I + S^{o_m}) / 2 is doubly stochastic but directed (not symmetric), and a rank sends ONE copy per step.  When
+R is a power of two, W_tau ... W_1 = 11^T / R: exact consensus every tau steps.  At R == 2 (tau == 1) the mix is
+(theta + theta_peer) / 2, deliberately not the ring's (theta + 2 theta_peer) / 3.  At R == 1 the name resolves to the
+ring.  Rank r has tau slots: slot m receives from r - o_m and out-slot m feeds slot m of r + o_m.  In event mode slot m
+keeps the last value that arrived from r - o_m, which can be from step k - tau or earlier; the trigger state is per
+tensor, not per peer.
 """
 from __future__ import annotations
 
@@ -21,7 +33,13 @@ from dataclasses import dataclass
 from typing import List, Tuple
 
 MAX_OFFSETS = 4          # degree <= 8 (csrc/api.h EG_MAX_SLOTS)
+MAX_SLOTS = 8            # csrc/api.h EG_MAX_SLOTS: the one-peer graph's period tau <= 8, i.e. R <= 256
 RING = (1,)
+ONEPEER = "onepeer-exp"
+
+
+def is_onepeer(spec) -> bool:
+    return isinstance(spec, str) and spec.strip().lower() == ONEPEER
 
 
 @dataclass(frozen=True)
@@ -61,6 +79,11 @@ class Ring:
     def n_slots(self) -> int:
         return 2
 
+    @property
+    def fanout(self) -> int:
+        """Messages one fired tensor costs per step (the event counter's unit)."""
+        return 2
+
     def neighbours(self):
         return self.left, self.right
 
@@ -86,7 +109,8 @@ def parse_topology(spec, world: int) -> Tuple[int, ...]:
     ring          (1,)
     exp           (1, 2, 4, ...) up to world // 2 (at most MAX_OFFSETS of them)
     "o1,o2,..."   explicit offsets: ascending, distinct, each in [1, world // 2], at most MAX_OFFSETS
-    At world == 1 every name resolves to the ring (serial / self-loop semantics)."""
+    At world == 1 every name resolves to the ring (serial / self-loop semantics).  onepeer-exp is time-varying and
+    has no static offsets: at world >= 2 it raises here (OnePeerExp / Graph.build handle it)."""
     if isinstance(spec, (tuple, list)):
         spec = ",".join(str(int(o)) for o in spec)
     s = str(spec).strip().lower()
@@ -94,6 +118,10 @@ def parse_topology(spec, world: int) -> Tuple[int, ...]:
         return RING
     if world < 1:
         raise ValueError(f"world must be >= 1, got {world}")
+    if s == ONEPEER:
+        if world == 1:
+            return RING
+        raise ValueError(f"{ONEPEER} is time-varying: it has no static offsets (use Graph.build / OnePeerExp)")
     half = world // 2
     if s == "exp":
         offs, o = [], 1
@@ -121,12 +149,13 @@ def parse_topology(spec, world: int) -> Tuple[int, ...]:
 def check_topology_name(spec) -> None:
     """World-independent syntax check of a topology name (TrainConfig.validate)."""
     s = str(spec).strip().lower()
-    if s in ("ring", "exp"):
+    if s in ("ring", "exp", ONEPEER):
         return
     try:
         offs = [int(x) for x in s.split(",")]
     except ValueError:
-        raise ValueError(f"topology must be ring, exp or comma-separated offsets like '1,3', got {spec!r}") from None
+        raise ValueError(f"topology must be ring, exp, {ONEPEER} or comma-separated offsets like '1,3', "
+                         f"got {spec!r}") from None
     if not offs or len(offs) > MAX_OFFSETS or offs != sorted(set(offs)) or offs[0] < 1:
         raise ValueError(f"topology {spec!r}: 1 to {MAX_OFFSETS} distinct ascending offsets >= 1")
 
@@ -144,8 +173,14 @@ class Graph:
         object.__setattr__(self, "offsets", parse_topology(tuple(self.offsets), self.world))
 
     @staticmethod
-    def build(rank: int, world: int, spec="ring") -> "Graph":
+    def build(rank: int, world: int, spec="ring"):
+        """The graph of `spec` for this rank: a `Graph`, or a `OnePeerExp` for onepeer-exp at world >= 2."""
+        if is_onepeer(spec) and world >= 2:
+            return OnePeerExp(rank, world)
         return Graph(rank, world, parse_topology(spec, world))
+
+    period = 0               # static graph (OnePeerExp: tau)
+    kind = "circulant"       # checkpoint tag (utils/ckpt.py via parallel/base.py)
 
     @property
     def is_ring(self) -> bool:
@@ -158,6 +193,11 @@ class Graph:
     @property
     def n_slots(self) -> int:
         return 2 * len(self.offsets)
+
+    @property
+    def fanout(self) -> int:
+        """Messages one fired tensor costs per step: one per slot it lands in."""
+        return self.n_slots
 
     def slots(self) -> List[int]:
         """Peer whose pushes land in each of my slots: for o ascending, r-o then r+o."""
@@ -205,3 +245,75 @@ class Graph:
 
     def neighbours(self):
         return self.left, self.right
+
+
+def onepeer_period(world: int) -> int:
+    """tau = ceil(log2 world) for world >= 2."""
+    if world < 2:
+        raise ValueError(f"{ONEPEER} needs at least 2 ranks, got {world}")
+    return (world - 1).bit_length()
+
+
+@dataclass(frozen=True)
+class OnePeerExp:
+    """Time-varying one-peer exponential graph of one rank (see the module docstring).  Slot m receives from r - o_m;
+    out-slot m feeds slot m of r + o_m; at step k (1-based) only slot active(k) takes part."""
+    rank: int
+    world: int
+
+    kind = ONEPEER
+    is_ring = False
+
+    def __post_init__(self):
+        if not (0 <= self.rank < self.world):
+            raise ValueError(f"rank {self.rank} outside world {self.world}")
+        if onepeer_period(self.world) > MAX_SLOTS:
+            raise ValueError(f"{ONEPEER}: at most {2 ** MAX_SLOTS} ranks ({MAX_SLOTS} slots), got {self.world}")
+
+    @property
+    def period(self) -> int:
+        return onepeer_period(self.world)
+
+    @property
+    def offsets(self) -> Tuple[int, ...]:
+        return tuple(1 << m for m in range(self.period))
+
+    @property
+    def serial(self) -> bool:
+        return False
+
+    @property
+    def n_slots(self) -> int:
+        return self.period
+
+    @property
+    def fanout(self) -> int:
+        """Messages one fired tensor costs per step: it goes to the single out-peer of the step."""
+        return 1
+
+    def active(self, step: int) -> int:
+        """Active slot / offset index of 1-based step `step`."""
+        if step < 1:
+            raise ValueError(f"steps are 1-based, got {step}")
+        return (step - 1) % self.period
+
+    def in_peer(self, step: int) -> int:
+        return (self.rank - self.offsets[self.active(step)]) % self.world
+
+    def out_peer(self, step: int) -> int:
+        return (self.rank + self.offsets[self.active(step)]) % self.world
+
+    def slots(self) -> List[int]:
+        """Peer whose pushes land in each of my slots: slot m from r - 2^m."""
+        return [(self.rank - o) % self.world for o in self.offsets]
+
+    def out_slots(self) -> List[Tuple[int, int]]:
+        """For each slot index m, the (peer, peer's slot) I push into when m is active: slot m of r + 2^m."""
+        return [((self.rank + o) % self.world, m) for m, o in enumerate(self.offsets)]
+
+    def mixing_row(self, step: int) -> List[float]:
+        """Row of W_step = (I + S^{o_m}) / 2: weight 1/2 on me and on the in-peer of the step."""
+        row = [0.0] * self.world
+        row[self.rank] += 0.5
+        row[self.in_peer(step)] += 0.5
+        return row

@@ -104,6 +104,13 @@ def mixk_(theta: torch.Tensor, slots) -> torch.Tensor:
 
 
 @torch.no_grad()
+def mix2_(theta: torch.Tensor, slot: torch.Tensor) -> torch.Tensor:
+    """theta <- (theta + slot) / 2: the one-peer exponential graph's mix (parallel/topology.py OnePeerExp), one rounded
+    add and a true division, as the kernel's __fdiv_rn(__fadd_rn(theta, s), 2.f)."""
+    return theta.add_(slot).div_(2)
+
+
+@torch.no_grad()
 def sgd_(theta: torch.Tensor, grad: torch.Tensor, mom, lr: float, mu: float, wd: float = 0.0,
          nesterov: bool = False) -> None:
     """torch.optim.SGD step with dampening 0 (dcifar10/event/event.cpp:196-200; zero momentum buffer ==
