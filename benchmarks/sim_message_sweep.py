@@ -40,6 +40,8 @@ def main():
     ap.add_argument("--sampler", default="sequential", choices=["sequential", "random"])
     ap.add_argument("--max-steps", type=int, default=0)
     ap.add_argument("--train-samples", type=int, default=60000)
+    ap.add_argument("--trigger", default="norm", choices=["norm", "drift"],
+                    help="trigger metric: norm (reference) or drift (||theta - sent||)")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     torch.set_num_threads(max(1, os.cpu_count() or 1))
@@ -53,7 +55,7 @@ def main():
         arena = ParamArena(model)
         t = arena.table
         names = [n for n, _ in model.named_parameters()]
-        sim = RingSimulator(R, arena.theta.clone(), t, a.algo, TriggerConfig(1, hz, 0.0, 2, 30), lr=a.lr,
+        sim = RingSimulator(R, arena.theta.clone(), t, a.algo, TriggerConfig(1, hz, 0.0, 2, 30, a.trigger), lr=a.lr,
                             momentum=a.momentum, topk_percent=a.topk, serial_skip=False)
         samplers = [ShardSampler(len(src), R, r, a.sampler) for r in range(R)]
         steps_per_epoch = samplers[0].num_batches(a.batch)
@@ -85,7 +87,7 @@ def main():
             xt = decode_augment_torch(test.images, test.scale, test.mean, test.std)
             acc = 100.0 * float((functional_call(model, params, (xt,)).argmax(1) == test.labels).float().mean())
         row = {"oracle": "RingSimulator (CPU)", "model": a.model, "algo": a.algo,
-               "topk_percent": a.topk if a.algo == "spevent" else None, "world": R, "horizon": hz, "epochs": a.epochs,
+               "topk_percent": a.topk if a.algo == "spevent" else None, "trigger": a.trigger, "world": R, "horizon": hz, "epochs": a.epochs,
                "steps": sim.pass_num, "events_total": sim.total_events(), "dense_messages": sim.dense_messages(),
                "messages_saved": 1.0 - sim.total_events() / sim.dense_messages(), "bytes_sent_all_ranks": int(sum(sim.bytes)),
                "test_acc": acc, "wall_s": time.perf_counter() - t0}

@@ -4,10 +4,11 @@ the communication on at world 1, so every kernel runs with its full protocol aga
 (CUPTI) kernel table; use it to see where a step's time goes before reaching for ncu.
 
     python benchmarks/step_kernel_profile.py [--algo spevent|decent|event|cent] [--topk 1] [--out file]
-        [--weight-decay 5e-4] [--nesterov] [--lr-schedule multistep|step|cosine]
+        [--weight-decay 5e-4] [--nesterov] [--lr-schedule multistep|step|cosine] [--trigger norm|drift]
 The optimizer flags run the same kernels with weight decay, Nesterov momentum and a per-step learning-rate table
 (engine/lr_schedule.py: two "epochs" spanning the run, so the lr changes inside the profiled window) instead of
-the reference's constant-lr heavy-ball SGD.
+the reference's constant-lr heavy-ball SGD.  The threshold is a constant 0, so event fires every tensor at every
+step; --trigger drift (event/spevent) adds the `sent` traffic of the drift trigger at that full firing rate.
 """
 import argparse
 import os
@@ -34,12 +35,13 @@ def main():
     ap.add_argument("--weight-decay", type=float, default=0.0)
     ap.add_argument("--nesterov", action="store_true")
     ap.add_argument("--lr-schedule", default="constant", choices=["constant", "step", "multistep", "cosine"])
+    ap.add_argument("--trigger", default="norm", choices=["norm", "drift"])
     a = ap.parse_args()
     env = DistEnv(0, 1, 0, torch.device("cuda", 0), "none")
     cfg = TrainConfig(algo=a.algo, dataset="mnist", model=a.model, lr=1e-2, momentum=0.9, sync_mode="iter",
                       thres_type=0, constant=0.0, topk_percent=a.topk, weight_decay=a.weight_decay,
                       nesterov=a.nesterov, lr_schedule=a.lr_schedule, lr_milestones=(1,), lr_step_epochs=1,
-                      epochs=2).validate()
+                      epochs=2, trigger=a.trigger).validate()
     torch.manual_seed(0)
     model = build_model(a.model)
     theta, grad, symm = preallocate_arena_buffers(model, cfg, env)
@@ -61,7 +63,7 @@ def main():
     rows = sorted(((e.key, e.device_time_total / a.steps, e.count / a.steps) for e in prof.key_averages()
                    if e.device_time_total > 0), key=lambda r: -r[1])
     lines = [f"{a.algo} topk={a.topk} model={a.model} wd={a.weight_decay} nesterov={int(a.nesterov)} "
-             f"lr_schedule={a.lr_schedule}: device us per step (calls per step)"]
+             f"lr_schedule={a.lr_schedule} trigger={a.trigger}: device us per step (calls per step)"]
     lines += [f"{us:10.1f} us  x{n:4.1f}  {k[:110]}" for k, us, n in rows]
     print("\n".join(lines))
     if a.out:

@@ -54,6 +54,8 @@ class TrainConfig:
     sent_history: int = 2
     initial_comm_passes: int = 30
     topk_percent: float = 10.0       # spevent only
+    trigger: str = "norm"            # norm: | ||theta|| - ||theta at last send|| | >= thres (the reference rule) |
+                                     # drift: ||theta - sent|| >= thres, sent = what the receivers hold (event/spevent)
     # ---- communication ---------------------------------------------------
     backend: str = "auto"            # auto | p2p (fused sm_90a kernels) | nccl | gloo | refport (reference-structured)
     sync_mode: str = "iter"          # iter (deterministic handshake) | async (reference RMA semantics)
@@ -132,6 +134,16 @@ class TrainConfig:
             raise ValueError(f"lr_milestones must be non-negative and strictly increasing, got {ms}")
         if not self.lr_warmup_epochs >= 0.0:
             raise ValueError("lr_warmup_epochs must be >= 0")
+        if self.trigger not in ("norm", "drift"):
+            raise ValueError(f"trigger must be norm|drift, got {self.trigger!r}")
+        if self.trigger == "drift":
+            if self.algo not in ("event", "spevent"):
+                raise ValueError(f"--trigger drift needs algo event or spevent ({self.algo!r} has no trigger)")
+            if self.backend == "refport":
+                raise ValueError("--trigger drift is not supported by --backend refport (the reference's norm rule only)")
+            if self.file_write:
+                raise ValueError("--trigger drift does not support file_write: the reference log format's norm column "
+                                 "would hold the drift")
         from .parallel.topology import check_topology_name
         check_topology_name(self.topology)
         if not self.ring_topology:
@@ -248,6 +260,9 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--seed", type=int, default=None)
     p.add_argument("--sent-history", type=int, default=None)
     p.add_argument("--initial-comm-passes", type=int, default=None)
+    p.add_argument("--trigger", default=None, choices=["norm", "drift"],
+                   help="event trigger: norm (default, the reference rule: |norm - norm at last send| >= threshold) or "
+                        "drift (||theta - what the neighbours hold|| >= threshold; event/spevent)")
     p.add_argument("--backend", default=None, choices=["auto", "p2p", "nccl", "gloo", "refport"])
     p.add_argument("--sync-mode", default=None, choices=["iter", "async"])
     p.add_argument("--overlap-push", action=argparse.BooleanOptionalAction, default=None,

@@ -48,6 +48,8 @@ struct FsmDev {
   int history;         // sent_history (<= 8)
   int initial_comm_passes;
   int enabled;         // 0: decent / cent (no trigger: fire[] stays all-ones)
+  int metric;          // trigger input: 0 norm difference | ||theta|| - ||theta at last send|| | (reference),
+                       // 1 drift ||theta - sent|| from what the receivers hold (GossipParams.sent); cur_norm holds it
 };
 
 struct SparseParams;
@@ -107,6 +109,10 @@ struct GossipParams {
   int nesterov;             // 1: Nesterov momentum (needs mu > 0)
   const float* lr_table;    // optional [lr_len]: lr of step s is lr_table[min(s-1, lr_len-1)]; null: the scalar lr
   int lr_len;
+  // drift trigger (fsm.metric = 1): what the receivers hold of theta.  event: every pushed tile also stores theta_k
+  // here, and the norm-on-write partials are sum (theta_{k+1} - sent)^2; spevent: the sparse `prev` (written by the
+  // compaction, never by the step kernel).  null: the norm rule, no extra loads or stores
+  float* sent;
 };
 
 // Circulant gossip graph beyond the ring (csrc/gossip_graph.cu): the 2|O| inbox slots that replace the ring's

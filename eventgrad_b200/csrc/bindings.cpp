@@ -65,12 +65,14 @@ static const std::unordered_map<std::string, Setter<GossipParams>> kGossip = {
     NUMF(GossipParams, send_ack), NUMF(GossipParams, zero_grad), NUMF(GossipParams, group_iters),
     PTRF(GossipParams, sparse), NUMF(GossipParams, need_norm), NUMF(GossipParams, phase), TAB_FIELDS(GossipParams),
     NUMF(GossipParams, wd), NUMF(GossipParams, nesterov), PTRF(GossipParams, lr_table), NUMF(GossipParams, lr_len),
+    PTRF(GossipParams, sent),
     PTRF2(GossipParams, fsm, thres), PTRF2(GossipParams, fsm, last_norm), PTRF2(GossipParams, fsm, last_iter),
     PTRF2(GossipParams, fsm, slopes), PTRF2(GossipParams, fsm, fire), PTRF2(GossipParams, fsm, cur_norm),
     PTRF2(GossipParams, fsm, counters), PTRF2(GossipParams, fsm, pass_num), PTRF2(GossipParams, fsm, log_ring),
     NUMF2(GossipParams, fsm, log_cap), NUMF2(GossipParams, fsm, horizon), NUMF2(GossipParams, fsm, constant),
     NUMF2(GossipParams, fsm, thres_type), NUMF2(GossipParams, fsm, history),
     NUMF2(GossipParams, fsm, initial_comm_passes), NUMF2(GossipParams, fsm, enabled),
+    NUMF2(GossipParams, fsm, metric),
 };
 
 static const std::unordered_map<std::string, Setter<GraphSlots>> kGraph = {

@@ -34,6 +34,10 @@
 // the ack of step k - tau) and the mix is (theta + in_m) / 2.  m comes from the device step counter (a uniform branch,
 // no extra instance), so a captured launch replays every step of the cycle.
 // GossipParams is unchanged, so the ring kernels compile exactly as before.
+// Drift trigger (GossipParams.sent set, fsm.metric = 1): every fired tile that is pushed also stores theta_k into
+// `sent` (the same thread that later mixes that tile, so no new cross-GPU ordering), and the norm-on-write partials
+// become sum (theta_{k+1} - sent)^2, read after the SGD update once the gradient and momentum registers are dead.  The
+// FSM then compares ||theta - sent|| with the threshold instead of | ||theta|| - ||theta at the last send|| |.
 #include "api.h"
 #include "common.cuh"
 #include "sparse_apply.cuh"
@@ -107,7 +111,8 @@ __device__ __forceinline__ void fsm_update_tensor(const FsmDev& f, const TableDe
     atomicAdd(f.counters + 1, nmsg * (unsigned long long)tab.t_msg_bytes[i]);
     atomicAdd(f.counters + 2, 1ull);
   }
-  const float value_diff = fabsf(__fsub_rn(norm, f.last_norm[i]));
+  // drift: `norm` already is ||theta - sent||; norm rule: the reference's |norm - last_norm|
+  const float value_diff = f.metric ? norm : fabsf(__fsub_rn(norm, f.last_norm[i]));
   const float iter_diff = __fsub_rn((float)next_step, f.last_iter[i]);
   float th = (f.thres_type == 1) ? __fmul_rn(f.thres[i], f.horizon) : f.constant;
   const bool fire = (value_diff >= th) || (next_step < f.initial_comm_passes);
@@ -221,12 +226,16 @@ __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, cons
 #pragma unroll
   for (int k = 0; k < EG_MAX_SLOTS; ++k)
     if (slot_on(p, k, slot)) st_f8(p.g.push[k] + base, th);
+  if (p.sent != nullptr) st_f8(p.sent + base, th);   // drift trigger: what the receivers now hold
 }
 #else
 __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
   // push_r == nullptr: 2-rank ring, the one neighbour is both left and right and reads the single copy twice
   st_f8(p.push_l + base, th);
   if (p.push_r != nullptr) st_f8(p.push_r + base, th);
+#ifndef EG_DBUF
+  if (p.sent != nullptr) st_f8(p.sent + base, th);   // drift trigger: what the receivers now hold (once, also at R = 2)
+#endif
 }
 #endif
 #ifdef EG_DBUF
@@ -377,6 +386,19 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
     for (int e = 0; e < 8; ++e) z.v[e] = 0.f;
     st_f8(p.grad + base, z);
   }
+#ifndef EG_DBUF
+  if (p.sent != nullptr) {
+    // drift trigger: sum (theta_{k+1} - sent)^2 replaces sum theta_{k+1}^2.  sent was stored by this thread's push of
+    // this tile (or by the split step's push phase / the sparse compaction, both stream-ordered before this kernel)
+    const F8 sv = ld_f8(p.sent + base);
+    ss = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float d = __fsub_rn(th.v[e], sv.v[e]);
+      ss = __fmaf_rn(d, d, ss);
+    }
+  }
+#endif
   ss = warp_sum(ss);
   if (logrecv) {
     ssl = warp_sum(ssl);
@@ -602,7 +624,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 }
 
 #if !defined(EG_DBUF) && !defined(EG_GRAPH)
-// (Re)compute tile partials (+ bf16 shadow) from theta; optionally evaluate the trigger for the
+// (Re)compute tile partials (+ bf16 shadow) from theta (drift trigger: from theta - sent); optionally evaluate the trigger for the
 // first step.  Used once at start-up and after theta is modified outside the step kernel
 // (checkpoint restore).
 __global__ void __launch_bounds__(EG_THREADS, 4) gossip_init_kernel(const GossipParams p, int run_fsm) {
@@ -613,8 +635,17 @@ __global__ void __launch_bounds__(EG_THREADS, 4) gossip_init_kernel(const Gossip
     const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
     const F8 th = ld_f8(p.theta + base);
     float ss = 0.f;
+    if (p.sent != nullptr) {   // drift trigger: sum (theta - sent)^2
+      const F8 sv = ld_f8(p.sent + base);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) ss = __fmaf_rn(th.v[e], th.v[e], ss);
+      for (int e = 0; e < 8; ++e) {
+        const float d = __fsub_rn(th.v[e], sv.v[e]);
+        ss = __fmaf_rn(d, d, ss);
+      }
+    } else {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) ss = __fmaf_rn(th.v[e], th.v[e], ss);
+    }
     if (p.shadow != nullptr) st_bf16x8(p.shadow + base, th);
     ss = warp_sum(ss);
     if (lane == 0) {
@@ -712,7 +743,8 @@ int gossip_dbuf_max_grid(int device) {
 
 // Dense iter-sync exchange only (decent): every tensor fires every step, inboxes hold 2 slots.
 cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_t s) {
-  if (p.phase != 0 || !p.sync || !p.do_push || !p.do_mix || p.fsm.enabled) return cudaErrorInvalidValue;
+  if (p.phase != 0 || !p.sync || !p.do_push || !p.do_mix || p.fsm.enabled || p.sent != nullptr)
+    return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
     gossip_step_kernel_dbuf<true><<<grid, EG_THREADS, 0, s>>>(p);

@@ -13,7 +13,7 @@ import torch
 
 from ..parallel.arena import TensorTable
 from ..parallel.topology import Graph
-from ..parallel.trigger import (TriggerConfig, TriggerState, mix2_, mix3_, mixk_, sgd_, topk_select,
+from ..parallel.trigger import (TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, sgd_, topk_select,
                                 trigger_step)
 from .lr_schedule import lr_at
 
@@ -27,7 +27,8 @@ class RingSimulator:
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
-        the ring."""
+        the ring.  `tcfg.metric == "drift"`: the trigger reads ||theta - sent|| per tensor, where sent[r] is what rank r's
+        receivers hold (event: zero at start, theta_k of every fired tensor at its push; spevent: prev)."""
         assert algo in ("cent", "decent", "event", "spevent")
         self.graphs = [Graph.build(r, world, offsets) for r in range(world)]
         self.offsets = self.graphs[0].offsets
@@ -62,6 +63,10 @@ class RingSimulator:
             if self.n_slots == 2 and not self.period:
                 self.inbox_l = [ib[0] for ib in self.inbox]       # ring: slot 0 = from left, slot 1 = from right
                 self.inbox_r = [ib[1] for ib in self.inbox]
+        self.drift = self.tcfg.metric == "drift" and algo in ("event", "spevent")
+        if self.drift:
+            # what each rank's receivers hold: event -- zero like the inboxes; spevent -- prev itself (same tensors)
+            self.sent = self.prev if algo == "spevent" else [torch.zeros_like(theta0) for _ in range(world)]
 
     # ------------------------------------------------------------------
     def _flat(self, buf, i):
@@ -71,6 +76,12 @@ class RingSimulator:
     def _norms(self, buf):
         return torch.stack([torch.linalg.vector_norm(self._flat(buf, i))
                             for i in range(self.table.n_tensors)]).float()
+
+    def trigger_norms(self, r):
+        """The trigger's per-tensor input for rank r's next decision: ||theta|| (norm) or ||theta - sent|| (drift)."""
+        if self.drift:
+            return drift_norms(self.theta[r], self.sent[r], self.table.offsets, self.table.numels)
+        return self._norms(self.theta[r])
 
     def _sgd(self, r, grad):
         lr = lr_at(self.lr_table, self.pass_num, self.lr)
@@ -87,8 +98,8 @@ class RingSimulator:
              norms: Optional[Sequence[torch.Tensor]] = None) -> None:
         """`fires` (optional, one bool mask per rank) overrides the trigger decisions -- used to
         compare the data path of a kernel bit-for-bit under the kernel's own decisions; `norms`
-        (optional, one [sz] tensor per rank) replaces the oracle's own norm computation so the FSM
-        logic can be compared exactly while norm accuracy is tested separately."""
+        (optional, one [sz] tensor per rank) replaces the oracle's own norm computation (trigger_norms: the drift
+        under the drift metric) so the FSM logic can be compared exactly while norm accuracy is tested separately."""
         R, t = self.R, self.table
         self.pass_num += 1
         if self.algo == "cent":
@@ -107,7 +118,7 @@ class RingSimulator:
             fires = [f.clone().bool().cpu() for f in fires]
         else:
             fires = [trigger_step(self.state[r],
-                                  self._norms(self.theta[r]) if norms is None else norms[r].float().cpu(),
+                                  self.trigger_norms(r) if norms is None else norms[r].float().cpu(),
                                   self.pass_num, self.tcfg)
                      for r in range(R)]
         self.fire_history.append([f.clone() for f in fires])
@@ -134,6 +145,8 @@ class RingSimulator:
                         outs = [outs[self.graphs[r].active(self.pass_num)]]
                     for p, j in outs:                          # a fired tensor goes into every slot I feed
                         self._flat(self.inbox[p][j], i).copy_(src)
+                    if self.drift:                             # one-peer graph: the last value pushed to any peer
+                        self._flat(self.sent[r], i).copy_(src)
                     self.bytes[r] += n * t.numels[i] * 4
         # ---- phase 2: mix with whatever the inboxes hold, then SGD -----------------------
         for r in range(R):

@@ -43,6 +43,18 @@ def check_topology_state(sd: Dict, ring, algo: str) -> None:
                          "resume with the same --topology")
 
 
+def check_trigger_state(sd: Dict, metric: str, algo: str) -> None:
+    """Refuse to resume event / spevent state saved under the other trigger metric: the FSM's thresholds, slopes and
+    pending decision were computed from a different quantity.  Checkpoints without a `trigger` key are norm-trigger
+    checkpoints (their format predates the drift trigger)."""
+    if algo not in ("event", "spevent"):
+        return
+    saved = str(sd.get("trigger", "norm"))
+    if saved != metric:
+        raise ValueError(f"checkpoint was written with --trigger {saved}, this run uses --trigger {metric}; "
+                         "resume with the same --trigger")
+
+
 class CommBackend:
     name = "base"
 

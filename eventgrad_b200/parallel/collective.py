@@ -24,8 +24,9 @@ from typing import List
 import torch
 import torch.distributed as dist
 
-from .base import CommBackend, StepLog, check_topology_state
-from .trigger import TriggerConfig, TriggerState, mix2_, mix3_, mixk_, sgd_, topk_select, trigger_step
+from .base import CommBackend, StepLog, check_topology_state, check_trigger_state
+from .trigger import (TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, sgd_, topk_select,
+                      trigger_step)
 
 
 class CollectiveBackend(CommBackend):
@@ -57,6 +58,11 @@ class CollectiveBackend(CommBackend):
             else:
                 # circulant or one-peer graph (parallel/topology.py): one zero-initialised inbox per slot
                 self.inbox = [torch.zeros_like(arena.theta) for _ in range(ring.n_slots)]
+        # drift trigger: what my receivers hold of my parameters (event: zero like their inboxes, the pushed theta_k of
+        # every fired tensor afterwards; spevent: prev, which the top-k pushes already keep element-wise)
+        self.drift = cfg.algo in ("event", "spevent") and self.tcfg.metric == "drift"
+        if self.drift:
+            self.sent = self.prev if cfg.algo == "spevent" else torch.zeros_like(arena.theta)
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
             self.last_recv_norm_l, self.last_recv_norm_r = z(), z()
@@ -168,10 +174,17 @@ class CollectiveBackend(CommBackend):
 
     def _fire(self):
         a = self.arena
-        norms = a.tensor_norms()
-        thres_before = None
+        t = a.table
+        norms = drift_norms(a.theta, self.sent, t.offsets, t.numels) if self.drift else a.tensor_norms()
         fire = trigger_step(self.state, norms, self.pass_num, self.tcfg)
         return norms, fire
+
+    def _mark_sent(self, mine) -> None:
+        """Drift trigger, event: the fired tensors' theta_k is now what the receivers hold."""
+        if self.drift and self.cfg.algo == "event":
+            for i, f in enumerate(mine):
+                if f:
+                    self._flat(self.sent, i).copy_(self._flat(self.arena.theta, i))
 
     def _masks(self, fire: torch.Tensor):
         """Exchange fire masks with both neighbours; returns host bool lists (mine, left's, right's)."""
@@ -194,6 +207,7 @@ class CollectiveBackend(CommBackend):
         self.events += fan * sum(mine)
         sent = [self._flat(a.theta, i) for i in range(t.n_tensors) if mine[i]]
         payload = torch.cat(sent) if sent else a.theta.new_empty(0)
+        self._mark_sent(mine)
         self.bytes += fan * payload.numel() * 4
         masks = {s: masks[s].bool().tolist() for s in act}
         bufs = [None] * n
@@ -224,6 +238,7 @@ class CollectiveBackend(CommBackend):
         self.events += 2 * nfired
         sent = [self._flat(a.theta, i) for i in range(t.n_tensors) if mine[i]]
         payload = torch.cat(sent) if sent else a.theta.new_empty(0)
+        self._mark_sent(mine)
         self.bytes += 2 * payload.numel() * 4
         nl = sum(t.numels[i] for i in range(t.n_tensors) if lm[i])
         nr = sum(t.numels[i] for i in range(t.n_tensors) if rm[i])
@@ -333,6 +348,10 @@ class CollectiveBackend(CommBackend):
         for k in ("inbox_l", "inbox_r", "prev", "rep_l", "rep_r"):
             if hasattr(self, k):
                 sd[k] = getattr(self, k).cpu().clone()
+        if self.cfg.algo in ("event", "spevent"):
+            sd["trigger"] = self.tcfg.metric
+            if self.drift and self.cfg.algo == "event":
+                sd["sent"] = self.sent.cpu().clone()
         if hasattr(self, "inbox"):
             sd["topology_offsets"] = list(self.ring.offsets)
             if self.ring.period:
@@ -346,7 +365,10 @@ class CollectiveBackend(CommBackend):
         self.events = int(sd["events"])
         self.bytes = int(sd.get("bytes", 0))
         check_topology_state(sd, self.ring, self.cfg.algo)
+        check_trigger_state(sd, self.tcfg.metric, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
+        if self.drift and self.cfg.algo == "event":
+            self.sent.copy_(sd["sent"].to(self.sent.device))
         if hasattr(self, "inbox"):
             for s, ib in enumerate(self.inbox):
                 ib.copy_(sd[f"inbox_{s}"].to(ib.device))

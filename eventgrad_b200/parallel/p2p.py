@@ -20,7 +20,7 @@ from typing import List
 import torch
 
 from .arena import TILE, ParamArena, TensorTable
-from .base import CommBackend, StepLog, check_topology_state
+from .base import CommBackend, StepLog, check_topology_state, check_trigger_state
 from .topology import Graph
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
 
@@ -208,6 +208,14 @@ class P2PBackend(CommBackend):
             self.desc = torch.zeros(t.n_tiles, dtype=torch.int64, device=dev)       # look-back descriptors
             self.sp_bar = zi(4)
             self.applied_l, self.applied_r = zi(t.n_tensors), zi(t.n_tensors)
+        # drift trigger (--trigger drift): the FSM reads ||theta - sent||.  event: `sent` is an arena-sized buffer,
+        # zero like the receivers' inboxes, that the step kernel's pushes keep equal to what was last pushed; spevent:
+        # `prev` already is what the receivers hold, element by element
+        self.metric = getattr(cfg, "trigger", "norm")
+        self.drift = self.metric == "drift" and cfg.algo in ("event", "spevent")
+        self.sent = None
+        if self.drift:
+            self.sent = self.prev if self.sparse else zf(t.n_padded)
         self.ar_ctr = zi(1)
         # gradient pointer table (table mode): device arrays + rotating pinned staging
         self.table_mode = bool(getattr(arena, "table_mode", False)) and cfg.algo != "cent"
@@ -274,6 +282,8 @@ class P2PBackend(CommBackend):
                 "fsm.thres_type": int(cfg.thres_type), "fsm.history": max(1, int(cfg.sent_history)),
                 "fsm.initial_comm_passes": int(cfg.initial_comm_passes),
                 "fsm.enabled": 1 if (cfg.algo in ("event", "spevent") and self.do_comm) else 0,
+                "fsm.metric": 1 if self.drift else 0,
+                "sent": P(self.sent) if (self.drift and self.do_comm) else 0,
             })
             if self.graph is None:
                 gp.update({
@@ -402,6 +412,16 @@ class P2PBackend(CommBackend):
                "lr_len": 0 if self.d_lr is None else int(self.d_lr.numel())}
         self.gp.update(upd)
         self.ap.update(upd)
+
+    def set_sparse_init(self, prev, rep_l, rep_r) -> None:
+        super().set_sparse_init(prev, rep_l, rep_r)
+        if self.drift and self._connected and self.do_comm:
+            # the first decision was taken at connect() from theta_0 - prev: take it again from the new prev, from
+            # the FSM's initial state (no step has run yet)
+            for x in (self.thres, self.last_norm, self.last_iter, self.slopes, self.cur_norm):
+                x.zero_()
+            self.fire.fill_(1)
+            self._init_norms(run_fsm=True)
 
     def _init_norms(self, run_fsm: bool) -> None:
         with torch.cuda.device(self.dev):
@@ -577,10 +597,15 @@ class P2PBackend(CommBackend):
         if self.sparse:
             for k in ("prev", "rep_l", "rep_r"):
                 sd[k] = getattr(self, k).cpu().clone()
+        if self.cfg.algo in ("event", "spevent"):
+            sd["trigger"] = self.metric
+            if self.drift and not self.sparse:
+                sd["sent"] = self.sent.cpu().clone()
         return sd
 
     def load_state_dict(self, sd):
         check_topology_state(sd, self.ring, self.cfg.algo)
+        check_trigger_state(sd, self.metric, self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
@@ -594,6 +619,8 @@ class P2PBackend(CommBackend):
         if self.sparse:
             for k in ("prev", "rep_l", "rep_r"):
                 getattr(self, k).copy_(sd[k].to(self.dev))
+        if self.drift and not self.sparse:
+            self.sent.copy_(sd["sent"].to(self.dev))
         if self.log_ring is not None:
             self._drained = self.pass_num          # log rows of the steps before the checkpoint are not replayed
         # NOTE: handshake counters (flags / acks) restart from pass_num on every rank

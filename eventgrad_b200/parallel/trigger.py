@@ -8,12 +8,21 @@ csrc/gossip.cu implement the same arithmetic on the device; tests compare them t
 Arithmetic types mirror the reference: all state is fp32 (`calloc(sz, 4)`), the slope
 average is accumulated in double (`auto slope_avg = 0.0`) and rounded to fp32 when it
 becomes the new threshold.
+
+Two trigger metrics (TriggerConfig.metric):
+  norm   the reference rule (quirk Q2): fire when | ||theta_i|| - ||theta_i at its last send|| | >= thres_i.  By the
+         triangle inequality this only bounds what the receivers miss from below; a sign flip or a permutation never fires.
+  drift  fire when ||theta_i - sent_i|| >= thres_i, where sent_i is what the receivers hold of tensor i (the value
+         pushed at its last firing; spevent: the element-wise `prev`).  The FSM is unchanged except for its input:
+         value_diff is the drift itself, and the slope / threshold history is computed from it.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
 
 import torch
+
+METRICS = ("norm", "drift")
 
 
 @dataclass
@@ -23,11 +32,12 @@ class TriggerConfig:
     constant: float = 0.0
     sent_history: int = 2
     initial_comm_passes: int = 30
+    metric: str = "norm"         # norm (reference: norm difference) | drift (||theta - sent||)
 
     @staticmethod
     def from_train(cfg) -> "TriggerConfig":
         return TriggerConfig(cfg.thres_type, cfg.horizon, cfg.constant,
-                             cfg.sent_history, cfg.initial_comm_passes)
+                             cfg.sent_history, cfg.initial_comm_passes, getattr(cfg, "trigger", "norm"))
 
 
 class TriggerState:
@@ -59,9 +69,13 @@ class TriggerState:
 def trigger_step(state: TriggerState, curr_norm: torch.Tensor, pass_num: int,
                  cfg: TriggerConfig) -> torch.Tensor:
     """Advance the FSM one training step. Returns the boolean fire mask [sz].
+    `curr_norm`: per-tensor ||theta|| (metric norm) or ||theta - sent|| (metric drift, drift_norms()).
     No host synchronisation: everything stays on curr_norm's device."""
     curr = curr_norm.to(torch.float32)
-    value_diff = (curr - state.last_norm).abs()                       # fabs(float)
+    if cfg.metric == "drift":
+        value_diff = curr.clone()                                     # the drift is the distance itself
+    else:
+        value_diff = (curr - state.last_norm).abs()                   # fabs(float)
     iter_diff = torch.tensor(float(pass_num), dtype=torch.float32,
                              device=curr.device) - state.last_iter    # int - float -> float
     if cfg.thres_type == 1:
@@ -81,6 +95,13 @@ def trigger_step(state: TriggerState, curr_norm: torch.Tensor, pass_num: int,
     state.last_iter.copy_(torch.where(fire, torch.full_like(curr, float(pass_num)),
                                       state.last_iter))
     return fire
+
+
+@torch.no_grad()
+def drift_norms(theta: torch.Tensor, sent: torch.Tensor, offsets, numels) -> torch.Tensor:
+    """Per-tensor ||theta_i - sent_i|| (fp32) of two flat arenas: the drift trigger's input."""
+    d = theta - sent
+    return torch.stack([torch.linalg.vector_norm(d[o:o + n]) for o, n in zip(offsets, numels)]).float()
 
 
 # ---------------------------------------------------------------------------------
