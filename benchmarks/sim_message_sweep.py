@@ -42,6 +42,8 @@ def main():
     ap.add_argument("--train-samples", type=int, default=60000)
     ap.add_argument("--trigger", default="norm", choices=["norm", "drift"],
                     help="trigger metric: norm (reference) or drift (||theta - sent||)")
+    ap.add_argument("--compress", default="none", choices=["none", "int8"],
+                    help="event on the ring: int8 error-feedback codes instead of fp32 messages (bytes_sent counts them)")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     torch.set_num_threads(max(1, os.cpu_count() or 1))
@@ -56,7 +58,7 @@ def main():
         t = arena.table
         names = [n for n, _ in model.named_parameters()]
         sim = RingSimulator(R, arena.theta.clone(), t, a.algo, TriggerConfig(1, hz, 0.0, 2, 30, a.trigger), lr=a.lr,
-                            momentum=a.momentum, topk_percent=a.topk, serial_skip=False)
+                            momentum=a.momentum, topk_percent=a.topk, serial_skip=False, compress=a.compress)
         samplers = [ShardSampler(len(src), R, r, a.sampler) for r in range(R)]
         steps_per_epoch = samplers[0].num_batches(a.batch)
         t0 = time.perf_counter()
@@ -87,7 +89,7 @@ def main():
             xt = decode_augment_torch(test.images, test.scale, test.mean, test.std)
             acc = 100.0 * float((functional_call(model, params, (xt,)).argmax(1) == test.labels).float().mean())
         row = {"oracle": "RingSimulator (CPU)", "model": a.model, "algo": a.algo,
-               "topk_percent": a.topk if a.algo == "spevent" else None, "trigger": a.trigger, "world": R, "horizon": hz, "epochs": a.epochs,
+               "topk_percent": a.topk if a.algo == "spevent" else None, "trigger": a.trigger, "compress": a.compress, "world": R, "horizon": hz, "epochs": a.epochs,
                "steps": sim.pass_num, "events_total": sim.total_events(), "dense_messages": sim.dense_messages(),
                "messages_saved": 1.0 - sim.total_events() / sim.dense_messages(), "bytes_sent_all_ranks": int(sum(sim.bytes)),
                "test_acc": acc, "wall_s": time.perf_counter() - t0}

@@ -76,6 +76,8 @@ class TrainConfig:
     topology: str = "ring"           # gossip graph (parallel/topology.py): ring | exp (offsets 1,2,4,...) | "o1,o2,..."
                                      # | onepeer-exp (time-varying: one peer r + 2^((k-1) mod ceil(log2 R)) per step)
                                      # (circulant offsets, at most 4); decent/event only beyond the ring
+    compress: str = "none"           # none | int8: decent/event on the ring send the int8 code of theta - prev (one fp32
+                                     # scale per 256 elements) with error feedback instead of fp32 theta
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -160,6 +162,29 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError(f"topology {self.topology!r} does not support file_write: the reference's log format "
                                  "has exactly one left and one right receive column")
+        if self.compress not in ("none", "int8"):
+            raise ValueError(f"compress must be none|int8, got {self.compress!r}")
+        if self.compress == "int8":
+            # the int8 step exists as the iter-sync fused ring step (csrc/gossip_q8.cu) and in the torch.distributed
+            # backends.  Explicit offsets other than "1" are never the ring; exp and onepeer-exp are the ring at small
+            # world sizes, so for_world() checks them once the world size is known
+            s = str(self.topology).strip().lower()
+            if not (self.ring_topology or s in ("exp", "onepeer-exp")):
+                raise ValueError(f"--compress int8 runs on the ring only, got topology {self.topology!r}")
+            if self.algo not in ("decent", "event"):
+                raise ValueError(f"--compress int8 needs algo decent or event, got {self.algo!r}"
+                                 + (" (spevent is its own compressor)" if self.algo == "spevent" else ""))
+            if self.sync_mode != "iter":
+                raise ValueError("--compress int8 needs --sync-mode iter: a delta applied to a torn or stale inbox is "
+                                 "not idempotent")
+            if self.backend == "refport":
+                raise ValueError("--compress int8 is not supported by --backend refport")
+            for name in ("overlap_push", "double_buffer", "ce_push"):
+                if getattr(self, name):
+                    raise ValueError(f"--compress int8 does not support {name} (fused single-kernel step only)")
+            if self.file_write:
+                raise ValueError("--compress int8 does not support file_write: the reference's log format records "
+                                 "the received fp32 tensors")
         return self
 
     @property
@@ -177,8 +202,13 @@ class TrainConfig:
             return self
         from .parallel.topology import is_onepeer, parse_topology
         if is_onepeer(self.topology):       # time-varying: the ring only when there is no peer at all
-            return dataclasses.replace(self, topology="ring") if world == 1 else self
-        return dataclasses.replace(self, topology="ring") if parse_topology(self.topology, world) == (1,) else self
+            ring = world == 1
+        else:
+            ring = parse_topology(self.topology, world) == (1,)
+        if not ring and self.compress == "int8":
+            raise ValueError(f"--compress int8 runs on the ring only; topology {self.topology!r} is not the ring for "
+                             f"{world} ranks")
+        return dataclasses.replace(self, topology="ring") if ring else self
 
     def resolved(self, device_type: str, world: int) -> "TrainConfig":
         """Fill the auto (None) execution switches for the device the job actually runs on: on a GPU the fast path
@@ -201,7 +231,7 @@ class TrainConfig:
             kw["cuda_graph"] = cuda
         if c.overlap_push is None:
             kw["overlap_push"] = bool(cuda and p2p and world >= 2 and c.algo in ("decent", "event")
-                                      and not bool(c.double_buffer) and c.ring_topology)
+                                      and not bool(c.double_buffer) and c.ring_topology and c.compress == "none")
         return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
@@ -274,6 +304,9 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
                    help="gossip graph: ring (default), exp (offsets 1,2,4,... up to R/2), explicit circulant offsets, or "
                         "onepeer-exp (time-varying: at step k push to r + 2^((k-1) mod ceil(log2 R)) only, "
                         "mix (theta + received) / 2)")
+    p.add_argument("--compress", default=None, choices=["none", "int8"],
+                   help="decent/event on the ring: send the int8 code of theta - (what the neighbours hold) with one "
+                        "fp32 scale per 256 elements, about a quarter of the fp32 bytes (default none)")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

@@ -133,6 +133,26 @@ struct GraphSlots {
   uint32_t* ack_to[EG_MAX_SLOTS];       // peer-mapped: ack_from[s] of the sender of slot s
 };
 
+// int8 error-feedback compression of the ring's pushes (csrc/gossip_q8.cu, --compress int8): a separate block passed
+// to the q8 kernel next to GossipParams, which keeps its ring flag / ack pointers.  Per fired tile each warp sends the
+// int8 code of theta - prev for its 256 elements (one 8-byte store per lane and neighbour) and one fp32 scale, adds the
+// dequantized delta to `prev`, and its receivers add the same delta to their replica of it; the mix reads the
+// replicas: theta <- ((theta + rep_l) + rep_r) / 3.  The codec (parallel/trigger.py q8_encode) is
+// s = max|d| / 127, q = s == 0 ? 0 : clamp(rint(d / s), -127, 127), deq = q * s, all IEEE round-to-nearest.
+struct Q8Slots {
+  const int8_t* q_from_l;   // local [n_tiles * EG_TILE] codes last pushed by my LEFT neighbour
+  const int8_t* q_from_r;
+  const float* s_from_l;    // local [n_tiles * 8] one scale per (tile, warp) block
+  const float* s_from_r;
+  int8_t* q_to_l;           // peer-mapped: LEFT neighbour's q_from_r
+  int8_t* q_to_r;           // peer-mapped: RIGHT neighbour's q_from_l
+  float* s_to_l;
+  float* s_to_r;
+  float* prev;              // what my neighbours hold of my theta (dequantized public copy)
+  float* rep_l;             // my copy of my LEFT neighbour's prev
+  float* rep_r;
+};
+
 int gossip_max_grid(int device);  // co-resident CTAs (persistent grid upper bound)
 cudaError_t launch_gossip_step(const GossipParams& p, int grid, cudaStream_t s);
 // experimental double-buffered dense variant (csrc/gossip_dbuf.cu): inbox_l/inbox_r/push_l/push_r address
@@ -146,6 +166,11 @@ cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_
 // [1, EG_MAX_SLOTS] (one-peer)
 int gossip_graph_max_grid(int device);
 cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g, int grid, cudaStream_t s);
+// int8-compressed ring step (csrc/gossip_q8.cu): the fused single-kernel step with the pushes, replicas and flags of
+// `q`; requires phase 0, sync, do_push and do_mix, no sparse block, and every pointer of `q` set.  The iter-sync flag of
+// (tile, warp) carries 2*step + fired (PROTOCOL.md 1.7)
+int gossip_q8_max_grid(int device);
+cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int grid, cudaStream_t s);
 // (re)compute tile_ss (+ shadow) from theta and evaluate the trigger for step pass_num+1.
 cudaError_t launch_gossip_init(const GossipParams& p, int grid, int run_fsm, cudaStream_t s);
 // Trigger FSM alone with externally supplied norms (unit tests against the oracle).

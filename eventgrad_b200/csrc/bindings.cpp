@@ -80,6 +80,12 @@ static const std::unordered_map<std::string, Setter<GraphSlots>> kGraph = {
     ARRF(GraphSlots, flag_to), ARRF(GraphSlots, ack_from), ARRF(GraphSlots, ack_to),
 };
 
+static const std::unordered_map<std::string, Setter<Q8Slots>> kQ8 = {
+    PTRF(Q8Slots, q_from_l), PTRF(Q8Slots, q_from_r), PTRF(Q8Slots, s_from_l), PTRF(Q8Slots, s_from_r),
+    PTRF(Q8Slots, q_to_l), PTRF(Q8Slots, q_to_r), PTRF(Q8Slots, s_to_l), PTRF(Q8Slots, s_to_r),
+    PTRF(Q8Slots, prev), PTRF(Q8Slots, rep_l), PTRF(Q8Slots, rep_r),
+};
+
 static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce = {
     PTRF(AllReduceParams, peer_bufs), PTRF(AllReduceParams, local), PTRF(AllReduceParams, theta),
     PTRF(AllReduceParams, mom), PTRF(AllReduceParams, shadow), PTRF(AllReduceParams, peer_flags),
@@ -165,6 +171,7 @@ PYBIND11_MODULE(_C, m) {
   m.attr("arch") = "sm_90a";
   bind_params<GossipParams>(m, "GossipParams", kGossip);
   bind_params<GraphSlots>(m, "GraphSlots", kGraph);
+  bind_params<Q8Slots>(m, "Q8Slots", kQ8);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
   bind_params<SparseParams>(m, "SparseParams", kSparse);
   bind_params<BnParams>(m, "BnParams", kBn);
@@ -186,6 +193,10 @@ PYBIND11_MODULE(_C, m) {
   m.def("gossip_graph_max_grid", &gossip_graph_max_grid);
   m.def("gossip_step_graph", [](const GossipParams& p, const GraphSlots& g, int grid, uintptr_t s) {
     check(launch_gossip_step_graph(p, g, grid, S(s)), "gossip_step_graph");
+  });
+  m.def("gossip_q8_max_grid", &gossip_q8_max_grid);
+  m.def("gossip_step_q8", [](const GossipParams& p, const Q8Slots& q, int grid, uintptr_t s) {
+    check(launch_gossip_step_q8(p, q, grid, S(s)), "gossip_step_q8");
   });
   m.def("gossip_init", [](const GossipParams& p, int grid, int run_fsm, uintptr_t s) {
     check(launch_gossip_init(p, grid, run_fsm, S(s)), "gossip_init");

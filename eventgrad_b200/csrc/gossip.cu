@@ -38,6 +38,12 @@
 // `sent` (the same thread that later mixes that tile, so no new cross-GPU ordering), and the norm-on-write partials
 // become sum (theta_{k+1} - sent)^2, read after the SGD update once the gradient and momentum registers are dead.  The
 // FSM then compares ||theta - sent|| with the threshold instead of | ||theta|| - ||theta at the last send|| |.
+// csrc/gossip_q8.cu defines EG_Q8 and includes it a fourth time for int8 error-feedback compression of the ring's
+// pushes (`gossip_step_kernel_q8`, decent/event, iter-sync fused step only): a fired tile's warp encodes theta - prev
+// of its 256 elements as int8 codes plus one fp32 scale, stores them into the neighbours' code / scale inboxes of the
+// Q8Slots block, and adds the dequantized delta to `prev`.  The (tile, warp) flag carries 2*step + fired, so the
+// receiver learns from the flag whether to add the neighbour's delta to its replica before the mix
+// ((theta + rep_l) + rep_r) / 3.  Under the drift trigger GossipParams.sent is `prev`.
 #include "api.h"
 #include "common.cuh"
 #include "sparse_apply.cuh"
@@ -48,6 +54,11 @@ struct GraphStepParams : GossipParams {   // kernel parameter of the graph build
   GraphSlots g;
 };
 using StepParams = GraphStepParams;
+#elif defined(EG_Q8)
+struct Q8StepParams : GossipParams {      // kernel parameter of the q8 build: the ring block + the int8 slots
+  Q8Slots q;
+};
+using StepParams = Q8StepParams;
 #else
 using StepParams = GossipParams;
 #endif
@@ -58,6 +69,9 @@ using StepParams = GossipParams;
 #define EG_SLOT_OFF(p, step) ((size_t)((step) & 1) * ((size_t)(p).tab.n_tiles * EG_TILE))
 #elif defined(EG_GRAPH)
 #define EG_SYM(name) name##_graph
+#define EG_SLOT_OFF(p, step) ((size_t)0)
+#elif defined(EG_Q8)
+#define EG_SYM(name) name##_q8
 #define EG_SLOT_OFF(p, step) ((size_t)0)
 #else
 #define EG_SYM(name) name
@@ -228,6 +242,76 @@ __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, cons
     if (slot_on(p, k, slot)) st_f8(p.g.push[k] + base, th);
   if (p.sent != nullptr) st_f8(p.sent + base, th);   // drift trigger: what the receivers now hold
 }
+#elif defined(EG_Q8)
+__device__ __forceinline__ void st_u32x2(void* p, uint32_t lo, uint32_t hi) {
+  asm volatile("st.global.v2.u32 [%0], {%1,%2};" ::"l"(p), "r"(lo), "r"(hi) : "memory");
+}
+__device__ __forceinline__ void ld_u32x2_cg(const void* p, uint32_t& lo, uint32_t& hi) {
+  asm volatile("ld.global.cg.v2.u32 {%0,%1}, [%2];" : "=r"(lo), "=r"(hi) : "l"(p));
+}
+// One block = the 256 elements of this warp's slice of the tile (base >> 8 is its (tile, warp) index).  Encode
+// d = theta - prev with one scale per block, push the 8 codes of this lane to both neighbours (one 8-byte store each),
+// lane 0 pushes the scale, and prev += deq.  Bit for bit parallel/trigger.py q8_encode / q8_decode.
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
+  F8 pv = ld_f8(p.q.prev + base);
+  F8 d;
+  float a = 0.f;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    d.v[e] = __fsub_rn(th.v[e], pv.v[e]);
+    a = fmaxf(a, fabsf(d.v[e]));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+  const float s = __fdiv_rn(a, 127.f);
+  uint32_t lo = 0u, hi = 0u;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const float qf = (s == 0.f) ? 0.f : fminf(fmaxf(rintf(__fdiv_rn(d.v[e], s)), -127.f), 127.f);
+    const uint32_t b = (uint32_t)((int)qf) & 0xffu;
+    if (e < 4)
+      lo |= b << (8 * e);
+    else
+      hi |= b << (8 * (e - 4));
+    pv.v[e] = __fadd_rn(pv.v[e], __fmul_rn(qf, s));
+  }
+  st_u32x2(p.q.q_to_l + base, lo, hi);
+  st_u32x2(p.q.q_to_r + base, lo, hi);
+  if ((threadIdx.x & 31) == 0) {
+    p.q.s_to_l[base >> 8] = s;
+    p.q.s_to_r[base >> 8] = s;
+  }
+  st_f8(p.q.prev + base, pv);
+}
+// Receive side of one neighbour: when it fired this block, add its dequantized delta to my replica of its prev (the
+// same fp32 add it applied to prev) and store the replica back; return theta + replica.
+__device__ __forceinline__ F8 q8_recv_add(float* rep, const int8_t* qin, const float* sin, size_t base, F8 th,
+                                          bool fired) {
+  F8 r = ld_f8(rep + base);
+  if (fired) {
+    uint32_t lo, hi;
+    ld_u32x2_cg(qin + base, lo, hi);
+    const float s = __ldcg(sin + (base >> 8));
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int qv = (int)(int8_t)(((e < 4) ? lo >> (8 * e) : hi >> (8 * (e - 4))) & 0xffu);
+      r.v[e] = __fadd_rn(r.v[e], __fmul_rn((float)qv, s));
+    }
+    st_f8(rep + base, r);
+  }
+#pragma unroll
+  for (int e = 0; e < 8; ++e) th.v[e] = __fadd_rn(th.v[e], r.v[e]);
+  return th;
+}
+// wait_ge that returns the flag value it saw.  In the q8 build a flag of step k is 2k + fired, and the WAR ack makes
+// the value seen exactly 2k or 2k + 1 (PROTOCOL.md 1.7).
+__device__ __forceinline__ uint32_t wait_ge_value(const uint32_t* flag, uint32_t want, int* status,
+                                                  uint64_t timeout_ns) {
+  const uint32_t v = ld_acquire_sys(flag);
+  if (v >= want) return v;
+  wait_ge(flag, want, status, timeout_ns);
+  return ld_acquire_sys(flag);
+}
 #else
 __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
   // push_r == nullptr: 2-rank ring, the one neighbour is both left and right and reads the single copy twice
@@ -342,6 +426,18 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
 #pragma unroll
     for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(th.v[e], k);
   }
+#elif defined(EG_Q8)
+  // `slot` carries the sides whose neighbour fired this block (bit 0 left, bit 1 right), read from the flags.  The
+  // replicas are loaded one side at a time after the gradient and momentum, as the graph build stages its slots
+  constexpr bool logrecv = false;
+  float ssl = 0.f, ssr = 0.f;
+  F8 m;
+  const F8 g = load_grad(p, ti, base, threadIdx.x);
+  if (kMom) m = ld_f8(p.mom + base);
+  th = q8_recv_add(p.q.rep_l, p.q.q_from_l, p.q.s_from_l, base, th, (slot & 1) != 0);
+  th = q8_recv_add(p.q.rep_r, p.q.q_from_r, p.q.s_from_r, base, th, (slot & 2) != 0);
+#pragma unroll
+  for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(th.v[e], 3.0f);
 #else
   const bool logrecv = (p.tile_ss_l != nullptr);
   float ssl = 0.f, ssr = 0.f;
@@ -500,7 +596,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   // when it reads the status word.  (Uniform per CTA; the run is over, so a partial step does not matter.)
   if (p.do_push && *reinterpret_cast<volatile int*>(p.status) != EG_OK) return;
 
-#if defined(EG_DBUF)
+#if defined(EG_DBUF) || defined(EG_Q8)
   if (p.phase != 0 || !(p.sync && push)) return;   // the launcher rejects these; never reached
 #elif defined(EG_GRAPH)
   if (p.phase != 0) return;                        // fused step only (the launcher rejects the rest)
@@ -512,7 +608,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #endif
   __shared__ TileInfo s_ti[EG_TI_CACHE];
   fill_tile_cache(p, s_ti);
-#if !defined(EG_DBUF) && !defined(EG_GRAPH)
+#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8)
   // spevent: receive side first -- scatter the records that arrived for this step into the replicas
   // (inbox_l / inbox_r point at them), grid barrier, then the dense mix below reads them tile by tile
   if (p.sparse != nullptr) sparse_apply_prologue(*p.sparse, p.sparse->bar);
@@ -590,10 +686,15 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         __syncwarp();
         if (lane == 0) {
           if (fired) fence_sys();                  // my warp's stores are performed before the flag
-#ifdef EG_GRAPH
+#if defined(EG_GRAPH)
 #pragma unroll
           for (int k = 0; k < EG_MAX_SLOTS; ++k)   // (k: out-slot; j is the tile loop's index)
             if (slot_on(p, k, slot)) st_release_sys(p.g.flag_to[k] + (size_t)t * EG_WARPS + warp, (uint32_t)step);
+#elif defined(EG_Q8)
+          // 2*step + fired: the receivers learn from the flag whether this block carries a delta
+          const uint32_t v = 2u * (uint32_t)step + (fired ? 1u : 0u);
+          st_release_sys(p.flag_to_l + (size_t)t * EG_WARPS + warp, v);
+          st_release_sys(p.flag_to_r + (size_t)t * EG_WARPS + warp, v);
 #else
           st_release_sys(p.flag_to_l + (size_t)t * EG_WARPS + warp, (uint32_t)step);
           st_release_sys(p.flag_to_r + (size_t)t * EG_WARPS + warp, (uint32_t)step);
@@ -602,6 +703,18 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
       }
       const int t2 = b + (j - D) * G;
       if (j >= D && t2 < n_tiles) {
+#ifdef EG_Q8
+        uint32_t fl = 0u, fr = 0u;
+        if (lane == 0) {
+          fl = wait_ge_value(p.flag_from_l + (size_t)t2 * EG_WARPS + warp, 2u * (uint32_t)step, p.status, p.timeout_ns);
+          fr = wait_ge_value(p.flag_from_r + (size_t)t2 * EG_WARPS + warp, 2u * (uint32_t)step, p.status, p.timeout_ns);
+        }
+        __syncwarp();
+        // the fired bits lane 0 observed, to the whole warp
+        const int sides = __shfl_sync(0xffffffffu, (int)((fl & 1u) | ((fr & 1u) << 1)), 0);
+        const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
+        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, sides);
+#else
         if (lane == 0) {
 #ifdef EG_GRAPH
 #pragma unroll
@@ -616,6 +729,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         __syncwarp();
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
         mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, slot);
+#endif
       }
     }
   }
@@ -623,7 +737,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   grid_tail(p, step, slot);
 }
 
-#if !defined(EG_DBUF) && !defined(EG_GRAPH)
+#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8)
 // (Re)compute tile partials (+ bf16 shadow) from theta (drift trigger: from theta - sent); optionally evaluate the trigger for the
 // first step.  Used once at start-up and after theta is modified outside the step kernel
 // (checkpoint restore).
@@ -727,6 +841,34 @@ cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g,
     gossip_step_kernel_graph<true><<<grid, EG_THREADS, 0, s>>>(q);
   else
     gossip_step_kernel_graph<false><<<grid, EG_THREADS, 0, s>>>(q);
+  return cudaGetLastError();
+}
+
+#elif defined(EG_Q8)   // only the step kernel + its launcher exist in this translation unit
+int gossip_q8_max_grid(int device) {
+  int sms = 0, a = 0, b = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_q8<true>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_q8<false>, EG_THREADS, 0);
+  if (b < a) a = b;
+  if (a < 1) a = 1;
+  return sms * a;
+}
+
+// int8-compressed ring step (decent/event): iter-sync fused step only.
+cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int grid, cudaStream_t s) {
+  const bool ptrs = q.q_from_l && q.q_from_r && q.s_from_l && q.s_from_r && q.q_to_l && q.q_to_r && q.s_to_l &&
+                    q.s_to_r && q.prev && q.rep_l && q.rep_r && p.flag_from_l && p.flag_from_r && p.flag_to_l &&
+                    p.flag_to_r && p.ack_from_l && p.ack_from_r && p.ack_to_l && p.ack_to_r;
+  if (p.phase != 0 || !p.sync || p.sparse != nullptr || !p.do_push || !p.do_mix || !ptrs) return cudaErrorInvalidValue;
+  Q8StepParams k;
+  static_cast<GossipParams&>(k) = p;
+  k.q = q;
+  eg_count_launch(EG_FAM_GOSSIP, 1);
+  if (p.mu != 0.f && p.mom != nullptr)
+    gossip_step_kernel_q8<true><<<grid, EG_THREADS, 0, s>>>(k);
+  else
+    gossip_step_kernel_q8<false><<<grid, EG_THREADS, 0, s>>>(k);
   return cudaGetLastError();
 }
 

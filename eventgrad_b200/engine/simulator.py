@@ -13,8 +13,8 @@ import torch
 
 from ..parallel.arena import TensorTable
 from ..parallel.topology import Graph
-from ..parallel.trigger import (TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, sgd_, topk_select,
-                                trigger_step)
+from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode,
+                                q8_encode, q8_msg_bytes, sgd_, topk_select, trigger_step)
 from .lr_schedule import lr_at
 
 
@@ -23,13 +23,19 @@ class RingSimulator:
                  tcfg: Optional[TriggerConfig] = None, lr: float = 1e-2, momentum: float = 0.0,
                  topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
                  weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
-                 offsets=(1,)):
+                 offsets=(1,), compress: str = "none"):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
         the ring.  `tcfg.metric == "drift"`: the trigger reads ||theta - sent|| per tensor, where sent[r] is what rank r's
-        receivers hold (event: zero at start, theta_k of every fired tensor at its push; spevent: prev)."""
+        receivers hold (event: zero at start, theta_k of every fired tensor at its push; spevent: prev).
+        `compress="int8"` (decent/event on the ring): a fired tensor sends the int8 code of theta - prev (q8_encode)
+        instead of theta; sender and receivers add the same dequantized delta to prev and to their replica of it, the
+        mix reads the replicas, and under drift `sent` is prev."""
         assert algo in ("cent", "decent", "event", "spevent")
+        if compress not in COMPRESS:
+            raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
+        self.q8 = compress == "int8"
         self.graphs = [Graph.build(r, world, offsets) for r in range(world)]
         self.offsets = self.graphs[0].offsets
         self.n_slots = self.graphs[0].n_slots
@@ -37,6 +43,8 @@ class RingSimulator:
         self.fanout = self.graphs[0].fanout          # messages per fired tensor
         if not self.graphs[0].is_ring and algo not in ("decent", "event"):
             raise ValueError(f"topology {offsets!r}: only decent and event gossip beyond the ring")
+        if self.q8 and (algo not in ("decent", "event") or not self.graphs[0].is_ring):
+            raise ValueError("compress int8: decent or event on the ring only")
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -57,6 +65,12 @@ class RingSimulator:
             self.prev = [p0.clone() for _ in range(world)]
             self.rep_l = [l0.clone() for _ in range(world)]
             self.rep_r = [r0.clone() for _ in range(world)]
+        elif self.q8:
+            # prev[r]: what r's neighbours hold of theta_r; rep_l / rep_r: r's replicas of its neighbours' prev.  theta_0
+            # is identical on every rank, so the receivers hold it without a message
+            self.prev = [theta0.clone() for _ in range(world)]
+            self.rep_l = [theta0.clone() for _ in range(world)]
+            self.rep_r = [theta0.clone() for _ in range(world)]
         elif algo in ("decent", "event"):
             # inbox[r][s]: what rank r last received in slot s (zero-initialised RMA window, event.cpp:144-147)
             self.inbox = [[torch.zeros_like(theta0) for _ in range(self.n_slots)] for _ in range(world)]
@@ -66,12 +80,17 @@ class RingSimulator:
         self.drift = self.tcfg.metric == "drift" and algo in ("event", "spevent")
         if self.drift:
             # what each rank's receivers hold: event -- zero like the inboxes; spevent -- prev itself (same tensors)
-            self.sent = self.prev if algo == "spevent" else [torch.zeros_like(theta0) for _ in range(world)]
+            self.sent = self.prev if (algo == "spevent" or self.q8) else [torch.zeros_like(theta0) for _ in range(world)]
 
     # ------------------------------------------------------------------
     def _flat(self, buf, i):
         t = self.table
         return buf[t.offsets[i]: t.offsets[i] + t.numels[i]]
+
+    def _padded(self, buf, i):
+        """Tensor i's whole tiles (its elements and the zero padding after them): the blocks of the int8 codec."""
+        t = self.table
+        return buf[t.offsets[i]: t.offsets[i] + t.tile_count[i] * t.tile]
 
     def _norms(self, buf):
         return torch.stack([torch.linalg.vector_norm(self._flat(buf, i))
@@ -139,6 +158,13 @@ class RingSimulator:
                     self._flat(self.rep_r[L], i)[ix] = v     # I am my left neighbour's right
                     self._flat(self.rep_l[Rn], i)[ix] = v    # and my right neighbour's left
                     self.bytes[r] += 2 * 2 * self.k[i] * 4
+                elif self.q8:
+                    pv = self._padded(self.prev[r], i)
+                    deq = q8_decode(*q8_encode(self._padded(snap[r], i) - pv))
+                    pv.add_(deq)
+                    self._padded(self.rep_r[L], i).add_(deq)    # I am my left neighbour's right
+                    self._padded(self.rep_l[Rn], i).add_(deq)   # and my right neighbour's left
+                    self.bytes[r] += 2 * q8_msg_bytes(t.numels[i])
                 else:
                     outs = self.graphs[r].out_slots()
                     if self.period:                            # one-peer graph: only this step's out-slot
@@ -150,7 +176,7 @@ class RingSimulator:
                     self.bytes[r] += n * t.numels[i] * 4
         # ---- phase 2: mix with whatever the inboxes hold, then SGD -----------------------
         for r in range(R):
-            if self.algo == "spevent":
+            if self.algo == "spevent" or self.q8:
                 mix3_(self.theta[r], self.rep_l[r], self.rep_r[r])
             elif self.period:
                 mix2_(self.theta[r], self.inbox[r][self.graphs[r].active(self.pass_num)])

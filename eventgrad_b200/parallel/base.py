@@ -55,6 +55,18 @@ def check_trigger_state(sd: Dict, metric: str, algo: str) -> None:
                          "resume with the same --trigger")
 
 
+def check_compress_state(sd: Dict, compress: str, algo: str) -> None:
+    """Refuse to resume decent / event state saved under the other --compress setting: int8 state is the public copy
+    `prev` and the neighbour replicas, dense state the inboxes.  Checkpoints without a `compress` key are dense (their
+    format predates compression)."""
+    if algo not in ("decent", "event"):
+        return
+    saved = str(sd.get("compress", "none"))
+    if saved != compress:
+        raise ValueError(f"checkpoint was written with --compress {saved}, this run uses --compress {compress}; "
+                         "resume with the same --compress")
+
+
 class CommBackend:
     name = "base"
 

@@ -10,6 +10,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
                                             (/root/reference/dcifar10/event/event.cpp:282-479)
   spevent fired tensors travel as (top-k values, indices) records; receiver scatters into
           persistent neighbour replicas      (/root/reference/dcifar10/spevent/spevent.cpp:342-542)
+  --compress int8 (decent / event, ring): fired tensors travel as int8 codes of theta - prev plus block scales;
+          both ends add the dequantized delta to prev / their replica of it, and the mix reads the replicas
 
 torch.distributed has no one-sided RMA, so the "window" is emulated with an iteration-
 synchronous exchange: first the fire masks, then a payload holding only the fired tensors.
@@ -24,9 +26,9 @@ from typing import List
 import torch
 import torch.distributed as dist
 
-from .base import CommBackend, StepLog, check_topology_state, check_trigger_state
-from .trigger import (TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, sgd_, topk_select,
-                      trigger_step)
+from .base import CommBackend, StepLog, check_compress_state, check_topology_state, check_trigger_state
+from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode, q8_encode,
+                      q8_msg_bytes, sgd_, topk_select, trigger_step)
 
 
 class CollectiveBackend(CommBackend):
@@ -44,7 +46,15 @@ class CollectiveBackend(CommBackend):
         self.bytes = 0
         self.recv_rms = cfg.dataset == "mnist"      # MNIST logs RMS, CIFAR L2 (SURVEY H5)
         gossip = cfg.algo in ("decent", "event", "spevent")
-        if gossip:
+        # --compress int8 (decent/event, ring): fired tensors travel as int8 codes of theta - prev plus one scale per
+        # block; prev and the neighbour replicas start from theta_0 (identical on all ranks), the mix reads the replicas
+        self.compress = getattr(cfg, "compress", "none")
+        self.q8 = gossip and self.compress == "int8"
+        if self.q8:
+            self.prev = arena.theta.clone()
+            self.rep_l = arena.theta.clone()
+            self.rep_r = arena.theta.clone()
+        elif gossip:
             if cfg.algo == "spevent":
                 # Q8: replicas / prev start from theta_0 (identical on all ranks), not fresh random nets
                 self.prev = arena.theta.clone()
@@ -62,7 +72,7 @@ class CollectiveBackend(CommBackend):
         # every fired tensor afterwards; spevent: prev, which the top-k pushes already keep element-wise)
         self.drift = cfg.algo in ("event", "spevent") and self.tcfg.metric == "drift"
         if self.drift:
-            self.sent = self.prev if cfg.algo == "spevent" else torch.zeros_like(arena.theta)
+            self.sent = self.prev if (cfg.algo == "spevent" or self.q8) else torch.zeros_like(arena.theta)
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
             self.last_recv_norm_l, self.last_recv_norm_r = z(), z()
@@ -161,6 +171,8 @@ class CollectiveBackend(CommBackend):
 
     def _step_decent(self) -> None:
         a = self.arena
+        if self.q8:
+            return self._step_q8([True] * a.table.n_tensors, None)
         if hasattr(self, "inbox"):
             self._exchange_slots(a.theta, self.inbox)
             self.bytes += self.ring.fanout * a.table.n_elems * 4
@@ -224,9 +236,53 @@ class CollectiveBackend(CommBackend):
         self._mix_slots()
         self._opt()
 
+    def _padded(self, buf, i):
+        """Tensor i's whole tiles: the blocks of the int8 codec (parallel/trigger.py q8_encode)."""
+        t = self.arena.table
+        return buf[t.offsets[i]: t.offsets[i] + t.tile_count[i] * t.tile]
+
+    def _step_q8(self, mine, masks) -> None:
+        """int8 ring step: my fired tensors' codes of theta - prev and their block scales go to both neighbours (decent:
+        every tensor; event: after the fire-mask exchange, `masks` = (left's, right's)); each side adds the dequantized
+        delta to prev / to its replica of the sender's prev, then theta <- ((theta + rep_l) + rep_r) / 3 and SGD."""
+        a, t = self.arena, self.arena.table
+        lm, rm = masks if masks is not None else (mine, mine)
+        qs, ss = [], []
+        for i in range(t.n_tensors):
+            if mine[i]:
+                pv = self._padded(self.prev, i)
+                q, s = q8_encode(self._padded(a.theta, i) - pv)
+                pv.add_(q8_decode(q, s))
+                qs.append(q)
+                ss.append(s)
+                self.bytes += 2 * q8_msg_bytes(t.numels[i])
+        pq = torch.cat(qs) if qs else torch.empty(0, dtype=torch.int8, device=a.theta.device)
+        ps = torch.cat(ss) if ss else a.theta.new_empty(0)
+        blocks = [t.tile_count[i] * t.tile for i in range(t.n_tensors)]
+        nl = sum(blocks[i] for i in range(t.n_tensors) if lm[i])
+        nr = sum(blocks[i] for i in range(t.n_tensors) if rm[i])
+        ql, qr = torch.empty(nl, dtype=torch.int8, device=a.theta.device), torch.empty(nr, dtype=torch.int8,
+                                                                                       device=a.theta.device)
+        sl, sr = a.theta.new_empty(nl // Q8_BLOCK), a.theta.new_empty(nr // Q8_BLOCK)
+        self._exchange([pq, ps], [pq, ps], [ql, sl], [qr, sr])
+        for mask, qb, sb, rep in ((lm, ql, sl, self.rep_l), (rm, qr, sr, self.rep_r)):
+            off = 0
+            for i in range(t.n_tensors):
+                if mask[i]:
+                    n = blocks[i]
+                    self._padded(rep, i).add_(q8_decode(qb[off:off + n], sb[off // Q8_BLOCK:(off + n) // Q8_BLOCK]))
+                    off += n
+        mix3_(a.theta, self.rep_l, self.rep_r)
+        self._opt()
+
     def _step_event(self) -> None:
         if hasattr(self, "inbox"):
             return self._step_event_graph()
+        if self.q8:
+            _, fire = self._fire()
+            mine, lm, rm = self._masks(fire)
+            self.events += 2 * sum(mine)
+            return self._step_q8(mine, (lm, rm))
         a, t = self.arena, self.arena.table
         thres_used = None
         if self.want_logs:
@@ -348,9 +404,11 @@ class CollectiveBackend(CommBackend):
         for k in ("inbox_l", "inbox_r", "prev", "rep_l", "rep_r"):
             if hasattr(self, k):
                 sd[k] = getattr(self, k).cpu().clone()
+        if self.cfg.algo in ("decent", "event"):
+            sd["compress"] = self.compress          # int8: prev / rep_l / rep_r are saved above
         if self.cfg.algo in ("event", "spevent"):
             sd["trigger"] = self.tcfg.metric
-            if self.drift and self.cfg.algo == "event":
+            if self.drift and self.cfg.algo == "event" and not self.q8:
                 sd["sent"] = self.sent.cpu().clone()
         if hasattr(self, "inbox"):
             sd["topology_offsets"] = list(self.ring.offsets)
@@ -366,8 +424,9 @@ class CollectiveBackend(CommBackend):
         self.bytes = int(sd.get("bytes", 0))
         check_topology_state(sd, self.ring, self.cfg.algo)
         check_trigger_state(sd, self.tcfg.metric, self.cfg.algo)
+        check_compress_state(sd, self.compress, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
-        if self.drift and self.cfg.algo == "event":
+        if self.drift and self.cfg.algo == "event" and not self.q8:
             self.sent.copy_(sd["sent"].to(self.sent.device))
         if hasattr(self, "inbox"):
             for s, ib in enumerate(self.inbox):

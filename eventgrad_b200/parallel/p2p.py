@@ -8,6 +8,8 @@ Per training step, after backward():
            (t+s_m)/2 -> SGD, same kernel)
   event    ONE launch: as decent, but a tensor is pushed only if its device-resident trigger fired;
            the same kernel accumulates the norms and runs the trigger FSM for the next step
+           (--compress int8, ring: csrc/gossip_q8.cu pushes the int8 code of theta - prev + block scales, the receivers
+           add the delta to their replicas of prev, and the mix reads the replicas)
   spevent  batched segmented radix-select top-k + compaction straight into the neighbours'
            inboxes, scatter of arrived records into replicas, then the dense mix+SGD kernel
 No NCCL/MPI call, no separate elementwise kernel and no host synchronisation on that path
@@ -20,8 +22,9 @@ from typing import List
 import torch
 
 from .arena import TILE, ParamArena, TensorTable
-from .base import CommBackend, StepLog, check_topology_state, check_trigger_state
+from .base import CommBackend, StepLog, check_compress_state, check_topology_state, check_trigger_state
 from .topology import Graph
+from .trigger import q8_msg_bytes
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
 
 ONE_SHOT_MAX_BYTES = 512 * 1024        # above this the all-reduce switches to two-shot
@@ -44,7 +47,13 @@ def _wants_dbuf(cfg) -> bool:
     only; there it is the default (double_buffer=None), `--no-double-buffer` selects the single-slot + ack protocol."""
     db = getattr(cfg, "double_buffer", None)
     return ((db is None or bool(db)) and cfg.algo == "decent" and cfg.sync_mode == "iter"
-            and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True))
+            and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True)
+            and not _wants_q8(cfg))
+
+
+def _wants_q8(cfg) -> bool:
+    """--compress int8: decent/event on the ring run the int8 step of csrc/gossip_q8.cu."""
+    return getattr(cfg, "compress", "none") == "int8" and cfg.algo in ("decent", "event")
 
 
 def _graph_of(cfg, rank: int, world: int):
@@ -68,7 +77,13 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None)
             lay.add(f"ack_from_{k}", 256)
         lay.add("ar_flags", 3 * max_grid * world * 4)
         return lay
-    if cfg.algo in ("decent", "event"):
+    if _wants_q8(cfg):
+        # int8 codes (one byte per arena element) and one fp32 scale per (tile, warp) block from each neighbour
+        lay.add("q_from_l", table.n_padded)
+        lay.add("q_from_r", table.n_padded)
+        lay.add("qs_from_l", table.n_tiles * 8 * 4)
+        lay.add("qs_from_r", table.n_tiles * 8 * 4)
+    elif cfg.algo in ("decent", "event"):
         slots = 2 if _wants_dbuf(cfg) else 1      # double-buffered decent: slot = step & 1
         lay.add("inbox_l", n * slots)
         lay.add("inbox_r", n * slots)
@@ -102,6 +117,8 @@ def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
         max_grid = min(max_grid, C.gossip_dbuf_max_grid(env.device.index or 0))
     if graph is not None:
         max_grid = min(max_grid, C.gossip_graph_max_grid(env.device.index or 0))
+    if _wants_q8(cfg):
+        max_grid = min(max_grid, C.gossip_q8_max_grid(env.device.index or 0))
     lay = build_layout(table, cfg, env.world, max_grid, graph)
     symm = wants_symm_window(env) and bootstrap is None      # NVLS path: torch symmetric memory + multicast mapping
     win = (SymmWindow if symm else Window)(lay, env.rank, env.world, env.device)
@@ -148,6 +165,11 @@ class P2PBackend(CommBackend):
         # split step: everything that depends only on theta_k (pushes / top-k records) is launched on a
         # side stream at the start of the step and overlaps forward+backward
         self.overlap = bool(getattr(cfg, "overlap_push", False)) and self.do_comm
+        # --compress int8: the iter-sync fused ring step of csrc/gossip_q8.cu
+        self.q8 = _wants_q8(cfg)
+        if self.q8 and (self.graph is not None or self.overlap or getattr(cfg, "ce_push", False) or self.want_logs
+                        or not self.sync):
+            raise ValueError("p2p backend: --compress int8 runs decent/event on the ring's fused iter-sync step only")
         self.dbuf = _wants_dbuf(cfg) and self.do_comm
         self.ce_push = bool(getattr(cfg, "ce_push", False)) and self.overlap and cfg.algo == "decent" and self.sync
         self.nvls = self.nvls_step = False      # set in connect() when the window has a multicast mapping
@@ -170,6 +192,8 @@ class P2PBackend(CommBackend):
                 acc += 2 * k
             self.K = sum(self.k)
             self.d_k, self.d_rec_off = i32(self.k), i32(rec_off)
+        elif self.q8:
+            msg = [q8_msg_bytes(n) for n in t.numels]     # int8 codes of the real elements + the blocks' scales
         else:
             msg = [n * 4 for n in t.numels]
         self.msg_bytes = msg
@@ -208,6 +232,12 @@ class P2PBackend(CommBackend):
             self.desc = torch.zeros(t.n_tiles, dtype=torch.int64, device=dev)       # look-back descriptors
             self.sp_bar = zi(4)
             self.applied_l, self.applied_r = zi(t.n_tensors), zi(t.n_tensors)
+        if self.q8:
+            # the public copy of my theta and my replicas of the neighbours' copies, all theta_0 (identical on all
+            # ranks, so the receivers hold it without a message)
+            self.prev = arena.theta.clone()
+            self.rep_l = arena.theta.clone()
+            self.rep_r = arena.theta.clone()
         # drift trigger (--trigger drift): the FSM reads ||theta - sent||.  event: `sent` is an arena-sized buffer,
         # zero like the receivers' inboxes, that the step kernel's pushes keep equal to what was last pushed; spevent:
         # `prev` already is what the receivers hold, element by element
@@ -215,7 +245,7 @@ class P2PBackend(CommBackend):
         self.drift = self.metric == "drift" and cfg.algo in ("event", "spevent")
         self.sent = None
         if self.drift:
-            self.sent = self.prev if self.sparse else zf(t.n_padded)
+            self.sent = self.prev if (self.sparse or self.q8) else zf(t.n_padded)
         self.ar_ctr = zi(1)
         # gradient pointer table (table mode): device arrays + rotating pinned staging
         self.table_mode = bool(getattr(arena, "table_mode", False)) and cfg.algo != "cent"
@@ -226,7 +256,7 @@ class P2PBackend(CommBackend):
         self._grads_alive = None
         self.host_bytes = 0
         self._connected = False
-        self.gp = self.ap = self.ap_avg = self.sp = self.gs = None
+        self.gp = self.ap = self.ap_avg = self.sp = self.gs = self.qs = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
@@ -311,7 +341,19 @@ class P2PBackend(CommBackend):
                     "ack_to": [win.addr(f"ack_from_{s}", ins[s]) for s in range(n)],
                 })
                 self.gs = gs
-            if dense and self.graph is None:
+            if self.q8:
+                # I am my left neighbour's right and my right neighbour's left.  R = 2: the one neighbour gets two
+                # copies in two inboxes and keeps two replicas (no wire dedup)
+                qs = C.Q8Slots()
+                qs.update({
+                    "q_from_l": win.addr("q_from_l"), "q_from_r": win.addr("q_from_r"),
+                    "s_from_l": win.addr("qs_from_l"), "s_from_r": win.addr("qs_from_r"),
+                    "q_to_l": win.addr("q_from_r", L), "q_to_r": win.addr("q_from_l", R),
+                    "s_to_l": win.addr("qs_from_r", L), "s_to_r": win.addr("qs_from_l", R),
+                    "prev": P(self.prev), "rep_l": P(self.rep_l), "rep_r": P(self.rep_r),
+                })
+                self.qs = qs
+            elif dense and self.graph is None:
                 gp.update({"inbox_l": win.addr("inbox_l"), "inbox_r": win.addr("inbox_r"),
                            "push_l": win.addr("inbox_r", L), "push_r": win.addr("inbox_l", R)})
                 # 2-rank ring: left == right.  Push theta ONCE (into the peer's inbox_r) and let the peer read that
@@ -499,6 +541,8 @@ class P2PBackend(CommBackend):
                 if not self.overlap:
                     C.sparse_select_push(self.sp, self.grid, s)        # 3 launches: hist, candidates, compaction
                 C.gossip_step(self.gp, self.grid, s)                   # receive prologue + mix + SGD + trigger
+            elif self.q8 and self.do_comm:
+                C.gossip_step_q8(self.gp, self.qs, self.grid, s)
             elif self.overlap:
                 C.gossip_step_phase(self.gp, 2, self.grid, s)
             elif self.dbuf:
@@ -513,6 +557,8 @@ class P2PBackend(CommBackend):
         self.pass_num += 1
         if self.cfg.algo == "cent" and self.ring.world > 1:
             self.host_bytes += self.table.n_elems * 4
+        elif self.cfg.algo == "decent" and self.do_comm and self.q8:
+            self.host_bytes += 2 * sum(self.msg_bytes)
         elif self.cfg.algo == "decent" and self.do_comm:
             self.host_bytes += getattr(self.ring, "fanout", 2) * self.table.n_elems * 4
 
@@ -591,21 +637,24 @@ class P2PBackend(CommBackend):
                 sd["topology"] = self.graph.kind
             for k in range(self.graph.n_slots):
                 sd[f"inbox_{k}"] = self.win.view(f"inbox_{k}", torch.float32).cpu().clone()
-        elif self.cfg.algo in ("decent", "event"):
+        elif self.cfg.algo in ("decent", "event") and not self.q8:
             sd["inbox_l"] = self.win.view("inbox_l", torch.float32).cpu().clone()
             sd["inbox_r"] = self.win.view("inbox_r", torch.float32).cpu().clone()
-        if self.sparse:
+        if self.cfg.algo in ("decent", "event"):
+            sd["compress"] = "int8" if self.q8 else "none"
+        if self.sparse or self.q8:
             for k in ("prev", "rep_l", "rep_r"):
                 sd[k] = getattr(self, k).cpu().clone()
         if self.cfg.algo in ("event", "spevent"):
             sd["trigger"] = self.metric
-            if self.drift and not self.sparse:
+            if self.drift and not self.sparse and not self.q8:
                 sd["sent"] = self.sent.cpu().clone()
         return sd
 
     def load_state_dict(self, sd):
         check_topology_state(sd, self.ring, self.cfg.algo)
         check_trigger_state(sd, self.metric, self.cfg.algo)
+        check_compress_state(sd, "int8" if self.q8 else "none", self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
@@ -616,10 +665,10 @@ class P2PBackend(CommBackend):
         elif "inbox_l" in sd and self.cfg.algo in ("decent", "event"):
             self.win.view("inbox_l", torch.float32).copy_(sd["inbox_l"].to(self.dev))
             self.win.view("inbox_r", torch.float32).copy_(sd["inbox_r"].to(self.dev))
-        if self.sparse:
+        if self.sparse or self.q8:
             for k in ("prev", "rep_l", "rep_r"):
                 getattr(self, k).copy_(sd[k].to(self.dev))
-        if self.drift and not self.sparse:
+        if self.drift and not self.sparse and not self.q8:
             self.sent.copy_(sd["sent"].to(self.dev))
         if self.log_ring is not None:
             self._drained = self.pass_num          # log rows of the steps before the checkpoint are not replayed
@@ -637,6 +686,10 @@ class P2PBackend(CommBackend):
             return
         for name in ("flag_from_l", "flag_from_r", "ack_from_l", "ack_from_r", "pushed_from_l", "pushed_from_r"):
             self.win.view(name, torch.int32).fill_(step)
+        if self.q8:
+            # the q8 kernel's (tile, warp) flags carry 2 * step + fired (PROTOCOL.md 1.7)
+            for name in ("flag_from_l", "flag_from_r"):
+                self.win.view(name, torch.int32).fill_(2 * step)
         if self.sparse:
             for name in ("done_from_l", "done_from_r"):
                 self.win.view(name, torch.int32).fill_(step)

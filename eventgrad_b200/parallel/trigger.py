@@ -145,6 +145,38 @@ def sgd_(theta: torch.Tensor, grad: torch.Tensor, mom, lr: float, mu: float, wd:
     theta.add_(d, alpha=-lr)
 
 
+Q8_BLOCK = 256          # elements per int8 scale: one warp's slice of a 2048-float tile (never straddles tensors)
+COMPRESS = ("none", "int8")
+
+
+def q8_msg_bytes(numel: int) -> int:
+    """Logical bytes of one tensor's int8 message: one code per real element + one fp32 scale per block holding any."""
+    return numel + 4 * (-(-numel // Q8_BLOCK))
+
+
+@torch.no_grad()
+def q8_encode(d: torch.Tensor):
+    """int8 code of a padded flat arena d (length a multiple of Q8_BLOCK), one fp32 scale per block of Q8_BLOCK:
+        a = max |d| ; s = a / 127 ; q = s == 0 ? 0 : clamp(rint(d / s), -127, 127)
+    IEEE fp32 with round to nearest even throughout, so it matches the q8 step kernel (csrc/gossip.cu, EG_Q8) bit for
+    bit.  Both divisions are tensor / tensor: a division by a Python scalar may become a multiply by its reciprocal.
+    Returns (q int8 [n], s fp32 [n / Q8_BLOCK])."""
+    b = d.reshape(-1, Q8_BLOCK).to(torch.float32)
+    a = b.abs().amax(dim=1)
+    s = a / torch.full_like(a, 127.0)
+    zero = s == 0
+    safe = torch.where(zero, torch.ones_like(s), s)
+    q = torch.round(b / safe[:, None]).clamp_(-127.0, 127.0)
+    q = torch.where(zero[:, None], torch.zeros_like(q), q)
+    return q.to(torch.int8).reshape(-1), s
+
+
+@torch.no_grad()
+def q8_decode(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """deq = (float)q * s per block (one rounded multiply): the delta both ends add to prev / their replica."""
+    return (q.reshape(-1, Q8_BLOCK).to(torch.float32) * s.reshape(-1, 1)).reshape(-1)
+
+
 @torch.no_grad()
 def topk_select(theta_flat: torch.Tensor, prev_flat: torch.Tensor, k: int):
     """k indices with the largest |theta - prev| (spevent.cpp:346-349). Ties are broken

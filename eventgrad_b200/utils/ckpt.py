@@ -4,7 +4,9 @@
 One file per rank: arena (theta + momentum, with its layout), the backend's communication state (trigger FSM,
 inboxes / sparse replicas, event counters, pass_num; on a gossip graph every slot's inbox, the offsets and, for
 onepeer-exp, the topology name, checked on resume by parallel/base.py; event/spevent: the trigger name, and under
---trigger drift event's `sent` buffer, also checked on resume), BN buffers, RNG state (global + the loader's
+--trigger drift event's `sent` buffer, also checked on resume; decent/event: the `compress` setting, and under
+--compress int8 `prev` and the neighbour replicas `rep_l` / `rep_r` instead of the inboxes, checked on resume by
+check_compress_state), BN buffers, RNG state (global + the loader's
 private augmentation generator), step counter and epoch.  Only tensors / numbers / strings / lists / dicts are stored, so
 files are read back with `weights_only=True` (no pickle code execution from a user-supplied --resume path).  The
 ranks' models differ between consensus rounds, so a decentralized run can only be resumed
