@@ -78,9 +78,13 @@ class TrainConfig:
                                      # (circulant offsets, at most 4); decent/event only beyond the ring
     compress: str = "none"           # none | int8: decent/event on the ring send the int8 code of theta - prev (one fp32
                                      # scale per 256 elements) with error feedback instead of fp32 theta
+    gradient_tracking: bool = False  # decent on the ring: also gossip y, which tracks the average gradient, and step
+                                     # along y instead of the local gradient (DSGT / DIGing; fused single-slot step)
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
+    partition: str = "iid"           # iid (a block of a random / the identity order) | label (shards cut from the
+                                     # samples sorted by class: heterogeneous, still equal-sized)
     augment: bool = True             # pad4 + flip + crop (cifar only)
     native_loader: str = "auto"      # auto (CPU: native C++ prefetcher, CUDA: Python staging) | on | off
     train_samples: int = 50000
@@ -185,6 +189,29 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError("--compress int8 does not support file_write: the reference's log format records "
                                  "the received fp32 tensors")
+        if self.gradient_tracking:
+            # the tracking step exists as the iter-sync fused single-slot ring step (csrc/gossip_gt.cu), in the
+            # torch.distributed backends and in the simulator; sum_r y_r = sum_r g_r holds only if every y a rank mixes
+            # is its neighbour's current one
+            if self.algo in ("event", "spevent"):
+                raise ValueError(f"--gradient-tracking needs algo decent, got {self.algo!r}: a held tensor leaves the "
+                                 "neighbours mixing a stale y, which breaks sum(y) = sum(g)")
+            if self.algo != "decent":
+                raise ValueError(f"--gradient-tracking needs algo decent, got {self.algo!r}")
+            if not self.ring_topology:
+                raise ValueError(f"--gradient-tracking runs on the ring only, got topology {self.topology!r}")
+            if self.backend == "refport":
+                raise ValueError("--gradient-tracking is not supported by --backend refport")
+            for name in ("overlap_push", "double_buffer", "ce_push"):
+                if getattr(self, name):
+                    raise ValueError(f"--gradient-tracking does not support {name} (fused single-slot step only)")
+            if self.compress != "none":
+                raise ValueError("--gradient-tracking does not support --compress int8")
+            if self.file_write:
+                raise ValueError("--gradient-tracking does not support file_write: the reference's log format has no "
+                                 "column for y")
+        if self.partition not in ("iid", "label"):
+            raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
 
     @property
@@ -231,7 +258,8 @@ class TrainConfig:
             kw["cuda_graph"] = cuda
         if c.overlap_push is None:
             kw["overlap_push"] = bool(cuda and p2p and world >= 2 and c.algo in ("decent", "event")
-                                      and not bool(c.double_buffer) and c.ring_topology and c.compress == "none")
+                                      and not bool(c.double_buffer) and c.ring_topology and c.compress == "none"
+                                      and not c.gradient_tracking)
         return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
@@ -307,11 +335,17 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--compress", default=None, choices=["none", "int8"],
                    help="decent/event on the ring: send the int8 code of theta - (what the neighbours hold) with one "
                         "fp32 scale per 256 elements, about a quarter of the fp32 bytes (default none)")
+    p.add_argument("--gradient-tracking", action="store_true", default=None,
+                   help="decent on the ring: also gossip y, a running estimate of the average gradient, and step along "
+                        "it (DSGT): removes the bias of constant-lr D-PSGD under heterogeneous data")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)
     p.add_argument("--data", default=None, help="'synthetic' or dataset root directory")
     p.add_argument("--sampler", default=None, choices=["random", "sequential"])
+    p.add_argument("--partition", default=None, choices=["iid", "label"],
+                   help="data shards: iid (default) or label (cut from the samples sorted by class: each rank sees few "
+                        "classes, every shard has the same size)")
     p.add_argument("--no-augment", dest="augment", action="store_false", default=None)
     p.add_argument("--native-loader", default=None, choices=["auto", "on", "off"])
     p.add_argument("--train-samples", type=int, default=None)

@@ -153,6 +153,22 @@ struct Q8Slots {
   float* rep_r;
 };
 
+// Gradient tracking for decent on the ring (csrc/gossip_gt.cu, --gradient-tracking): a separate block passed to the
+// tracking kernel next to GossipParams, which keeps its ring inbox / push / flag / ack pointers for theta.  Each rank
+// also gossips y, which tracks the average gradient, and steps along it:
+//   push  theta_k and y_{k-1} to both neighbours (same thread, before the same (tile, warp) flag)
+//   y_k = ((y_{k-1} + yL) + yR) / 3 + (g_k - g_{k-1}),  g_prev <- g_k,  theta' = ((theta_k + L) + R) / 3,
+//   theta_{k+1} = sgd_elem(theta', y_k, ...)
+// 2-rank ring: y_to_r is null and y_in_l == y_in_r, exactly as push_r / inbox_l of the single-copy wire dedup.
+struct TrackSlots {
+  float* y;                 // local: y_{k-1} before the step, y_k after it
+  float* g_prev;            // local: the gradient of the previous step (fp32, also when the gradient is bf16)
+  const float* y_in_l;      // local: y last pushed by my LEFT neighbour
+  const float* y_in_r;
+  float* y_to_l;            // peer-mapped: LEFT neighbour's y_in_r
+  float* y_to_r;            // peer-mapped: RIGHT neighbour's y_in_l (null on the 2-rank ring)
+};
+
 int gossip_max_grid(int device);  // co-resident CTAs (persistent grid upper bound)
 cudaError_t launch_gossip_step(const GossipParams& p, int grid, cudaStream_t s);
 // experimental double-buffered dense variant (csrc/gossip_dbuf.cu): inbox_l/inbox_r/push_l/push_r address
@@ -171,6 +187,11 @@ cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g,
 // (tile, warp) carries 2*step + fired (PROTOCOL.md 1.7)
 int gossip_q8_max_grid(int device);
 cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int grid, cudaStream_t s);
+// gradient-tracking ring step (csrc/gossip_gt.cu): the fused single-kernel decent step that also gossips y and steps
+// along it; requires phase 0, sync, do_push and do_mix, no sparse block, no `sent`, the ring's inbox / push / flag /
+// ack pointers and every pointer of `y` (y_to_r null exactly when push_r is null)
+int gossip_gt_max_grid(int device);
+cudaError_t launch_gossip_step_gt(const GossipParams& p, const TrackSlots& y, int grid, cudaStream_t s);
 // (re)compute tile_ss (+ shadow) from theta and evaluate the trigger for step pass_num+1.
 cudaError_t launch_gossip_init(const GossipParams& p, int grid, int run_fsm, cudaStream_t s);
 // Trigger FSM alone with externally supplied norms (unit tests against the oracle).

@@ -86,6 +86,11 @@ static const std::unordered_map<std::string, Setter<Q8Slots>> kQ8 = {
     PTRF(Q8Slots, prev), PTRF(Q8Slots, rep_l), PTRF(Q8Slots, rep_r),
 };
 
+static const std::unordered_map<std::string, Setter<TrackSlots>> kTrack = {
+    PTRF(TrackSlots, y), PTRF(TrackSlots, g_prev), PTRF(TrackSlots, y_in_l), PTRF(TrackSlots, y_in_r),
+    PTRF(TrackSlots, y_to_l), PTRF(TrackSlots, y_to_r),
+};
+
 static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce = {
     PTRF(AllReduceParams, peer_bufs), PTRF(AllReduceParams, local), PTRF(AllReduceParams, theta),
     PTRF(AllReduceParams, mom), PTRF(AllReduceParams, shadow), PTRF(AllReduceParams, peer_flags),
@@ -172,6 +177,7 @@ PYBIND11_MODULE(_C, m) {
   bind_params<GossipParams>(m, "GossipParams", kGossip);
   bind_params<GraphSlots>(m, "GraphSlots", kGraph);
   bind_params<Q8Slots>(m, "Q8Slots", kQ8);
+  bind_params<TrackSlots>(m, "TrackSlots", kTrack);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
   bind_params<SparseParams>(m, "SparseParams", kSparse);
   bind_params<BnParams>(m, "BnParams", kBn);
@@ -197,6 +203,10 @@ PYBIND11_MODULE(_C, m) {
   m.def("gossip_q8_max_grid", &gossip_q8_max_grid);
   m.def("gossip_step_q8", [](const GossipParams& p, const Q8Slots& q, int grid, uintptr_t s) {
     check(launch_gossip_step_q8(p, q, grid, S(s)), "gossip_step_q8");
+  });
+  m.def("gossip_gt_max_grid", &gossip_gt_max_grid);
+  m.def("gossip_step_gt", [](const GossipParams& p, const TrackSlots& y, int grid, uintptr_t s) {
+    check(launch_gossip_step_gt(p, y, grid, S(s)), "gossip_step_gt");
   });
   m.def("gossip_init", [](const GossipParams& p, int grid, int run_fsm, uintptr_t s) {
     check(launch_gossip_init(p, grid, run_fsm, S(s)), "gossip_init");

@@ -44,6 +44,12 @@
 // Q8Slots block, and adds the dequantized delta to `prev`.  The (tile, warp) flag carries 2*step + fired, so the
 // receiver learns from the flag whether to add the neighbour's delta to its replica before the mix
 // ((theta + rep_l) + rep_r) / 3.  Under the drift trigger GossipParams.sent is `prev`.
+// csrc/gossip_gt.cu defines EG_GT and includes it a fifth time for gradient tracking (`gossip_step_kernel_gt`, decent
+// on the ring, iter-sync fused step only): next to theta_k, the same thread pushes y_{k-1} of its slice into the
+// neighbours' y inboxes of the TrackSlots block before the unchanged (tile, warp) flag, and the mix forms
+// y_k = ((y + yL) + yR) / 3 + (g_k - g_prev) first, stores y and g_prev, mixes theta and hands y_k to sgd_elem in place
+// of the gradient.  The ack of step k covers both inboxes, so there is no new synchronisation variable
+// (PROTOCOL.md 1.8).
 #include "api.h"
 #include "common.cuh"
 #include "sparse_apply.cuh"
@@ -59,6 +65,11 @@ struct Q8StepParams : GossipParams {      // kernel parameter of the q8 build: t
   Q8Slots q;
 };
 using StepParams = Q8StepParams;
+#elif defined(EG_GT)
+struct GtStepParams : GossipParams {      // kernel parameter of the tracking build: the ring block + the y slots
+  TrackSlots gt;
+};
+using StepParams = GtStepParams;
 #else
 using StepParams = GossipParams;
 #endif
@@ -72,6 +83,9 @@ using StepParams = GossipParams;
 #define EG_SLOT_OFF(p, step) ((size_t)0)
 #elif defined(EG_Q8)
 #define EG_SYM(name) name##_q8
+#define EG_SLOT_OFF(p, step) ((size_t)0)
+#elif defined(EG_GT)
+#define EG_SYM(name) name##_gt
 #define EG_SLOT_OFF(p, step) ((size_t)0)
 #else
 #define EG_SYM(name) name
@@ -312,6 +326,19 @@ __device__ __forceinline__ uint32_t wait_ge_value(const uint32_t* flag, uint32_t
   wait_ge(flag, want, status, timeout_ns);
   return ld_acquire_sys(flag);
 }
+#elif defined(EG_GT)
+// theta_k and y_{k-1} of this thread's 8 elements to both neighbours, both before the (tile, warp) flag.  The thread
+// that later mixes this slice overwrites y with y_k only after this load (program order), so no new ordering is needed.
+// push_r == nullptr: 2-rank ring, one copy of each (y_to_r is null too)
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
+  const F8 y = ld_f8(p.gt.y + base);
+  st_f8(p.push_l + base, th);
+  st_f8(p.gt.y_to_l + base, y);
+  if (p.push_r != nullptr) {
+    st_f8(p.push_r + base, th);
+    st_f8(p.gt.y_to_r + base, y);
+  }
+}
 #else
 __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
   // push_r == nullptr: 2-rank ring, the one neighbour is both left and right and reads the single copy twice
@@ -438,6 +465,34 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
   th = q8_recv_add(p.q.rep_r, p.q.q_from_r, p.q.s_from_r, base, th, (slot & 2) != 0);
 #pragma unroll
   for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(th.v[e], 3.0f);
+#elif defined(EG_GT)
+  // staged so the gradient registers die before theta and its inboxes are loaded (the caller passes no theta): (1) g,
+  // g_prev -> g - g_prev, g_prev <- g; y, yL, yR -> y_k, stored; (2) theta and its inboxes, mix; (3) sgd_elem on y_k
+  // (held in `g`, the optimizer's input)
+  constexpr bool logrecv = false;
+  float ssl = 0.f, ssr = 0.f;
+  F8 g, m;
+  {
+    const F8 gk = load_grad(p, ti, base, threadIdx.x);
+    const F8 gp = ld_f8(p.gt.g_prev + base);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) g.v[e] = __fsub_rn(gk.v[e], gp.v[e]);
+    st_f8(p.gt.g_prev + base, gk);
+  }
+  {
+    const F8 y = ld_f8(p.gt.y + base), yl = ld_f8_cg(p.gt.y_in_l + base), yr = ld_f8_cg(p.gt.y_in_r + base);
+#pragma unroll
+    for (int e = 0; e < 8; ++e)
+      g.v[e] = __fadd_rn(__fdiv_rn(__fadd_rn(__fadd_rn(y.v[e], yl.v[e]), yr.v[e]), 3.0f), g.v[e]);
+    st_f8(p.gt.y + base, g);
+  }
+  {
+    th = ld_f8(p.theta + base);
+    const F8 L = ld_f8_cg(p.inbox_l + base), R = ld_f8_cg(p.inbox_r + base);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(__fadd_rn(__fadd_rn(th.v[e], L.v[e]), R.v[e]), 3.0f);
+  }
+  if (kMom) m = ld_f8(p.mom + base);
 #else
   const bool logrecv = (p.tile_ss_l != nullptr);
   float ssl = 0.f, ssr = 0.f;
@@ -482,7 +537,7 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
     for (int e = 0; e < 8; ++e) z.v[e] = 0.f;
     st_f8(p.grad + base, z);
   }
-#ifndef EG_DBUF
+#if !defined(EG_DBUF) && !defined(EG_GT)
   if (p.sent != nullptr) {
     // drift trigger: sum (theta_{k+1} - sent)^2 replaces sum theta_{k+1}^2.  sent was stored by this thread's push of
     // this tile (or by the split step's push phase / the sparse compaction, both stream-ordered before this kernel)
@@ -596,7 +651,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   // when it reads the status word.  (Uniform per CTA; the run is over, so a partial step does not matter.)
   if (p.do_push && *reinterpret_cast<volatile int*>(p.status) != EG_OK) return;
 
-#if defined(EG_DBUF) || defined(EG_Q8)
+#if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT)
   if (p.phase != 0 || !(p.sync && push)) return;   // the launcher rejects these; never reached
 #elif defined(EG_GRAPH)
   if (p.phase != 0) return;                        // fused step only (the launcher rejects the rest)
@@ -608,7 +663,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #endif
   __shared__ TileInfo s_ti[EG_TI_CACHE];
   fill_tile_cache(p, s_ti);
-#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8)
+#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT)
   // spevent: receive side first -- scatter the records that arrived for this step into the replicas
   // (inbox_l / inbox_r point at them), grid barrier, then the dense mix below reads them tile by tile
   if (p.sparse != nullptr) sparse_apply_prologue(*p.sparse, p.sparse->bar);
@@ -728,7 +783,12 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         }
         __syncwarp();
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
+#ifdef EG_GT
+        // the tracking mix loads theta itself, after the y stage: held from here it would spill
+        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot);
+#else
         mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, slot);
+#endif
 #endif
       }
     }
@@ -737,7 +797,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   grid_tail(p, step, slot);
 }
 
-#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8)
+#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT)
 // (Re)compute tile partials (+ bf16 shadow) from theta (drift trigger: from theta - sent); optionally evaluate the trigger for the
 // first step.  Used once at start-up and after theta is modified outside the step kernel
 // (checkpoint restore).
@@ -869,6 +929,37 @@ cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int g
     gossip_step_kernel_q8<true><<<grid, EG_THREADS, 0, s>>>(k);
   else
     gossip_step_kernel_q8<false><<<grid, EG_THREADS, 0, s>>>(k);
+  return cudaGetLastError();
+}
+
+#elif defined(EG_GT)   // only the step kernel + its launcher exist in this translation unit
+int gossip_gt_max_grid(int device) {
+  int sms = 0, a = 0, b = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_gt<true>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_gt<false>, EG_THREADS, 0);
+  if (b < a) a = b;
+  if (a < 1) a = 1;
+  return sms * a;
+}
+
+// Gradient-tracking ring step (decent): iter-sync fused step only, every tensor pushed every step.
+cudaError_t launch_gossip_step_gt(const GossipParams& p, const TrackSlots& y, int grid, cudaStream_t s) {
+  const bool ptrs = y.y && y.g_prev && y.y_in_l && y.y_in_r && y.y_to_l &&
+                    (y.y_to_r == nullptr) == (p.push_r == nullptr) && p.inbox_l && p.inbox_r && p.push_l &&
+                    p.flag_from_l && p.flag_from_r && p.flag_to_l && p.flag_to_r && p.ack_from_l && p.ack_from_r &&
+                    p.ack_to_l && p.ack_to_r;
+  if (p.phase != 0 || !p.sync || p.sparse != nullptr || p.sent != nullptr || p.fsm.enabled || !p.do_push || !p.do_mix ||
+      !p.send_ack || !ptrs)
+    return cudaErrorInvalidValue;
+  GtStepParams k;
+  static_cast<GossipParams&>(k) = p;
+  k.gt = y;
+  eg_count_launch(EG_FAM_GOSSIP, 1);
+  if (p.mu != 0.f && p.mom != nullptr)
+    gossip_step_kernel_gt<true><<<grid, EG_THREADS, 0, s>>>(k);
+  else
+    gossip_step_kernel_gt<false><<<grid, EG_THREADS, 0, s>>>(k);
   return cudaGetLastError();
 }
 

@@ -23,7 +23,7 @@ class RingSimulator:
                  tcfg: Optional[TriggerConfig] = None, lr: float = 1e-2, momentum: float = 0.0,
                  topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
                  weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
-                 offsets=(1,), compress: str = "none"):
+                 offsets=(1,), compress: str = "none", gradient_tracking: bool = False):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -31,7 +31,11 @@ class RingSimulator:
         receivers hold (event: zero at start, theta_k of every fired tensor at its push; spevent: prev).
         `compress="int8"` (decent/event on the ring): a fired tensor sends the int8 code of theta - prev (q8_encode)
         instead of theta; sender and receivers add the same dequantized delta to prev and to their replica of it, the
-        mix reads the replicas, and under drift `sent` is prev."""
+        mix reads the replicas, and under drift `sent` is prev.
+        `gradient_tracking=True` (decent on the ring, DSGT): every rank also keeps y (tracking the average gradient),
+        the previous gradient g_prev and y inboxes, all zero at start; at step k it pushes theta_k and y_{k-1}, then
+        y_k = mix3_(y, yL, yR) + (g_k - g_prev), g_prev <- g_k, and the SGD step reads y_k instead of g_k.  At R = 1 the
+        plain serial step runs.  Any dtype works (float64 for convergence studies)."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -45,6 +49,9 @@ class RingSimulator:
             raise ValueError(f"topology {offsets!r}: only decent and event gossip beyond the ring")
         if self.q8 and (algo not in ("decent", "event") or not self.graphs[0].is_ring):
             raise ValueError("compress int8: decent or event on the ring only")
+        if gradient_tracking and (algo != "decent" or not self.graphs[0].is_ring or self.q8):
+            raise ValueError("gradient tracking: decent on the ring, without compression, only")
+        self.gt = bool(gradient_tracking) and world > 1
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -77,6 +84,11 @@ class RingSimulator:
             if self.n_slots == 2 and not self.period:
                 self.inbox_l = [ib[0] for ib in self.inbox]       # ring: slot 0 = from left, slot 1 = from right
                 self.inbox_r = [ib[1] for ib in self.inbox]
+        if self.gt:
+            self.y = [torch.zeros_like(theta0) for _ in range(world)]
+            self.g_prev = [torch.zeros_like(theta0) for _ in range(world)]
+            self.y_in_l = [torch.zeros_like(theta0) for _ in range(world)]
+            self.y_in_r = [torch.zeros_like(theta0) for _ in range(world)]
         self.drift = self.tcfg.metric == "drift" and algo in ("event", "spevent")
         if self.drift:
             # what each rank's receivers hold: event -- zero like the inboxes; spevent -- prev itself (same tensors)
@@ -174,6 +186,12 @@ class RingSimulator:
                     if self.drift:                             # one-peer graph: the last value pushed to any peer
                         self._flat(self.sent[r], i).copy_(src)
                     self.bytes[r] += n * t.numels[i] * 4
+        if self.gt:
+            # y_{k-1} travels with theta_k to both neighbours (every tensor: decent), and doubles the bytes
+            for r in range(R):
+                self.y_in_r[self.left(r)].copy_(self.y[r])
+                self.y_in_l[self.right(r)].copy_(self.y[r])
+                self.bytes[r] += 2 * t.n_elems * 4
         # ---- phase 2: mix with whatever the inboxes hold, then SGD -----------------------
         for r in range(R):
             if self.algo == "spevent" or self.q8:
@@ -184,6 +202,12 @@ class RingSimulator:
                 mix3_(self.theta[r], self.inbox[r][0], self.inbox[r][1])
             else:
                 mixk_(self.theta[r], self.inbox[r])
+            if self.gt:
+                g = grads[r].to(self.y[r].dtype)
+                mix3_(self.y[r], self.y_in_l[r], self.y_in_r[r]).add_(g.sub(self.g_prev[r]))
+                self.g_prev[r].copy_(g)
+                self._sgd(r, self.y[r])
+                continue
             self._sgd(r, grads[r])
 
     def final_average(self) -> torch.Tensor:

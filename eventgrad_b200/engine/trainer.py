@@ -89,7 +89,8 @@ class Trainer:
         self.train_src = train_source or load_source(cfg.dataset, cfg.data, cfg.train_samples, True)
         self.test_src = test_source
         mode = cfg.sampler
-        self.sampler = ShardSampler(len(self.train_src), env.world, env.rank, mode, seed=cfg.seed)
+        self.sampler = ShardSampler(len(self.train_src), env.world, env.rank, mode, seed=cfg.seed,
+                                    partition=cfg.partition, labels=self.train_src.labels)
         self.batch = per_rank_batch(cfg, env.world, self.sampler.local_size)
         self.loader = BatchLoader(self.train_src, self.sampler, self.batch, dev,
                                   augment=cfg.augment and cfg.dataset == "cifar10",

@@ -67,6 +67,19 @@ def check_compress_state(sd: Dict, compress: str, algo: str) -> None:
                          "resume with the same --compress")
 
 
+def check_tracking_state(sd: Dict, tracking: bool, algo: str) -> None:
+    """Refuse to resume decent state saved under the other --gradient-tracking setting: tracking state is y, the
+    previous gradient and the y inboxes, which a plain run neither saves nor restores.  Checkpoints without a
+    `gradient_tracking` key are non-tracking (their format predates gradient tracking)."""
+    if algo != "decent":
+        return
+    saved = bool(sd.get("gradient_tracking", False))
+    if saved != bool(tracking):
+        flag = lambda on: "--gradient-tracking" if on else "no --gradient-tracking"
+        raise ValueError(f"checkpoint was written with {flag(saved)}, this run uses {flag(tracking)}; "
+                         "resume with the same --gradient-tracking setting")
+
+
 class CommBackend:
     name = "base"
 

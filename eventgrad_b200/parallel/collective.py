@@ -12,6 +12,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
           persistent neighbour replicas      (/root/reference/dcifar10/spevent/spevent.cpp:342-542)
   --compress int8 (decent / event, ring): fired tensors travel as int8 codes of theta - prev plus block scales;
           both ends add the dequantized delta to prev / their replica of it, and the mix reads the replicas
+  --gradient-tracking (decent, ring): theta and y travel in one batched exchange; y_k = (y + yL + yR)/3 + g_k - g_prev,
+          and SGD steps along y_k
 
 torch.distributed has no one-sided RMA, so the "window" is emulated with an iteration-
 synchronous exchange: first the fire masks, then a payload holding only the fired tensors.
@@ -26,7 +28,8 @@ from typing import List
 import torch
 import torch.distributed as dist
 
-from .base import CommBackend, StepLog, check_compress_state, check_topology_state, check_trigger_state
+from .base import (CommBackend, StepLog, check_compress_state, check_topology_state, check_tracking_state,
+                   check_trigger_state)
 from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode, q8_encode,
                       q8_msg_bytes, sgd_, topk_select, trigger_step)
 
@@ -73,6 +76,12 @@ class CollectiveBackend(CommBackend):
         self.drift = cfg.algo in ("event", "spevent") and self.tcfg.metric == "drift"
         if self.drift:
             self.sent = self.prev if (cfg.algo == "spevent" or self.q8) else torch.zeros_like(arena.theta)
+        # --gradient-tracking (decent, ring): y, the previous gradient and the y inboxes, all zero at start.  R = 1 runs
+        # the plain step (tracking reduces to SGD on g)
+        self.gt = cfg.algo == "decent" and bool(getattr(cfg, "gradient_tracking", False)) and ring.world > 1
+        if self.gt:
+            self.y, self.g_prev = torch.zeros_like(arena.theta), torch.zeros_like(arena.theta)
+            self.y_in_l, self.y_in_r = torch.zeros_like(arena.theta), torch.zeros_like(arena.theta)
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
             self.last_recv_norm_l, self.last_recv_norm_r = z(), z()
@@ -173,6 +182,8 @@ class CollectiveBackend(CommBackend):
         a = self.arena
         if self.q8:
             return self._step_q8([True] * a.table.n_tensors, None)
+        if self.gt:
+            return self._step_tracking()
         if hasattr(self, "inbox"):
             self._exchange_slots(a.theta, self.inbox)
             self.bytes += self.ring.fanout * a.table.n_elems * 4
@@ -183,6 +194,18 @@ class CollectiveBackend(CommBackend):
         self.bytes += 2 * a.table.n_elems * 4
         mix3_(a.theta, self.inbox_l, self.inbox_r)
         self._opt()
+
+    def _step_tracking(self) -> None:
+        """Gradient tracking: theta_k and y_{k-1} to both neighbours in one batched exchange, then the simulator's ops:
+        y <- mix3_(y, yL, yR) + (g - g_prev), g_prev <- g, theta <- mix3_(theta, L, R), SGD along y."""
+        a = self.arena
+        self._exchange([a.theta, self.y], [a.theta, self.y], [self.inbox_l, self.y_in_l], [self.inbox_r, self.y_in_r])
+        self.bytes += 2 * 2 * a.table.n_elems * 4
+        mix3_(self.y, self.y_in_l, self.y_in_r).add_(a.grad.sub(self.g_prev))
+        self.g_prev.copy_(a.grad)
+        mix3_(a.theta, self.inbox_l, self.inbox_r)
+        sgd_(a.theta, self.y, a.mom, self.step_lr(self.pass_num), self.cfg.momentum, self.cfg.weight_decay,
+             self.cfg.nesterov)
 
     def _fire(self):
         a = self.arena
@@ -404,6 +427,11 @@ class CollectiveBackend(CommBackend):
         for k in ("inbox_l", "inbox_r", "prev", "rep_l", "rep_r"):
             if hasattr(self, k):
                 sd[k] = getattr(self, k).cpu().clone()
+        if self.cfg.algo == "decent":
+            sd["gradient_tracking"] = self.gt
+            if self.gt:
+                for k in ("y", "g_prev", "y_in_l", "y_in_r"):
+                    sd[k] = getattr(self, k).cpu().clone()
         if self.cfg.algo in ("decent", "event"):
             sd["compress"] = self.compress          # int8: prev / rep_l / rep_r are saved above
         if self.cfg.algo in ("event", "spevent"):
@@ -425,7 +453,11 @@ class CollectiveBackend(CommBackend):
         check_topology_state(sd, self.ring, self.cfg.algo)
         check_trigger_state(sd, self.tcfg.metric, self.cfg.algo)
         check_compress_state(sd, self.compress, self.cfg.algo)
+        check_tracking_state(sd, self.gt, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
+        if self.gt:
+            for k in ("y", "g_prev", "y_in_l", "y_in_r"):
+                getattr(self, k).copy_(sd[k].to(getattr(self, k).device))
         if self.drift and self.cfg.algo == "event" and not self.q8:
             self.sent.copy_(sd["sent"].to(self.sent.device))
         if hasattr(self, "inbox"):

@@ -10,6 +10,8 @@ Per training step, after backward():
            the same kernel accumulates the norms and runs the trigger FSM for the next step
            (--compress int8, ring: csrc/gossip_q8.cu pushes the int8 code of theta - prev + block scales, the receivers
            add the delta to their replicas of prev, and the mix reads the replicas)
+           (--gradient-tracking, decent on the ring: csrc/gossip_gt.cu also pushes y_{k-1} before the same flag, forms
+           y_k = (y + yL + yR)/3 + g_k - g_prev and steps along y_k)
   spevent  batched segmented radix-select top-k + compaction straight into the neighbours'
            inboxes, scatter of arrived records into replicas, then the dense mix+SGD kernel
 No NCCL/MPI call, no separate elementwise kernel and no host synchronisation on that path
@@ -22,7 +24,8 @@ from typing import List
 import torch
 
 from .arena import TILE, ParamArena, TensorTable
-from .base import CommBackend, StepLog, check_compress_state, check_topology_state, check_trigger_state
+from .base import (CommBackend, StepLog, check_compress_state, check_topology_state, check_tracking_state,
+                   check_trigger_state)
 from .topology import Graph
 from .trigger import q8_msg_bytes
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
@@ -48,12 +51,18 @@ def _wants_dbuf(cfg) -> bool:
     db = getattr(cfg, "double_buffer", None)
     return ((db is None or bool(db)) and cfg.algo == "decent" and cfg.sync_mode == "iter"
             and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True)
-            and not _wants_q8(cfg))
+            and not _wants_q8(cfg) and not getattr(cfg, "gradient_tracking", False))
 
 
 def _wants_q8(cfg) -> bool:
     """--compress int8: decent/event on the ring run the int8 step of csrc/gossip_q8.cu."""
     return getattr(cfg, "compress", "none") == "int8" and cfg.algo in ("decent", "event")
+
+
+def _wants_gt(cfg, world: int) -> bool:
+    """--gradient-tracking: decent on the ring of >= 2 ranks runs the tracking step of csrc/gossip_gt.cu (at R = 1
+    tracking is plain SGD on the gradient, the existing path)."""
+    return bool(getattr(cfg, "gradient_tracking", False)) and cfg.algo == "decent" and world > 1
 
 
 def _graph_of(cfg, rank: int, world: int):
@@ -87,6 +96,9 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None)
         slots = 2 if _wants_dbuf(cfg) else 1      # double-buffered decent: slot = step & 1
         lay.add("inbox_l", n * slots)
         lay.add("inbox_r", n * slots)
+        if _wants_gt(cfg, world):
+            lay.add("y_in_l", n)                  # gradient tracking: y from each neighbour
+            lay.add("y_in_r", n)
     if cfg.algo == "spevent":
         K = sum(table.topk_counts(cfg.topk_percent))
         lay.add("rec_from_l", 2 * K * 4)
@@ -119,6 +131,8 @@ def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
         max_grid = min(max_grid, C.gossip_graph_max_grid(env.device.index or 0))
     if _wants_q8(cfg):
         max_grid = min(max_grid, C.gossip_q8_max_grid(env.device.index or 0))
+    if _wants_gt(cfg, env.world):
+        max_grid = min(max_grid, C.gossip_gt_max_grid(env.device.index or 0))
     lay = build_layout(table, cfg, env.world, max_grid, graph)
     symm = wants_symm_window(env) and bootstrap is None      # NVLS path: torch symmetric memory + multicast mapping
     win = (SymmWindow if symm else Window)(lay, env.rank, env.world, env.device)
@@ -170,6 +184,11 @@ class P2PBackend(CommBackend):
         if self.q8 and (self.graph is not None or self.overlap or getattr(cfg, "ce_push", False) or self.want_logs
                         or not self.sync):
             raise ValueError("p2p backend: --compress int8 runs decent/event on the ring's fused iter-sync step only")
+        # --gradient-tracking: the iter-sync fused single-slot ring step of csrc/gossip_gt.cu
+        self.gt = _wants_gt(cfg, ring.world) and self.do_comm
+        if self.gt and (self.graph is not None or self.overlap or getattr(cfg, "ce_push", False) or self.want_logs
+                        or not self.sync or self.q8):
+            raise ValueError("p2p backend: --gradient-tracking runs decent on the ring's fused iter-sync step only")
         self.dbuf = _wants_dbuf(cfg) and self.do_comm
         self.ce_push = bool(getattr(cfg, "ce_push", False)) and self.overlap and cfg.algo == "decent" and self.sync
         self.nvls = self.nvls_step = False      # set in connect() when the window has a multicast mapping
@@ -238,6 +257,9 @@ class P2PBackend(CommBackend):
             self.prev = arena.theta.clone()
             self.rep_l = arena.theta.clone()
             self.rep_r = arena.theta.clone()
+        if self.gt:
+            # y, the previous gradient (fp32 whatever the gradient dtype) and the y inboxes start at zero on every rank
+            self.y, self.g_prev = zf(t.n_padded), zf(t.n_padded)
         # drift trigger (--trigger drift): the FSM reads ||theta - sent||.  event: `sent` is an arena-sized buffer,
         # zero like the receivers' inboxes, that the step kernel's pushes keep equal to what was last pushed; spevent:
         # `prev` already is what the receivers hold, element by element
@@ -256,7 +278,7 @@ class P2PBackend(CommBackend):
         self._grads_alive = None
         self.host_bytes = 0
         self._connected = False
-        self.gp = self.ap = self.ap_avg = self.sp = self.gs = self.qs = None
+        self.gp = self.ap = self.ap_avg = self.sp = self.gs = self.qs = self.ts = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
@@ -362,6 +384,15 @@ class P2PBackend(CommBackend):
                 self.wire_dedup = self.ring.world == 2 and L == R
                 if self.wire_dedup:
                     gp.update({"inbox_l": win.addr("inbox_r"), "push_r": 0})
+                if self.gt:
+                    # y travels exactly as theta does, the single-copy dedup of the 2-rank ring included
+                    ts = C.TrackSlots()
+                    ts.update({"y": P(self.y), "g_prev": P(self.g_prev),
+                               "y_in_l": win.addr("y_in_r" if self.wire_dedup else "y_in_l"),
+                               "y_in_r": win.addr("y_in_r"),
+                               "y_to_l": win.addr("y_in_r", L),
+                               "y_to_r": 0 if self.wire_dedup else win.addr("y_in_l", R)})
+                    self.ts = ts
             elif self.sparse:
                 gp.update({"inbox_l": P(self.rep_l), "inbox_r": P(self.rep_r)})
             self.gp = gp
@@ -543,6 +574,8 @@ class P2PBackend(CommBackend):
                 C.gossip_step(self.gp, self.grid, s)                   # receive prologue + mix + SGD + trigger
             elif self.q8 and self.do_comm:
                 C.gossip_step_q8(self.gp, self.qs, self.grid, s)
+            elif self.gt:
+                C.gossip_step_gt(self.gp, self.ts, self.grid, s)
             elif self.overlap:
                 C.gossip_step_phase(self.gp, 2, self.grid, s)
             elif self.dbuf:
@@ -559,6 +592,8 @@ class P2PBackend(CommBackend):
             self.host_bytes += self.table.n_elems * 4
         elif self.cfg.algo == "decent" and self.do_comm and self.q8:
             self.host_bytes += 2 * sum(self.msg_bytes)
+        elif self.gt:
+            self.host_bytes += 2 * 2 * self.table.n_elems * 4      # theta and y, to both neighbours
         elif self.cfg.algo == "decent" and self.do_comm:
             self.host_bytes += getattr(self.ring, "fanout", 2) * self.table.n_elems * 4
 
@@ -642,6 +677,12 @@ class P2PBackend(CommBackend):
             sd["inbox_r"] = self.win.view("inbox_r", torch.float32).cpu().clone()
         if self.cfg.algo in ("decent", "event"):
             sd["compress"] = "int8" if self.q8 else "none"
+        if self.cfg.algo == "decent":
+            sd["gradient_tracking"] = self.gt
+            if self.gt:
+                sd["y"], sd["g_prev"] = self.y.cpu().clone(), self.g_prev.cpu().clone()
+                sd["y_in_l"] = self.win.view("y_in_l", torch.float32).cpu().clone()
+                sd["y_in_r"] = self.win.view("y_in_r", torch.float32).cpu().clone()
         if self.sparse or self.q8:
             for k in ("prev", "rep_l", "rep_r"):
                 sd[k] = getattr(self, k).cpu().clone()
@@ -655,6 +696,7 @@ class P2PBackend(CommBackend):
         check_topology_state(sd, self.ring, self.cfg.algo)
         check_trigger_state(sd, self.metric, self.cfg.algo)
         check_compress_state(sd, "int8" if self.q8 else "none", self.cfg.algo)
+        check_tracking_state(sd, self.gt, self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
@@ -670,6 +712,11 @@ class P2PBackend(CommBackend):
                 getattr(self, k).copy_(sd[k].to(self.dev))
         if self.drift and not self.sparse and not self.q8:
             self.sent.copy_(sd["sent"].to(self.dev))
+        if self.gt:
+            self.y.copy_(sd["y"].to(self.dev))
+            self.g_prev.copy_(sd["g_prev"].to(self.dev))
+            self.win.view("y_in_l", torch.float32).copy_(sd["y_in_l"].to(self.dev))
+            self.win.view("y_in_r", torch.float32).copy_(sd["y_in_r"].to(self.dev))
         if self.log_ring is not None:
             self._drained = self.pass_num          # log rows of the steps before the checkpoint are not replayed
         # NOTE: handshake counters (flags / acks) restart from pass_num on every rank
