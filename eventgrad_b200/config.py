@@ -80,6 +80,8 @@ class TrainConfig:
                                      # scale per 256 elements) with error feedback instead of fp32 theta
     gradient_tracking: bool = False  # decent on the ring: also gossip y, which tracks the average gradient, and step
                                      # along y instead of the local gradient (DSGT / DIGing; fused single-slot step)
+    local_steps: int = 1             # decent: gossip at every H-th step only (step k iff H divides k); the H - 1 steps
+                                     # between are serial SGD steps with no exchange (local / periodic D-PSGD)
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -210,6 +212,30 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError("--gradient-tracking does not support file_write: the reference's log format has no "
                                  "column for y")
+        if not isinstance(self.local_steps, int) or self.local_steps < 1:
+            raise ValueError(f"--local-steps must be an integer >= 1, got {self.local_steps!r}")
+        if self.local_steps > 1:
+            # periodic gossip exists for decent in the fused single-kernel ring / graph step (csrc/gossip.cu,
+            # csrc/gossip_graph.cu), the torch.distributed backends and the simulator
+            h = f"--local-steps {self.local_steps}"
+            if self.algo == "cent":
+                raise ValueError(f"{h} needs algo decent: local SGD with periodic parameter averaging is a different "
+                                 "all-reduce step, and cent's momentum lives outside the peer window")
+            if self.algo in ("event", "spevent"):
+                raise ValueError(f"{h} needs algo decent, got {self.algo!r}: the trigger already decides when to send, "
+                                 "and its slope history and event accounting are indexed by step, not by round")
+            if self.gradient_tracking:
+                raise ValueError(f"{h} does not support --gradient-tracking")
+            if self.compress != "none":
+                raise ValueError(f"{h} does not support --compress int8")
+            if self.backend == "refport":
+                raise ValueError(f"{h} is not supported by --backend refport")
+            for name in ("overlap_push", "double_buffer", "ce_push"):
+                if getattr(self, name):
+                    raise ValueError(f"{h} does not support {name} (fused single-kernel step only)")
+            if self.file_write:
+                raise ValueError(f"{h} does not support file_write: the reference's log format records an exchange "
+                                 "at every step")
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
@@ -259,7 +285,7 @@ class TrainConfig:
         if c.overlap_push is None:
             kw["overlap_push"] = bool(cuda and p2p and world >= 2 and c.algo in ("decent", "event")
                                       and not bool(c.double_buffer) and c.ring_topology and c.compress == "none"
-                                      and not c.gradient_tracking)
+                                      and not c.gradient_tracking and c.local_steps == 1)
         return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
@@ -338,6 +364,9 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--gradient-tracking", action="store_true", default=None,
                    help="decent on the ring: also gossip y, a running estimate of the average gradient, and step along "
                         "it (DSGT): removes the bias of constant-lr D-PSGD under heterogeneous data")
+    p.add_argument("--local-steps", type=int, default=None, metavar="H",
+                   help="decent: gossip only at every H-th step and take plain local SGD steps in between (local "
+                        "D-PSGD); sends 1/H of the bytes (default 1: every step)")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

@@ -109,6 +109,10 @@ struct GossipParams {
   int nesterov;             // 1: Nesterov momentum (needs mu > 0)
   const float* lr_table;    // optional [lr_len]: lr of step s is lr_table[min(s-1, lr_len-1)]; null: the scalar lr
   int lr_len;
+  // periodic gossip (--local-steps H, decent on the ring and on graphs): step k gossips iff H divides k, every other
+  // step is the serial SGD step (no push, no flag, no ack, no mix).  0 or 1: every step gossips.  It sits in the padding
+  // in front of `sent`, so the size of this block and the offset of every other field are unchanged
+  int local_steps;
   // drift trigger (fsm.metric = 1): what the receivers hold of theta.  event: every pushed tile also stores theta_k
   // here, and the norm-on-write partials are sum (theta_{k+1} - sent)^2; spevent: the sparse `prev` (written by the
   // compaction, never by the step kernel).  null: the norm rule, no extra loads or stores

@@ -50,6 +50,10 @@
 // y_k = ((y + yL) + yR) / 3 + (g_k - g_prev) first, stores y and g_prev, mixes theta and hands y_k to sgd_elem in place
 // of the gradient.  The ack of step k covers both inboxes, so there is no new synchronisation variable
 // (PROTOCOL.md 1.8).
+// Periodic gossip (GossipParams.local_steps = H > 1, decent, ring and graph builds): step k pushes, flags, waits, mixes
+// and acks only when H divides k; the other steps are the single-pass plain SGD step.  The WAR guard waits for the ack
+// of the previous round (k - H; one-peer: k - tau * H) and the one-peer slot is indexed by the round k / H (PROTOCOL.md
+// 1.9).
 #include "api.h"
 #include "common.cuh"
 #include "sparse_apply.cuh"
@@ -100,8 +104,25 @@ using StepParams = GossipParams;
 #define EG_NMSG(p) 2ull
 #define EG_ACTIVE_SLOT(p, step) (-1)
 #endif
+// Periodic gossip (GossipParams.local_steps = H > 1) exists in the ring and graph builds only; the other builds gossip
+// at every step and their launchers reject H > 1
+#if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT)
+#define EG_LOCAL_STEPS 0
+#else
+#define EG_LOCAL_STEPS 1
+#endif
 
 namespace egb {
+
+// Does 1-based step `step` gossip?  --local-steps H: iff H divides it.  Re-evaluated where it is needed instead of held
+// in a register across the tile loops
+__device__ __forceinline__ bool gossip_step_comm(const StepParams& p, int step) {
+#if EG_LOCAL_STEPS
+  return p.local_steps <= 1 || step % p.local_steps == 0;
+#else
+  return true;
+#endif
+}
 
 // Per-CTA tile metadata, resolved ONCE at kernel start (thread j resolves iteration j, so the
 // dependent table look-ups tile->tensor->{fire, grad pointer, numel} run in parallel instead of
@@ -419,10 +440,11 @@ __device__ __forceinline__ F8 load_grad(const StepParams& p, const TileInfo& ti,
   return g;
 }
 
-// mix + SGD + norm-on-write for one tile. `th` already holds theta_k for this thread's 8 floats.
+// mix + SGD + norm-on-write for one tile. `th` already holds theta_k for this thread's 8 floats.  `mix`: p.do_mix of
+// a gossip step, false on a local step of --local-steps (plain SGD); the q8 and tracking builds always mix
 template <bool kMom>
 __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileInfo& ti, size_t base, F8 th,
-                                         int lane, int warp, int step, int slot) {
+                                         int lane, int warp, int step, int slot, bool mix) {
 #ifdef EG_GRAPH
   // no receive-norm logging on graphs (file_write is ring only); slots are loaded two at a time after the gradient
   // and momentum, which keeps the kernel at 64 registers whatever the degree
@@ -431,7 +453,7 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
   F8 m;
   const F8 g = load_grad(p, ti, base, threadIdx.x);
   if (kMom) m = ld_f8(p.mom + base);
-  if (p.do_mix && p.g.period) {
+  if (mix && p.g.period) {
     // one-peer graph: theta <- (theta + in_slot) / 2
     const float* in = p.g.inbox[0];
 #pragma unroll
@@ -440,7 +462,7 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
     const F8 A = ld_f8_cg(in + base);
 #pragma unroll
     for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(__fadd_rn(th.v[e], A.v[e]), 2.f);
-  } else if (p.do_mix) {
+  } else if (mix) {
 #pragma unroll
     for (int s = 0; s < EG_MAX_SLOTS; s += 2) {
       if (s < p.g.n_slots) {
@@ -498,7 +520,7 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
   float ssl = 0.f, ssr = 0.f;
   // issue every load of the tile before the first dependent FP op (5 x 32 B in flight per lane)
   F8 L, R, m;
-  if (p.do_mix) {
+  if (mix) {
 #ifdef EG_DBUF
     L = ld_f8_cg(p.inbox_l + EG_SLOT_OFF(p, step) + base);
     R = ld_f8_cg(p.inbox_r + EG_SLOT_OFF(p, step) + base);
@@ -509,7 +531,7 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
   }
   const F8 g = load_grad(p, ti, base, threadIdx.x);
   if (kMom) m = ld_f8(p.mom + base);
-  if (p.do_mix) {
+  if (mix) {
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       th.v[e] = __fdiv_rn(__fadd_rn(__fadd_rn(th.v[e], L.v[e]), R.v[e]), 3.0f);
@@ -566,8 +588,10 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
 }
 
 // Elect the last CTA of the grid; it acks and bumps the step counter (the trigger FSM itself is
-// run per tensor by whichever warp completes that tensor, see cta_finish_tensors).
+// run per tensor by whichever warp completes that tensor, see cta_finish_tensors).  A local step of --local-steps
+// read no inbox and acks nothing.
 __device__ __forceinline__ void grid_tail(const StepParams& p, int step, int slot) {
+  const bool comm = gossip_step_comm(p, step);
   __shared__ int s_last;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -581,7 +605,7 @@ __device__ __forceinline__ void grid_tail(const StepParams& p, int step, int slo
     *p.ticket = 0u;
     *p.fsm.pass_num = step;
 #if defined(EG_GRAPH)
-    if (p.sync && p.send_ack) {
+    if (p.sync && p.send_ack && comm) {
       // every CTA of this rank has finished reading its inboxes for `step`: ack every active slot's sender
       fence_sys();
 #pragma unroll
@@ -589,7 +613,7 @@ __device__ __forceinline__ void grid_tail(const StepParams& p, int step, int slo
         if (slot_on(p, s, slot)) st_release_sys(p.g.ack_to[s], (uint32_t)step);
     }
 #elif !defined(EG_DBUF)
-    if (p.sync && p.send_ack) {
+    if (p.sync && p.send_ack && comm) {
       // every CTA of this rank has finished reading its inboxes for `step`
       fence_sys();
       st_release_sys(p.ack_to_l, (uint32_t)step);
@@ -643,9 +667,17 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   const int b = blockIdx.x, G = gridDim.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int step = *p.fsm.pass_num + 1;
+  // --local-steps H: step k gossips iff H divides k, as round k / H; every other step is the serial SGD step.  A uniform
+  // branch on the device pass counter, which iter-sync keeps equal on every rank (PROTOCOL.md 1.9)
+  const bool comm = gossip_step_comm(p, step);
+#if EG_LOCAL_STEPS
+  const int H = max(p.local_steps, 1);
+  const int slot = EG_ACTIVE_SLOT(p, step / H);
+#else
   const int slot = EG_ACTIVE_SLOT(p, step);
+#endif
   const int n_tiles = p.tab.n_tiles;
-  const bool push = p.do_push != 0 && p.phase != 2;
+  const bool push = p.do_push != 0 && p.phase != 2 && comm;
   // Sticky failure: once any peer wait has timed out (this or an earlier launch) the step is a no-op on every
   // CTA -- nothing is stored into a peer that may be wedged or dead, theta stops changing, and the host raises
   // when it reads the status word.  (Uniform per CTA; the run is over, so a partial step does not matter.)
@@ -681,14 +713,14 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   }
 
   if (!(p.sync && push)) {
-    // ---------------- async / split / no exchange: single pass, theta read once ---------------
+    // ---------------- async / split / no exchange / local step: single pass, theta read once -------
     int j = 0;
     for (int t = b; t < n_tiles; t += G, ++j) {
       const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
       const TileInfo ti = tile_info(p, s_ti, j, t);
       const F8 th = ld_f8(p.theta + base);
       if (push && (ti.flags & 1)) push_tile(p, base, th, slot);
-      mix_tile<kMom>(p, t, ti, base, th, lane, warp, step, slot);
+      mix_tile<kMom>(p, t, ti, base, th, lane, warp, step, slot, p.do_mix != 0 && comm);
     }
   } else {
     // ---------------- iter-sync: per-WARP software pipeline, no block barriers ------------------
@@ -701,9 +733,10 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
     __shared__ int s_ok;
     if (tid == 0) {
       // WAR guard: every peer I push into must have consumed what I last pushed into its slot before I overwrite
-      // it -- at step-1 on a static graph, at step-period on a one-peer graph (slot m is written every period steps)
+      // it -- at step-1 on a static graph, at step-period on a one-peer graph (slot m is written every period steps);
+      // with --local-steps H the last push into a slot was H (static) or period * H (one-peer) steps ago
       bool ok = true;
-      const int prev = max(step - (p.g.period ? p.g.period : 1), 0);   // the first tau steps wait for nothing
+      const int prev = max(step - (p.g.period ? p.g.period : 1) * H, 0);   // the first round(s) wait for nothing
 #pragma unroll
       for (int k = 0; k < EG_MAX_SLOTS; ++k)
         if (slot_on(p, k, slot)) ok = wait_ge(p.g.ack_from[k], (uint32_t)prev, p.status, p.timeout_ns) && ok;
@@ -714,9 +747,15 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #elif !defined(EG_DBUF)
     __shared__ int s_ok;
     if (tid == 0) {
-      // WAR guard: neighbours must have consumed what I pushed at step-1 before I overwrite it
-      bool ok = wait_ge(p.ack_from_l, (uint32_t)(step - 1), p.status, p.timeout_ns);
-      ok = wait_ge(p.ack_from_r, (uint32_t)(step - 1), p.status, p.timeout_ns) && ok;
+      // WAR guard: neighbours must have consumed what I pushed at step-1 (--local-steps H: at step-H, the last
+      // round) before I overwrite it
+#if EG_LOCAL_STEPS
+      const uint32_t prev = (uint32_t)max(step - H, 0);
+#else
+      const uint32_t prev = (uint32_t)(step - 1);
+#endif
+      bool ok = wait_ge(p.ack_from_l, prev, p.status, p.timeout_ns);
+      ok = wait_ge(p.ack_from_r, prev, p.status, p.timeout_ns) && ok;
       s_ok = ok;
     }
     __syncthreads();
@@ -768,7 +807,8 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         // the fired bits lane 0 observed, to the whole warp
         const int sides = __shfl_sync(0xffffffffu, (int)((fl & 1u) | ((fr & 1u) << 1)), 0);
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
-        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, sides);
+        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, sides,
+                       p.do_mix != 0);
 #else
         if (lane == 0) {
 #ifdef EG_GRAPH
@@ -785,9 +825,10 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
 #ifdef EG_GT
         // the tracking mix loads theta itself, after the y stage: held from here it would spill
-        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot);
+        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot, p.do_mix != 0);
 #else
-        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, slot);
+        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, slot,
+                       p.do_mix != 0);
 #endif
 #endif
       }
@@ -856,6 +897,9 @@ int gossip_max_grid(int device) {
 }
 
 cudaError_t launch_gossip_step(const GossipParams& p, int grid, cudaStream_t s) {
+  // --local-steps: the fused dense step only (no split phases, no sparse records, no trigger, no drift copy)
+  if (p.local_steps > 1 && (p.phase != 0 || p.sparse != nullptr || p.fsm.enabled || p.sent != nullptr))
+    return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
     gossip_step_kernel<true><<<grid, EG_THREADS, 0, s>>>(p);
@@ -893,6 +937,7 @@ cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g,
   const bool slots_ok = g.period == 0 ? (g.n_slots >= 2 && g.n_slots <= EG_MAX_SLOTS && !(g.n_slots & 1))
                                       : (g.period >= 1 && g.period <= EG_MAX_SLOTS && g.n_slots == g.period);
   if (p.phase != 0 || p.sparse != nullptr || !p.do_push || !p.do_mix || !slots_ok) return cudaErrorInvalidValue;
+  if (p.local_steps > 1 && (p.fsm.enabled || p.sent != nullptr)) return cudaErrorInvalidValue;   // decent only
   GraphStepParams q;
   static_cast<GossipParams&>(q) = p;
   q.g = g;
@@ -920,7 +965,8 @@ cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int g
   const bool ptrs = q.q_from_l && q.q_from_r && q.s_from_l && q.s_from_r && q.q_to_l && q.q_to_r && q.s_to_l &&
                     q.s_to_r && q.prev && q.rep_l && q.rep_r && p.flag_from_l && p.flag_from_r && p.flag_to_l &&
                     p.flag_to_r && p.ack_from_l && p.ack_from_r && p.ack_to_l && p.ack_to_r;
-  if (p.phase != 0 || !p.sync || p.sparse != nullptr || !p.do_push || !p.do_mix || !ptrs) return cudaErrorInvalidValue;
+  if (p.phase != 0 || !p.sync || p.sparse != nullptr || !p.do_push || !p.do_mix || !ptrs || p.local_steps > 1)
+    return cudaErrorInvalidValue;
   Q8StepParams k;
   static_cast<GossipParams&>(k) = p;
   k.q = q;
@@ -950,7 +996,7 @@ cudaError_t launch_gossip_step_gt(const GossipParams& p, const TrackSlots& y, in
                     p.flag_from_l && p.flag_from_r && p.flag_to_l && p.flag_to_r && p.ack_from_l && p.ack_from_r &&
                     p.ack_to_l && p.ack_to_r;
   if (p.phase != 0 || !p.sync || p.sparse != nullptr || p.sent != nullptr || p.fsm.enabled || !p.do_push || !p.do_mix ||
-      !p.send_ack || !ptrs)
+      !p.send_ack || !ptrs || p.local_steps > 1)
     return cudaErrorInvalidValue;
   GtStepParams k;
   static_cast<GossipParams&>(k) = p;
@@ -976,7 +1022,7 @@ int gossip_dbuf_max_grid(int device) {
 
 // Dense iter-sync exchange only (decent): every tensor fires every step, inboxes hold 2 slots.
 cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_t s) {
-  if (p.phase != 0 || !p.sync || !p.do_push || !p.do_mix || p.fsm.enabled || p.sent != nullptr)
+  if (p.phase != 0 || !p.sync || !p.do_push || !p.do_mix || p.fsm.enabled || p.sent != nullptr || p.local_steps > 1)
     return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)

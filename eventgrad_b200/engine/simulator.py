@@ -23,7 +23,7 @@ class RingSimulator:
                  tcfg: Optional[TriggerConfig] = None, lr: float = 1e-2, momentum: float = 0.0,
                  topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
                  weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
-                 offsets=(1,), compress: str = "none", gradient_tracking: bool = False):
+                 offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -35,7 +35,11 @@ class RingSimulator:
         `gradient_tracking=True` (decent on the ring, DSGT): every rank also keeps y (tracking the average gradient),
         the previous gradient g_prev and y inboxes, all zero at start; at step k it pushes theta_k and y_{k-1}, then
         y_k = mix3_(y, yL, yR) + (g_k - g_prev), g_prev <- g_k, and the SGD step reads y_k instead of g_k.  At R = 1 the
-        plain serial step runs.  Any dtype works (float64 for convergence studies)."""
+        plain serial step runs.  Any dtype works (float64 for convergence studies).
+        `local_steps=H` (decent, periodic gossip): step k (1-based) communicates iff H divides k, as round n = k / H --
+        exactly the decent step above, with the one-peer graph's active slot (n - 1) mod tau taken from the round.  Every
+        other step is the serial step theta <- sgd(theta, g_k): no push, no mix, the inboxes keep what the last round
+        delivered, momentum stays local and the lr table stays indexed by step.  Bytes count at communicating steps only."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -52,6 +56,11 @@ class RingSimulator:
         if gradient_tracking and (algo != "decent" or not self.graphs[0].is_ring or self.q8):
             raise ValueError("gradient tracking: decent on the ring, without compression, only")
         self.gt = bool(gradient_tracking) and world > 1
+        if int(local_steps) != local_steps or local_steps < 1:
+            raise ValueError(f"local_steps must be an integer >= 1, got {local_steps!r}")
+        if local_steps > 1 and (algo != "decent" or self.q8 or gradient_tracking):
+            raise ValueError("local steps: decent without compression or gradient tracking only")
+        self.local_steps = int(local_steps)
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -118,6 +127,14 @@ class RingSimulator:
         lr = lr_at(self.lr_table, self.pass_num, self.lr)
         sgd_(self.theta[r], grad, self.mom[r], lr, self.mu, self.wd, self.nesterov)
 
+    def communicates(self, step: int) -> bool:
+        """Does 1-based step `step` gossip (local_steps H: iff H divides it)?"""
+        return step % self.local_steps == 0
+
+    def round_of(self, step: int) -> int:
+        """Gossip round of a communicating step: the one-peer graph's active slot is indexed by it."""
+        return step // self.local_steps
+
     def left(self, r):
         return (r - 1) % self.R
 
@@ -139,9 +156,11 @@ class RingSimulator:
                 self._sgd(r, g)
                 self.bytes[r] += t.n_elems * 4 if R > 1 else 0
             return
-        if R == 1 and self.serial_skip:
-            self._sgd(0, grads[0])
+        if (R == 1 and self.serial_skip) or not self.communicates(self.pass_num):
+            for r in range(R):                                 # serial step / local step of --local-steps
+                self._sgd(r, grads[r])
             return
+        rnd = self.round_of(self.pass_num)
         # ---- phase 1: every rank decides and "Puts" (uses pre-mix theta_k) --------------
         if self.algo == "decent":
             fires = [torch.ones(t.n_tensors, dtype=torch.bool) for _ in range(R)]
@@ -179,8 +198,8 @@ class RingSimulator:
                     self.bytes[r] += 2 * q8_msg_bytes(t.numels[i])
                 else:
                     outs = self.graphs[r].out_slots()
-                    if self.period:                            # one-peer graph: only this step's out-slot
-                        outs = [outs[self.graphs[r].active(self.pass_num)]]
+                    if self.period:                            # one-peer graph: only this round's out-slot
+                        outs = [outs[self.graphs[r].active(rnd)]]
                     for p, j in outs:                          # a fired tensor goes into every slot I feed
                         self._flat(self.inbox[p][j], i).copy_(src)
                     if self.drift:                             # one-peer graph: the last value pushed to any peer
@@ -197,7 +216,7 @@ class RingSimulator:
             if self.algo == "spevent" or self.q8:
                 mix3_(self.theta[r], self.rep_l[r], self.rep_r[r])
             elif self.period:
-                mix2_(self.theta[r], self.inbox[r][self.graphs[r].active(self.pass_num)])
+                mix2_(self.theta[r], self.inbox[r][self.graphs[r].active(rnd)])
             elif self.n_slots == 2:
                 mix3_(self.theta[r], self.inbox[r][0], self.inbox[r][1])
             else:
@@ -222,9 +241,12 @@ class RingSimulator:
         return self.fanout * self.table.n_tensors * self.pass_num * self.R
 
     def mixing_matrix(self, step: Optional[int] = None) -> torch.Tensor:
-        """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD.  The one-peer graph's W depends
-        on the 1-based step (default: the next one)."""
+        """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD.  It depends on the 1-based step
+        (default: the next one) on the one-peer graph, whose slot is that of the step's round, and under local_steps,
+        where a step that does not communicate has W = I."""
+        k = self.pass_num + 1 if step is None else step
+        if not self.communicates(k):
+            return torch.eye(self.R, dtype=torch.float64)
         if self.period:
-            k = self.pass_num + 1 if step is None else step
-            return torch.tensor([g.mixing_row(k) for g in self.graphs], dtype=torch.float64)
+            return torch.tensor([g.mixing_row(self.round_of(k)) for g in self.graphs], dtype=torch.float64)
         return torch.tensor([g.mixing_row() for g in self.graphs], dtype=torch.float64)

@@ -80,6 +80,19 @@ def check_tracking_state(sd: Dict, tracking: bool, algo: str) -> None:
                          "resume with the same --gradient-tracking setting")
 
 
+def check_local_steps_state(sd: Dict, local_steps: int, algo: str) -> None:
+    """Refuse to resume decent state saved under another --local-steps: the inboxes hold what the last round of that
+    schedule delivered, and the one-peer graph's slot is indexed by its rounds.  Checkpoints without a `local_steps` key
+    gossiped at every step (their format predates periodic gossip).  A resume at a step that is not a multiple of H
+    continues the cycle by itself: which step gossips is a function of the restored step counter."""
+    if algo != "decent":
+        return
+    saved = int(sd.get("local_steps", 1))
+    if saved != int(local_steps):
+        raise ValueError(f"checkpoint was written with --local-steps {saved}, this run uses --local-steps "
+                         f"{int(local_steps)}; resume with the same --local-steps")
+
+
 class CommBackend:
     name = "base"
 

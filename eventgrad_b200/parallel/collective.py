@@ -14,6 +14,7 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
           both ends add the dequantized delta to prev / their replica of it, and the mix reads the replicas
   --gradient-tracking (decent, ring): theta and y travel in one batched exchange; y_k = (y + yL + yR)/3 + g_k - g_prev,
           and SGD steps along y_k
+  --local-steps H (decent): only every H-th step runs the exchange and mix; the others are the SGD update alone
 
 torch.distributed has no one-sided RMA, so the "window" is emulated with an iteration-
 synchronous exchange: first the fire masks, then a payload holding only the fired tensors.
@@ -28,8 +29,8 @@ from typing import List
 import torch
 import torch.distributed as dist
 
-from .base import (CommBackend, StepLog, check_compress_state, check_topology_state, check_tracking_state,
-                   check_trigger_state)
+from .base import (CommBackend, StepLog, check_compress_state, check_local_steps_state, check_topology_state,
+                   check_tracking_state, check_trigger_state)
 from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode, q8_encode,
                       q8_msg_bytes, sgd_, topk_select, trigger_step)
 
@@ -82,6 +83,8 @@ class CollectiveBackend(CommBackend):
         if self.gt:
             self.y, self.g_prev = torch.zeros_like(arena.theta), torch.zeros_like(arena.theta)
             self.y_in_l, self.y_in_r = torch.zeros_like(arena.theta), torch.zeros_like(arena.theta)
+        # --local-steps H (decent): step k gossips iff H divides k, as round k / H; the other steps are _opt() alone
+        self.local_steps = int(getattr(cfg, "local_steps", 1)) if cfg.algo == "decent" else 1
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
             self.last_recv_norm_l, self.last_recv_norm_r = z(), z()
@@ -129,7 +132,7 @@ class CollectiveBackend(CommBackend):
     def _active_slots(self) -> List[int]:
         """Slots that take part in this step: all of a static graph, the one active slot of a one-peer graph."""
         g = self.ring
-        return [g.active(self.pass_num)] if g.period else list(range(g.n_slots))
+        return [g.active(self.pass_num // self.local_steps)] if g.period else list(range(g.n_slots))
 
     def _exchange_slots(self, payload: torch.Tensor, recv: List[torch.Tensor]) -> None:
         """Graph rendezvous over the active slots: `payload` goes into every active slot I feed (out-slot j = slot j of
@@ -144,9 +147,9 @@ class CollectiveBackend(CommBackend):
             w.wait()
 
     def _mix_slots(self) -> None:
-        """Static graph: mixk_ over every slot.  One-peer graph: (theta + active slot) / 2."""
+        """Static graph: mixk_ over every slot.  One-peer graph: (theta + active slot) / 2, the slot of this round."""
         if self.ring.period:
-            mix2_(self.arena.theta, self.inbox[self.ring.active(self.pass_num)])
+            mix2_(self.arena.theta, self.inbox[self.ring.active(self.pass_num // self.local_steps)])
         else:
             mixk_(self.arena.theta, self.inbox)
 
@@ -161,8 +164,8 @@ class CollectiveBackend(CommBackend):
         algo = self.cfg.algo
         if algo == "cent":
             self._step_cent()
-        elif not self.comm_enabled:
-            self._opt()
+        elif not self.comm_enabled or self.pass_num % self.local_steps:
+            self._opt()                                # serial step / local step of --local-steps
         elif algo == "decent":
             self._step_decent()
         elif algo == "event":
@@ -429,6 +432,7 @@ class CollectiveBackend(CommBackend):
                 sd[k] = getattr(self, k).cpu().clone()
         if self.cfg.algo == "decent":
             sd["gradient_tracking"] = self.gt
+            sd["local_steps"] = self.local_steps
             if self.gt:
                 for k in ("y", "g_prev", "y_in_l", "y_in_r"):
                     sd[k] = getattr(self, k).cpu().clone()
@@ -454,6 +458,7 @@ class CollectiveBackend(CommBackend):
         check_trigger_state(sd, self.tcfg.metric, self.cfg.algo)
         check_compress_state(sd, self.compress, self.cfg.algo)
         check_tracking_state(sd, self.gt, self.cfg.algo)
+        check_local_steps_state(sd, self.local_steps, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
         if self.gt:
             for k in ("y", "g_prev", "y_in_l", "y_in_r"):

@@ -24,8 +24,8 @@ from typing import List
 import torch
 
 from .arena import TILE, ParamArena, TensorTable
-from .base import (CommBackend, StepLog, check_compress_state, check_topology_state, check_tracking_state,
-                   check_trigger_state)
+from .base import (CommBackend, StepLog, check_compress_state, check_local_steps_state, check_topology_state,
+                   check_tracking_state, check_trigger_state)
 from .topology import Graph
 from .trigger import q8_msg_bytes
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
@@ -51,7 +51,8 @@ def _wants_dbuf(cfg) -> bool:
     db = getattr(cfg, "double_buffer", None)
     return ((db is None or bool(db)) and cfg.algo == "decent" and cfg.sync_mode == "iter"
             and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True)
-            and not _wants_q8(cfg) and not getattr(cfg, "gradient_tracking", False))
+            and not _wants_q8(cfg) and not getattr(cfg, "gradient_tracking", False)
+            and getattr(cfg, "local_steps", 1) == 1)
 
 
 def _wants_q8(cfg) -> bool:
@@ -189,6 +190,12 @@ class P2PBackend(CommBackend):
         if self.gt and (self.graph is not None or self.overlap or getattr(cfg, "ce_push", False) or self.want_logs
                         or not self.sync or self.q8):
             raise ValueError("p2p backend: --gradient-tracking runs decent on the ring's fused iter-sync step only")
+        # --local-steps H (decent): the fused single-slot ring / graph step gossips at every H-th step only; the
+        # kernel takes that choice from its device step counter, so one captured launch serves the whole cycle
+        self.local_steps = int(getattr(cfg, "local_steps", 1)) if cfg.algo == "decent" else 1
+        if getattr(cfg, "local_steps", 1) > 1 and (cfg.algo != "decent" or self.overlap or self.q8 or self.gt
+                                                   or getattr(cfg, "ce_push", False) or self.want_logs):
+            raise ValueError("p2p backend: --local-steps runs decent on the fused single-kernel step only")
         self.dbuf = _wants_dbuf(cfg) and self.do_comm
         self.ce_push = bool(getattr(cfg, "ce_push", False)) and self.overlap and cfg.algo == "decent" and self.sync
         self.nvls = self.nvls_step = False      # set in connect() when the window has a multicast mapping
@@ -336,6 +343,7 @@ class P2PBackend(CommBackend):
                 "fsm.enabled": 1 if (cfg.algo in ("event", "spevent") and self.do_comm) else 0,
                 "fsm.metric": 1 if self.drift else 0,
                 "sent": P(self.sent) if (self.drift and self.do_comm) else 0,
+                "local_steps": self.local_steps,
             })
             if self.graph is None:
                 gp.update({
@@ -594,7 +602,8 @@ class P2PBackend(CommBackend):
             self.host_bytes += 2 * sum(self.msg_bytes)
         elif self.gt:
             self.host_bytes += 2 * 2 * self.table.n_elems * 4      # theta and y, to both neighbours
-        elif self.cfg.algo == "decent" and self.do_comm:
+        elif self.cfg.algo == "decent" and self.do_comm and self.pass_num % self.local_steps == 0:
+            # --local-steps H: only every H-th step sends
             self.host_bytes += getattr(self.ring, "fanout", 2) * self.table.n_elems * 4
 
     def step(self) -> None:
@@ -679,6 +688,7 @@ class P2PBackend(CommBackend):
             sd["compress"] = "int8" if self.q8 else "none"
         if self.cfg.algo == "decent":
             sd["gradient_tracking"] = self.gt
+            sd["local_steps"] = self.local_steps
             if self.gt:
                 sd["y"], sd["g_prev"] = self.y.cpu().clone(), self.g_prev.cpu().clone()
                 sd["y_in_l"] = self.win.view("y_in_l", torch.float32).cpu().clone()
@@ -697,6 +707,7 @@ class P2PBackend(CommBackend):
         check_trigger_state(sd, self.metric, self.cfg.algo)
         check_compress_state(sd, "int8" if self.q8 else "none", self.cfg.algo)
         check_tracking_state(sd, self.gt, self.cfg.algo)
+        check_local_steps_state(sd, self.local_steps, self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
@@ -719,7 +730,9 @@ class P2PBackend(CommBackend):
             self.win.view("y_in_r", torch.float32).copy_(sd["y_in_r"].to(self.dev))
         if self.log_ring is not None:
             self._drained = self.pass_num          # log rows of the steps before the checkpoint are not replayed
-        # NOTE: handshake counters (flags / acks) restart from pass_num on every rank
+        # NOTE: handshake counters (flags / acks) restart from pass_num on every rank.  Under --local-steps H the next
+        # gossip step k is the first multiple of H above pass_num, so the WAR bound k - H (one-peer: k - tau * H) is at
+        # most pass_num, and only that round's pushes reach the flag value k
         if self.gossip:
             self._init_norms(run_fsm=False)
             self._reset_handshake(self.pass_num)
