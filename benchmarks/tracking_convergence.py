@@ -1,17 +1,19 @@
 #!/usr/bin/env python
-"""Decent with and without gradient tracking on label-sorted shards, on the CPU (gloo), no timing.
+"""Decent, decent with gradient tracking and decent with exact diffusion on label-sorted shards, on the CPU (gloo), no
+timing.
 
     torchrun --nproc-per-node 4 benchmarks/tracking_convergence.py [--steps 300] [--data synthetic|DIR] [--lr 0.05]
                                                                     [--out file]
 
 Each rank trains MNIST `cnn2` on its own `--partition label` shard (the samples sorted by class, cut into R equal
-blocks: each rank sees two or three of the ten classes) with constant-lr SGD, batch 32 per rank, once with plain decent
-and once with --gradient-tracking, from the same seed.  After --steps steps it reports, per run:
+blocks: each rank sees two or three of the ten classes) with constant-lr SGD, batch 32 per rank, once with plain
+decent, once with --gradient-tracking and once with --exact-diffusion, from the same seed.  After --steps steps it
+reports, per run:
   consensus   sqrt(mean_r ||theta_r - theta_bar||^2) / ||theta_bar||, before the final average
   local_acc   the test accuracy of every rank's own model, before the final average
   avg_acc     the test accuracy of the averaged model
 The default data is the project's synthetic MNIST (class templates plus noise), which may be too easy to separate the
-two algorithms; pass a dataset root with --data for the real set.
+algorithms; pass a dataset root with --data for the real set.
 """
 import argparse
 import json
@@ -28,11 +30,12 @@ from eventgrad_b200.engine.trainer import Trainer  # noqa: E402
 from eventgrad_b200.utils.dist import init_distributed, shutdown  # noqa: E402
 
 
-def run(a, env, tracking: bool) -> dict:
+def run(a, env, tracking: bool, ed: bool = False) -> dict:
     n_train = 32 * a.steps * env.world          # one epoch of a.steps steps
     cfg = preset("decent", device="cpu", backend="gloo", model="cnn2", batch_mode="per_rank", batch_size=32,
                  sampler="random", partition="label", lr=a.lr, momentum=0.0, epochs=1, max_steps=a.steps,
-                 train_samples=n_train, test_samples=a.test_samples, quiet=True, gradient_tracking=tracking)
+                 train_samples=n_train, test_samples=a.test_samples, quiet=True, gradient_tracking=tracking,
+                 exact_diffusion=ed)
     if a.data == "synthetic":
         train, test = synthetic_source("mnist", n_train), synthetic_source("mnist", a.test_samples, train=False)
     else:
@@ -53,7 +56,7 @@ def run(a, env, tracking: bool) -> dict:
     dist.all_gather_object(accs, local)
     dist.all_gather_object(cls, classes)
     res = tr.finalize(evaluate=True)
-    out = {"gradient_tracking": tracking, "world": env.world, "steps": tr.steps_done, "lr": a.lr, "data": a.data,
+    out = {"gradient_tracking": tracking, "exact_diffusion": ed, "world": env.world, "steps": tr.steps_done, "lr": a.lr, "data": a.data,
            "consensus": round(consensus, 6), "local_acc": [round(x, 2) for x in accs],
            "avg_acc": round(float(res.get("test_acc", float("nan"))), 2) if env.rank == 0 else None,
            "classes_per_rank": cls}
@@ -70,7 +73,7 @@ def main():
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     env = init_distributed("cpu")
-    lines = [json.dumps(run(a, env, t)) for t in (False, True)]
+    lines = [json.dumps(run(a, env, t, ed)) for t, ed in ((False, False), (True, False), (False, True))]
     if env.rank == 0:
         print("\n".join(lines), flush=True)
         if a.out:

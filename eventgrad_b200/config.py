@@ -82,6 +82,8 @@ class TrainConfig:
                                      # along y instead of the local gradient (DSGT / DIGing; fused single-slot step)
     local_steps: int = 1             # decent: gossip at every H-th step only (step k iff H divides k); the H - 1 steps
                                      # between are serial SGD steps with no exchange (local / periodic D-PSGD)
+    exact_diffusion: bool = False    # decent on the ring: exact diffusion (D^2 on (I + W) / 2): SGD before the push,
+                                     # gossip phi = p + theta - psi; no heterogeneity bias at decent's bytes
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -236,6 +238,35 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError(f"{h} does not support file_write: the reference's log format records an exchange "
                                  "at every step")
+        if self.exact_diffusion:
+            # the exact-diffusion step exists as the iter-sync fused single-slot ring step (csrc/gossip_ed.cu), in the
+            # torch.distributed backends and in the simulator; sum_r theta_r = sum_r psi_r holds only if every phi a rank
+            # mixes is its neighbour's current one
+            if self.algo in ("event", "spevent"):
+                raise ValueError(f"--exact-diffusion needs algo decent, got {self.algo!r}: a held tensor leaves the "
+                                 "neighbours mixing a stale phi, a difference-form message, which breaks "
+                                 "sum(theta) = sum(psi)")
+            if self.algo != "decent":
+                raise ValueError(f"--exact-diffusion needs algo decent, got {self.algo!r}")
+            if not self.ring_topology:
+                raise ValueError(f"--exact-diffusion runs on the ring only, got topology {self.topology!r}")
+            if self.backend == "refport":
+                raise ValueError("--exact-diffusion is not supported by --backend refport")
+            if self.overlap_push:
+                raise ValueError("--exact-diffusion does not support overlap_push: the message phi needs this step's "
+                                 "gradient, so it cannot be pushed during backward")
+            for name in ("double_buffer", "ce_push"):
+                if getattr(self, name):
+                    raise ValueError(f"--exact-diffusion does not support {name} (fused single-slot step only)")
+            if self.compress != "none":
+                raise ValueError("--exact-diffusion does not support --compress int8")
+            if self.gradient_tracking:
+                raise ValueError("--exact-diffusion does not support --gradient-tracking (both remove the same bias)")
+            if self.local_steps > 1:
+                raise ValueError(f"--exact-diffusion does not support --local-steps {self.local_steps}")
+            if self.file_write:
+                raise ValueError("--exact-diffusion does not support file_write: the reference's log format records "
+                                 "the received theta, and exact diffusion receives phi")
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
@@ -285,7 +316,8 @@ class TrainConfig:
         if c.overlap_push is None:
             kw["overlap_push"] = bool(cuda and p2p and world >= 2 and c.algo in ("decent", "event")
                                       and not bool(c.double_buffer) and c.ring_topology and c.compress == "none"
-                                      and not c.gradient_tracking and c.local_steps == 1)
+                                      and not c.gradient_tracking and c.local_steps == 1
+                                      and not c.exact_diffusion)
         return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
@@ -367,6 +399,10 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--local-steps", type=int, default=None, metavar="H",
                    help="decent: gossip only at every H-th step and take plain local SGD steps in between (local "
                         "D-PSGD); sends 1/H of the bytes (default 1: every step)")
+    p.add_argument("--exact-diffusion", action="store_true", default=None,
+                   help="decent on the ring: exact diffusion (D^2 on (I + W)/2): step before the push and gossip "
+                        "phi = p + theta - psi; removes the bias of constant-lr D-PSGD under heterogeneous data at "
+                        "decent's bytes")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

@@ -173,6 +173,15 @@ struct TrackSlots {
   float* y_to_r;            // peer-mapped: RIGHT neighbour's y_in_l (null on the 2-rank ring)
 };
 
+// Exact diffusion for decent on the ring (csrc/gossip_ed.cu, --exact-diffusion): D^2 on W_bar = (I + W) / 2.  A
+// separate block passed to the ED kernel next to GossipParams, which keeps its ring inbox / push / flag / ack pointers;
+// the pushed message is phi instead of theta:
+//   push  p = sgd_elem(theta_k, g_k, ...),  phi = p + (theta_k - psi),  psi <- p,  phi to both neighbours and to theta
+//   theta_{k+1} = (phi + ((phi + L) + R) / 3) / 2
+struct EdSlots {
+  float* psi;               // local: the previous optimizer output p (theta_0 before the first step)
+};
+
 int gossip_max_grid(int device);  // co-resident CTAs (persistent grid upper bound)
 cudaError_t launch_gossip_step(const GossipParams& p, int grid, cudaStream_t s);
 // experimental double-buffered dense variant (csrc/gossip_dbuf.cu): inbox_l/inbox_r/push_l/push_r address
@@ -196,6 +205,11 @@ cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int g
 // ack pointers and every pointer of `y` (y_to_r null exactly when push_r is null)
 int gossip_gt_max_grid(int device);
 cudaError_t launch_gossip_step_gt(const GossipParams& p, const TrackSlots& y, int grid, cudaStream_t s);
+// exact-diffusion ring step (csrc/gossip_ed.cu): the fused single-kernel decent step that runs the optimizer in the push
+// stage and gossips phi; requires phase 0, sync, do_push, do_mix and send_ack, no sparse block, no `sent`, the trigger
+// off, local_steps <= 1, the ring's inbox / push / flag / ack pointers and `psi`
+int gossip_ed_max_grid(int device);
+cudaError_t launch_gossip_step_ed(const GossipParams& p, const EdSlots& e, int grid, cudaStream_t s);
 // (re)compute tile_ss (+ shadow) from theta and evaluate the trigger for step pass_num+1.
 cudaError_t launch_gossip_init(const GossipParams& p, int grid, int run_fsm, cudaStream_t s);
 // Trigger FSM alone with externally supplied norms (unit tests against the oracle).

@@ -91,6 +91,10 @@ static const std::unordered_map<std::string, Setter<TrackSlots>> kTrack = {
     PTRF(TrackSlots, y_to_l), PTRF(TrackSlots, y_to_r),
 };
 
+static const std::unordered_map<std::string, Setter<EdSlots>> kEd = {
+    PTRF(EdSlots, psi),
+};
+
 static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce = {
     PTRF(AllReduceParams, peer_bufs), PTRF(AllReduceParams, local), PTRF(AllReduceParams, theta),
     PTRF(AllReduceParams, mom), PTRF(AllReduceParams, shadow), PTRF(AllReduceParams, peer_flags),
@@ -178,6 +182,7 @@ PYBIND11_MODULE(_C, m) {
   bind_params<GraphSlots>(m, "GraphSlots", kGraph);
   bind_params<Q8Slots>(m, "Q8Slots", kQ8);
   bind_params<TrackSlots>(m, "TrackSlots", kTrack);
+  bind_params<EdSlots>(m, "EdSlots", kEd);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
   bind_params<SparseParams>(m, "SparseParams", kSparse);
   bind_params<BnParams>(m, "BnParams", kBn);
@@ -207,6 +212,10 @@ PYBIND11_MODULE(_C, m) {
   m.def("gossip_gt_max_grid", &gossip_gt_max_grid);
   m.def("gossip_step_gt", [](const GossipParams& p, const TrackSlots& y, int grid, uintptr_t s) {
     check(launch_gossip_step_gt(p, y, grid, S(s)), "gossip_step_gt");
+  });
+  m.def("gossip_ed_max_grid", &gossip_ed_max_grid);
+  m.def("gossip_step_ed", [](const GossipParams& p, const EdSlots& e, int grid, uintptr_t s) {
+    check(launch_gossip_step_ed(p, e, grid, S(s)), "gossip_step_ed");
   });
   m.def("gossip_init", [](const GossipParams& p, int grid, int run_fsm, uintptr_t s) {
     check(launch_gossip_init(p, grid, run_fsm, S(s)), "gossip_init");

@@ -50,6 +50,12 @@
 // y_k = ((y + yL) + yR) / 3 + (g_k - g_prev) first, stores y and g_prev, mixes theta and hands y_k to sgd_elem in place
 // of the gradient.  The ack of step k covers both inboxes, so there is no new synchronisation variable
 // (PROTOCOL.md 1.8).
+// csrc/gossip_ed.cu defines EG_ED and includes it a sixth time for exact diffusion (`gossip_step_kernel_ed`, decent on
+// the ring, iter-sync fused step only; D^2 on W_bar = (I + W) / 2).  The optimizer moves from the mix to the push: the
+// thread that owns a (tile, warp) slice runs p = sgd_elem(theta_k, g_k, ...) there, forms phi = p + (theta_k - psi),
+// stores psi <- p, the momentum and phi into its own theta and both neighbours' inboxes, all before the unchanged flag.
+// The mix then loads phi back (stored by the same thread), L and R and forms theta_{k+1} = (phi + ((phi + L) + R)/3) / 2
+// with no optimizer.  Handshake, acks and the 2-rank single-copy dedup are the ring's (PROTOCOL.md 1.10).
 // Periodic gossip (GossipParams.local_steps = H > 1, decent, ring and graph builds): step k pushes, flags, waits, mixes
 // and acks only when H divides k; the other steps are the single-pass plain SGD step.  The WAR guard waits for the ack
 // of the previous round (k - H; one-peer: k - tau * H) and the one-peer slot is indexed by the round k / H (PROTOCOL.md
@@ -74,6 +80,11 @@ struct GtStepParams : GossipParams {      // kernel parameter of the tracking bu
   TrackSlots gt;
 };
 using StepParams = GtStepParams;
+#elif defined(EG_ED)
+struct EdStepParams : GossipParams {      // kernel parameter of the exact-diffusion build: the ring block + psi
+  EdSlots ed;
+};
+using StepParams = EdStepParams;
 #else
 using StepParams = GossipParams;
 #endif
@@ -91,6 +102,9 @@ using StepParams = GossipParams;
 #elif defined(EG_GT)
 #define EG_SYM(name) name##_gt
 #define EG_SLOT_OFF(p, step) ((size_t)0)
+#elif defined(EG_ED)
+#define EG_SYM(name) name##_ed
+#define EG_SLOT_OFF(p, step) ((size_t)0)
 #else
 #define EG_SYM(name) name
 #define EG_SLOT_OFF(p, step) ((size_t)0)
@@ -106,7 +120,7 @@ using StepParams = GossipParams;
 #endif
 // Periodic gossip (GossipParams.local_steps = H > 1) exists in the ring and graph builds only; the other builds gossip
 // at every step and their launchers reject H > 1
-#if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT)
+#if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT) || defined(EG_ED)
 #define EG_LOCAL_STEPS 0
 #else
 #define EG_LOCAL_STEPS 1
@@ -360,6 +374,12 @@ __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, cons
     st_f8(p.gt.y_to_r + base, y);
   }
 }
+#elif defined(EG_ED)
+// phi of this thread's 8 elements to both neighbours (ed_push_stage forms it).  push_r == nullptr: 2-rank ring, one copy
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& phi, int /*slot*/) {
+  st_f8(p.push_l + base, phi);
+  if (p.push_r != nullptr) st_f8(p.push_r + base, phi);
+}
 #else
 __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
   // push_r == nullptr: 2-rank ring, the one neighbour is both left and right and reads the single copy twice
@@ -440,6 +460,42 @@ __device__ __forceinline__ F8 load_grad(const StepParams& p, const TileInfo& ti,
   return g;
 }
 
+#ifdef EG_ED
+// Exact diffusion, push stage of one (tile, warp) slice, before its flag: t = theta_k - psi; p = sgd_elem(theta_k, g_k)
+// with this step's lr; psi <- p and the momentum stored; flat mode zeroes the gradient; phi = p + t goes into my theta
+// (the mix of this slice, run later by this thread, reads it back) and to both neighbours
+template <bool kMom>
+__device__ __forceinline__ void ed_push_stage(const StepParams& p, const TileInfo& ti, size_t base, int step) {
+  F8 th, t;
+  {
+    th = ld_f8(p.theta + base);
+    const F8 ps = ld_f8(p.ed.psi + base);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) t.v[e] = __fsub_rn(th.v[e], ps.v[e]);
+  }
+  {
+    const F8 g = load_grad(p, ti, base, threadIdx.x);
+    F8 m;
+    if (kMom) m = ld_f8(p.mom + base);
+    const float lr = sched_lr(p.lr_table, p.lr_len, p.lr, step);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) th.v[e] = sgd_elem<kMom>(th.v[e], g.v[e], m.v[e], lr, p.mu, p.wd, p.nesterov);
+    if (kMom) st_f8(p.mom + base, m);
+  }
+  st_f8(p.ed.psi + base, th);
+  if (p.zero_grad && ti.gptr == nullptr) {
+    F8 z;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) z.v[e] = 0.f;
+    st_f8(p.grad + base, z);
+  }
+#pragma unroll
+  for (int e = 0; e < 8; ++e) th.v[e] = __fadd_rn(th.v[e], t.v[e]);
+  st_f8(p.theta + base, th);
+  push_tile(p, base, th, -1);
+}
+#endif
+
 // mix + SGD + norm-on-write for one tile. `th` already holds theta_k for this thread's 8 floats.  `mix`: p.do_mix of
 // a gossip step, false on a local step of --local-steps (plain SGD); the q8 and tracking builds always mix
 template <bool kMom>
@@ -515,6 +571,17 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
     for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(__fadd_rn(__fadd_rn(th.v[e], L.v[e]), R.v[e]), 3.0f);
   }
   if (kMom) m = ld_f8(p.mom + base);
+#elif defined(EG_ED)
+  // load-only: phi (stored into theta by this thread's push stage), L and R; the optimizer already ran in the push
+  constexpr bool logrecv = false;
+  float ssl = 0.f, ssr = 0.f;
+  {
+    th = ld_f8(p.theta + base);
+    const F8 L = ld_f8_cg(p.inbox_l + base), R = ld_f8_cg(p.inbox_r + base);
+#pragma unroll
+    for (int e = 0; e < 8; ++e)
+      th.v[e] = __fdiv_rn(__fadd_rn(th.v[e], __fdiv_rn(__fadd_rn(__fadd_rn(th.v[e], L.v[e]), R.v[e]), 3.0f)), 2.f);
+  }
 #else
   const bool logrecv = (p.tile_ss_l != nullptr);
   float ssl = 0.f, ssr = 0.f;
@@ -542,6 +609,13 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
     }
   }
 #endif
+#ifdef EG_ED
+  float ss = 0.f;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) ss = __fmaf_rn(th.v[e], th.v[e], ss);
+  st_f8(p.theta + base, th);
+  if (p.shadow != nullptr) st_bf16x8(p.shadow + base, th);
+#else
   // learning rate of this step, looked up per tile (an L1 hit) rather than held in a register across the loop
   const float lr = sched_lr(p.lr_table, p.lr_len, p.lr, step);
   float ss = 0.f;
@@ -559,7 +633,8 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
     for (int e = 0; e < 8; ++e) z.v[e] = 0.f;
     st_f8(p.grad + base, z);
   }
-#if !defined(EG_DBUF) && !defined(EG_GT)
+#endif
+#if !defined(EG_DBUF) && !defined(EG_GT) && !defined(EG_ED)
   if (p.sent != nullptr) {
     // drift trigger: sum (theta_{k+1} - sent)^2 replaces sum theta_{k+1}^2.  sent was stored by this thread's push of
     // this tile (or by the split step's push phase / the sparse compaction, both stream-ordered before this kernel)
@@ -683,7 +758,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   // when it reads the status word.  (Uniform per CTA; the run is over, so a partial step does not matter.)
   if (p.do_push && *reinterpret_cast<volatile int*>(p.status) != EG_OK) return;
 
-#if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT)
+#if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT) || defined(EG_ED)
   if (p.phase != 0 || !(p.sync && push)) return;   // the launcher rejects these; never reached
 #elif defined(EG_GRAPH)
   if (p.phase != 0) return;                        // fused step only (the launcher rejects the rest)
@@ -695,7 +770,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #endif
   __shared__ TileInfo s_ti[EG_TI_CACHE];
   fill_tile_cache(p, s_ti);
-#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT)
+#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT) && !defined(EG_ED)
   // spevent: receive side first -- scatter the records that arrived for this step into the replicas
   // (inbox_l / inbox_r point at them), grid barrier, then the dense mix below reads them tile by tile
   if (p.sparse != nullptr) sparse_apply_prologue(*p.sparse, p.sparse->bar);
@@ -768,11 +843,17 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
     for (int j = 0; j < iters + D; ++j) {
       const int t = b + j * G;
       if (j < iters && t < n_tiles) {
+#ifdef EG_ED
+        constexpr bool fired = true;               // every exact-diffusion step is a full-fire decent step
+#else
         const bool fired = (tile_info(p, s_ti, j, t).flags & 1) != 0;
+#endif
         if (fired) {
           const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
 #ifdef EG_DBUF
           push_tile_slot(p, base, ld_f8(p.theta + base), step);
+#elif defined(EG_ED)
+          ed_push_stage<kMom>(p, tile_info(p, s_ti, j, t), base, step);
 #else
           push_tile(p, base, ld_f8(p.theta + base), slot);
 #endif
@@ -826,6 +907,9 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #ifdef EG_GT
         // the tracking mix loads theta itself, after the y stage: held from here it would spill
         mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot, p.do_mix != 0);
+#elif defined(EG_ED)
+        // the exact-diffusion mix loads phi itself
+        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot, p.do_mix != 0);
 #else
         mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, slot,
                        p.do_mix != 0);
@@ -838,7 +922,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   grid_tail(p, step, slot);
 }
 
-#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT)
+#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT) && !defined(EG_ED)
 // (Re)compute tile partials (+ bf16 shadow) from theta (drift trigger: from theta - sent); optionally evaluate the trigger for the
 // first step.  Used once at start-up and after theta is modified outside the step kernel
 // (checkpoint restore).
@@ -1006,6 +1090,35 @@ cudaError_t launch_gossip_step_gt(const GossipParams& p, const TrackSlots& y, in
     gossip_step_kernel_gt<true><<<grid, EG_THREADS, 0, s>>>(k);
   else
     gossip_step_kernel_gt<false><<<grid, EG_THREADS, 0, s>>>(k);
+  return cudaGetLastError();
+}
+
+#elif defined(EG_ED)   // only the step kernel + its launcher exist in this translation unit
+int gossip_ed_max_grid(int device) {
+  int sms = 0, a = 0, b = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_ed<true>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_ed<false>, EG_THREADS, 0);
+  if (b < a) a = b;
+  if (a < 1) a = 1;
+  return sms * a;
+}
+
+// Exact-diffusion ring step (decent): iter-sync fused step only, every tensor pushed every step.
+cudaError_t launch_gossip_step_ed(const GossipParams& p, const EdSlots& e, int grid, cudaStream_t s) {
+  const bool ptrs = e.psi && p.inbox_l && p.inbox_r && p.push_l && p.flag_from_l && p.flag_from_r && p.flag_to_l &&
+                    p.flag_to_r && p.ack_from_l && p.ack_from_r && p.ack_to_l && p.ack_to_r;
+  if (p.phase != 0 || !p.sync || p.sparse != nullptr || p.sent != nullptr || p.fsm.enabled || !p.do_push || !p.do_mix ||
+      !p.send_ack || !ptrs || p.local_steps > 1)
+    return cudaErrorInvalidValue;
+  EdStepParams k;
+  static_cast<GossipParams&>(k) = p;
+  k.ed = e;
+  eg_count_launch(EG_FAM_GOSSIP, 1);
+  if (p.mu != 0.f && p.mom != nullptr)
+    gossip_step_kernel_ed<true><<<grid, EG_THREADS, 0, s>>>(k);
+  else
+    gossip_step_kernel_ed<false><<<grid, EG_THREADS, 0, s>>>(k);
   return cudaGetLastError();
 }
 

@@ -23,7 +23,8 @@ class RingSimulator:
                  tcfg: Optional[TriggerConfig] = None, lr: float = 1e-2, momentum: float = 0.0,
                  topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
                  weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
-                 offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1):
+                 offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1,
+                 exact_diffusion: bool = False):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -39,7 +40,12 @@ class RingSimulator:
         `local_steps=H` (decent, periodic gossip): step k (1-based) communicates iff H divides k, as round n = k / H --
         exactly the decent step above, with the one-peer graph's active slot (n - 1) mod tau taken from the round.  Every
         other step is the serial step theta <- sgd(theta, g_k): no push, no mix, the inboxes keep what the last round
-        delivered, momentum stays local and the lr table stays indexed by step.  Bytes count at communicating steps only."""
+        delivered, momentum stays local and the lr table stays indexed by step.  Bytes count at communicating steps only.
+        `exact_diffusion=True` (decent on the ring; Yuan et al. 2019, D^2 on W_bar = (I + W) / 2): every rank also keeps
+        psi, theta_0 at start.  Step k runs the unchanged optimizer on theta_k first, p = sgd(theta_k, g_k), then
+        phi = p + (theta_k - psi), psi <- p, pushes phi (decent's bytes) and mixes
+        theta_{k+1} = (phi + mix3_(phi, L, R)) / 2 on the received phi's.  sum_r theta_r = sum_r psi_r after every step.
+        At R = 1 the plain serial step runs.  Any dtype works (float64 for convergence studies)."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -61,6 +67,11 @@ class RingSimulator:
         if local_steps > 1 and (algo != "decent" or self.q8 or gradient_tracking):
             raise ValueError("local steps: decent without compression or gradient tracking only")
         self.local_steps = int(local_steps)
+        if exact_diffusion and (algo != "decent" or not self.graphs[0].is_ring or self.q8 or gradient_tracking
+                                or local_steps > 1):
+            raise ValueError("exact diffusion: decent on the ring, without compression, gradient tracking or local "
+                             "steps, only")
+        self.ed = bool(exact_diffusion) and world > 1
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -98,6 +109,8 @@ class RingSimulator:
             self.g_prev = [torch.zeros_like(theta0) for _ in range(world)]
             self.y_in_l = [torch.zeros_like(theta0) for _ in range(world)]
             self.y_in_r = [torch.zeros_like(theta0) for _ in range(world)]
+        if self.ed:
+            self.psi = [theta0.clone() for _ in range(world)]
         self.drift = self.tcfg.metric == "drift" and algo in ("event", "spevent")
         if self.drift:
             # what each rank's receivers hold: event -- zero like the inboxes; spevent -- prev itself (same tensors)
@@ -160,6 +173,8 @@ class RingSimulator:
             for r in range(R):                                 # serial step / local step of --local-steps
                 self._sgd(r, grads[r])
             return
+        if self.ed:
+            return self._step_ed(grads)
         rnd = self.round_of(self.pass_num)
         # ---- phase 1: every rank decides and "Puts" (uses pre-mix theta_k) --------------
         if self.algo == "decent":
@@ -228,6 +243,25 @@ class RingSimulator:
                 self._sgd(r, self.y[r])
                 continue
             self._sgd(r, grads[r])
+
+    def _step_ed(self, grads) -> None:
+        """Exact diffusion: p = sgd(theta_k, g_k), phi = p + (theta_k - psi), psi <- p; phi goes to both neighbours (the
+        ring's inboxes, decent's bytes); theta_{k+1} = (phi + ((phi + L) + R) / 3) / 2."""
+        R, t = self.R, self.table
+        phis = []
+        for r in range(R):
+            th = self.theta[r].clone()
+            self._sgd(r, grads[r])                             # theta[r] <- p
+            phis.append(self.theta[r].add(th.sub_(self.psi[r])))
+            self.psi[r].copy_(self.theta[r])
+        self.fire_history.append([torch.ones(t.n_tensors, dtype=torch.bool) for _ in range(R)])
+        for r in range(R):
+            self.inbox_r[self.left(r)].copy_(phis[r])         # I am my left neighbour's right
+            self.inbox_l[self.right(r)].copy_(phis[r])        # and my right neighbour's left
+            self.bytes[r] += 2 * t.n_elems * 4
+        for r in range(R):
+            tmix = mix3_(phis[r].clone(), self.inbox_l[r], self.inbox_r[r])
+            self.theta[r].copy_(phis[r].add(tmix).div_(2))
 
     def final_average(self) -> torch.Tensor:
         return torch.stack(self.theta).sum(0) / self.R

@@ -93,6 +93,19 @@ def check_local_steps_state(sd: Dict, local_steps: int, algo: str) -> None:
                          f"{int(local_steps)}; resume with the same --local-steps")
 
 
+def check_exact_diffusion_state(sd: Dict, ed: bool, algo: str) -> None:
+    """Refuse to resume decent state saved under the other --exact-diffusion setting: exact-diffusion state is psi, and
+    its inboxes hold the neighbours' phi rather than their theta.  Checkpoints without an `exact_diffusion` key are plain
+    (their format predates exact diffusion)."""
+    if algo != "decent":
+        return
+    saved = bool(sd.get("exact_diffusion", False))
+    if saved != bool(ed):
+        flag = lambda on: "--exact-diffusion" if on else "no --exact-diffusion"
+        raise ValueError(f"checkpoint was written with {flag(saved)}, this run uses {flag(ed)}; "
+                         "resume with the same --exact-diffusion setting")
+
+
 class CommBackend:
     name = "base"
 

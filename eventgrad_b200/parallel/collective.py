@@ -15,6 +15,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
   --gradient-tracking (decent, ring): theta and y travel in one batched exchange; y_k = (y + yL + yR)/3 + g_k - g_prev,
           and SGD steps along y_k
   --local-steps H (decent): only every H-th step runs the exchange and mix; the others are the SGD update alone
+  --exact-diffusion (decent, ring): p = SGD(theta), phi = p + (theta - psi), psi <- p; phi travels in the ring exchange,
+          and theta <- (phi + (phi + L + R)/3) / 2
 
 torch.distributed has no one-sided RMA, so the "window" is emulated with an iteration-
 synchronous exchange: first the fire masks, then a payload holding only the fired tensors.
@@ -29,8 +31,8 @@ from typing import List
 import torch
 import torch.distributed as dist
 
-from .base import (CommBackend, StepLog, check_compress_state, check_local_steps_state, check_topology_state,
-                   check_tracking_state, check_trigger_state)
+from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_local_steps_state,
+                   check_topology_state, check_tracking_state, check_trigger_state)
 from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode, q8_encode,
                       q8_msg_bytes, sgd_, topk_select, trigger_step)
 
@@ -83,6 +85,11 @@ class CollectiveBackend(CommBackend):
         if self.gt:
             self.y, self.g_prev = torch.zeros_like(arena.theta), torch.zeros_like(arena.theta)
             self.y_in_l, self.y_in_r = torch.zeros_like(arena.theta), torch.zeros_like(arena.theta)
+        # --exact-diffusion (decent, ring): psi, the previous optimizer output, starts at theta_0 (identical on every
+        # rank).  R = 1 runs the plain step
+        self.ed = cfg.algo == "decent" and bool(getattr(cfg, "exact_diffusion", False)) and ring.world > 1
+        if self.ed:
+            self.psi = arena.theta.clone()
         # --local-steps H (decent): step k gossips iff H divides k, as round k / H; the other steps are _opt() alone
         self.local_steps = int(getattr(cfg, "local_steps", 1)) if cfg.algo == "decent" else 1
         if self.want_logs:
@@ -187,6 +194,8 @@ class CollectiveBackend(CommBackend):
             return self._step_q8([True] * a.table.n_tensors, None)
         if self.gt:
             return self._step_tracking()
+        if self.ed:
+            return self._step_ed()
         if hasattr(self, "inbox"):
             self._exchange_slots(a.theta, self.inbox)
             self.bytes += self.ring.fanout * a.table.n_elems * 4
@@ -209,6 +218,18 @@ class CollectiveBackend(CommBackend):
         mix3_(a.theta, self.inbox_l, self.inbox_r)
         sgd_(a.theta, self.y, a.mom, self.step_lr(self.pass_num), self.cfg.momentum, self.cfg.weight_decay,
              self.cfg.nesterov)
+
+    def _step_ed(self) -> None:
+        """Exact diffusion, the simulator's ops: p = SGD(theta_k), phi = p + (theta_k - psi), psi <- p, phi to both
+        neighbours in the ring exchange, theta <- (phi + mix3_(phi, L, R)) / 2."""
+        a = self.arena
+        t = a.theta.clone()
+        self._opt()                                    # theta <- p
+        phi = a.theta.add(t.sub_(self.psi))
+        self.psi.copy_(a.theta)
+        self._exchange([phi], [phi], [self.inbox_l], [self.inbox_r])
+        self.bytes += 2 * a.table.n_elems * 4
+        a.theta.copy_(phi.add(mix3_(phi.clone(), self.inbox_l, self.inbox_r)).div_(2))
 
     def _fire(self):
         a = self.arena
@@ -433,9 +454,12 @@ class CollectiveBackend(CommBackend):
         if self.cfg.algo == "decent":
             sd["gradient_tracking"] = self.gt
             sd["local_steps"] = self.local_steps
+            sd["exact_diffusion"] = self.ed
             if self.gt:
                 for k in ("y", "g_prev", "y_in_l", "y_in_r"):
                     sd[k] = getattr(self, k).cpu().clone()
+            if self.ed:
+                sd["psi"] = self.psi.cpu().clone()
         if self.cfg.algo in ("decent", "event"):
             sd["compress"] = self.compress          # int8: prev / rep_l / rep_r are saved above
         if self.cfg.algo in ("event", "spevent"):
@@ -459,7 +483,10 @@ class CollectiveBackend(CommBackend):
         check_compress_state(sd, self.compress, self.cfg.algo)
         check_tracking_state(sd, self.gt, self.cfg.algo)
         check_local_steps_state(sd, self.local_steps, self.cfg.algo)
+        check_exact_diffusion_state(sd, self.ed, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
+        if self.ed:
+            self.psi.copy_(sd["psi"].to(self.psi.device))
         if self.gt:
             for k in ("y", "g_prev", "y_in_l", "y_in_r"):
                 getattr(self, k).copy_(sd[k].to(getattr(self, k).device))

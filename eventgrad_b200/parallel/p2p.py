@@ -12,6 +12,8 @@ Per training step, after backward():
            add the delta to their replicas of prev, and the mix reads the replicas)
            (--gradient-tracking, decent on the ring: csrc/gossip_gt.cu also pushes y_{k-1} before the same flag, forms
            y_k = (y + yL + yR)/3 + g_k - g_prev and steps along y_k)
+           (--exact-diffusion, decent on the ring: csrc/gossip_ed.cu runs SGD in the push stage, pushes
+           phi = p + theta_k - psi, psi <- p, and mixes theta = (phi + (phi + L + R)/3) / 2)
   spevent  batched segmented radix-select top-k + compaction straight into the neighbours'
            inboxes, scatter of arrived records into replicas, then the dense mix+SGD kernel
 No NCCL/MPI call, no separate elementwise kernel and no host synchronisation on that path
@@ -24,8 +26,8 @@ from typing import List
 import torch
 
 from .arena import TILE, ParamArena, TensorTable
-from .base import (CommBackend, StepLog, check_compress_state, check_local_steps_state, check_topology_state,
-                   check_tracking_state, check_trigger_state)
+from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_local_steps_state,
+                   check_topology_state, check_tracking_state, check_trigger_state)
 from .topology import Graph
 from .trigger import q8_msg_bytes
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
@@ -52,7 +54,7 @@ def _wants_dbuf(cfg) -> bool:
     return ((db is None or bool(db)) and cfg.algo == "decent" and cfg.sync_mode == "iter"
             and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True)
             and not _wants_q8(cfg) and not getattr(cfg, "gradient_tracking", False)
-            and getattr(cfg, "local_steps", 1) == 1)
+            and getattr(cfg, "local_steps", 1) == 1 and not getattr(cfg, "exact_diffusion", False))
 
 
 def _wants_q8(cfg) -> bool:
@@ -64,6 +66,12 @@ def _wants_gt(cfg, world: int) -> bool:
     """--gradient-tracking: decent on the ring of >= 2 ranks runs the tracking step of csrc/gossip_gt.cu (at R = 1
     tracking is plain SGD on the gradient, the existing path)."""
     return bool(getattr(cfg, "gradient_tracking", False)) and cfg.algo == "decent" and world > 1
+
+
+def _wants_ed(cfg, world: int) -> bool:
+    """--exact-diffusion: decent on the ring of >= 2 ranks runs the exact-diffusion step of csrc/gossip_ed.cu (at R = 1
+    it is the plain serial step, the existing path)."""
+    return bool(getattr(cfg, "exact_diffusion", False)) and cfg.algo == "decent" and world > 1
 
 
 def _graph_of(cfg, rank: int, world: int):
@@ -100,6 +108,8 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None)
         if _wants_gt(cfg, world):
             lay.add("y_in_l", n)                  # gradient tracking: y from each neighbour
             lay.add("y_in_r", n)
+        if _wants_ed(cfg, world):
+            lay.add("psi", n)                     # exact diffusion: the previous optimizer output (this rank only)
     if cfg.algo == "spevent":
         K = sum(table.topk_counts(cfg.topk_percent))
         lay.add("rec_from_l", 2 * K * 4)
@@ -134,6 +144,8 @@ def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
         max_grid = min(max_grid, C.gossip_q8_max_grid(env.device.index or 0))
     if _wants_gt(cfg, env.world):
         max_grid = min(max_grid, C.gossip_gt_max_grid(env.device.index or 0))
+    if _wants_ed(cfg, env.world):
+        max_grid = min(max_grid, C.gossip_ed_max_grid(env.device.index or 0))
     lay = build_layout(table, cfg, env.world, max_grid, graph)
     symm = wants_symm_window(env) and bootstrap is None      # NVLS path: torch symmetric memory + multicast mapping
     win = (SymmWindow if symm else Window)(lay, env.rank, env.world, env.device)
@@ -190,11 +202,16 @@ class P2PBackend(CommBackend):
         if self.gt and (self.graph is not None or self.overlap or getattr(cfg, "ce_push", False) or self.want_logs
                         or not self.sync or self.q8):
             raise ValueError("p2p backend: --gradient-tracking runs decent on the ring's fused iter-sync step only")
+        # --exact-diffusion: the iter-sync fused single-slot ring step of csrc/gossip_ed.cu
+        self.ed = _wants_ed(cfg, ring.world) and self.do_comm
+        if self.ed and (self.graph is not None or self.overlap or getattr(cfg, "ce_push", False) or self.want_logs
+                        or not self.sync or self.q8 or self.gt):
+            raise ValueError("p2p backend: --exact-diffusion runs decent on the ring's fused iter-sync step only")
         # --local-steps H (decent): the fused single-slot ring / graph step gossips at every H-th step only; the
         # kernel takes that choice from its device step counter, so one captured launch serves the whole cycle
         self.local_steps = int(getattr(cfg, "local_steps", 1)) if cfg.algo == "decent" else 1
         if getattr(cfg, "local_steps", 1) > 1 and (cfg.algo != "decent" or self.overlap or self.q8 or self.gt
-                                                   or getattr(cfg, "ce_push", False) or self.want_logs):
+                                                   or self.ed or getattr(cfg, "ce_push", False) or self.want_logs):
             raise ValueError("p2p backend: --local-steps runs decent on the fused single-kernel step only")
         self.dbuf = _wants_dbuf(cfg) and self.do_comm
         self.ce_push = bool(getattr(cfg, "ce_push", False)) and self.overlap and cfg.algo == "decent" and self.sync
@@ -267,6 +284,11 @@ class P2PBackend(CommBackend):
         if self.gt:
             # y, the previous gradient (fp32 whatever the gradient dtype) and the y inboxes start at zero on every rank
             self.y, self.g_prev = zf(t.n_padded), zf(t.n_padded)
+        self.psi = None
+        if self.ed:
+            # psi starts at theta_0, which is identical on every rank
+            self.psi = self.win.view("psi", torch.float32)
+            self.psi.copy_(arena.theta)
         # drift trigger (--trigger drift): the FSM reads ||theta - sent||.  event: `sent` is an arena-sized buffer,
         # zero like the receivers' inboxes, that the step kernel's pushes keep equal to what was last pushed; spevent:
         # `prev` already is what the receivers hold, element by element
@@ -285,7 +307,7 @@ class P2PBackend(CommBackend):
         self._grads_alive = None
         self.host_bytes = 0
         self._connected = False
-        self.gp = self.ap = self.ap_avg = self.sp = self.gs = self.qs = self.ts = None
+        self.gp = self.ap = self.ap_avg = self.sp = self.gs = self.qs = self.ts = self.es = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
@@ -401,6 +423,11 @@ class P2PBackend(CommBackend):
                                "y_to_l": win.addr("y_in_r", L),
                                "y_to_r": 0 if self.wire_dedup else win.addr("y_in_l", R)})
                     self.ts = ts
+                if self.ed:
+                    # phi travels in theta's inboxes, the single-copy dedup of the 2-rank ring included
+                    es = C.EdSlots()
+                    es.update({"psi": P(self.psi)})
+                    self.es = es
             elif self.sparse:
                 gp.update({"inbox_l": P(self.rep_l), "inbox_r": P(self.rep_r)})
             self.gp = gp
@@ -584,6 +611,8 @@ class P2PBackend(CommBackend):
                 C.gossip_step_q8(self.gp, self.qs, self.grid, s)
             elif self.gt:
                 C.gossip_step_gt(self.gp, self.ts, self.grid, s)
+            elif self.ed:
+                C.gossip_step_ed(self.gp, self.es, self.grid, s)
             elif self.overlap:
                 C.gossip_step_phase(self.gp, 2, self.grid, s)
             elif self.dbuf:
@@ -689,6 +718,9 @@ class P2PBackend(CommBackend):
         if self.cfg.algo == "decent":
             sd["gradient_tracking"] = self.gt
             sd["local_steps"] = self.local_steps
+            sd["exact_diffusion"] = self.ed
+            if self.ed:
+                sd["psi"] = self.psi.cpu().clone()
             if self.gt:
                 sd["y"], sd["g_prev"] = self.y.cpu().clone(), self.g_prev.cpu().clone()
                 sd["y_in_l"] = self.win.view("y_in_l", torch.float32).cpu().clone()
@@ -708,6 +740,7 @@ class P2PBackend(CommBackend):
         check_compress_state(sd, "int8" if self.q8 else "none", self.cfg.algo)
         check_tracking_state(sd, self.gt, self.cfg.algo)
         check_local_steps_state(sd, self.local_steps, self.cfg.algo)
+        check_exact_diffusion_state(sd, self.ed, self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
@@ -728,6 +761,8 @@ class P2PBackend(CommBackend):
             self.g_prev.copy_(sd["g_prev"].to(self.dev))
             self.win.view("y_in_l", torch.float32).copy_(sd["y_in_l"].to(self.dev))
             self.win.view("y_in_r", torch.float32).copy_(sd["y_in_r"].to(self.dev))
+        if self.ed:
+            self.psi.copy_(sd["psi"].to(self.dev))
         if self.log_ring is not None:
             self._drained = self.pass_num          # log rows of the steps before the checkpoint are not replayed
         # NOTE: handshake counters (flags / acks) restart from pass_num on every rank.  Under --local-steps H the next
