@@ -1,13 +1,14 @@
 #!/usr/bin/env python
-"""Decent, decent with gradient tracking and decent with exact diffusion on label-sorted shards, on the CPU (gloo), no
-timing.
+"""Decent, decent with gradient tracking, decent with exact diffusion and decent with periodic global averaging on
+label-sorted shards, on the CPU (gloo), no timing.
 
     torchrun --nproc-per-node 4 benchmarks/tracking_convergence.py [--steps 300] [--data synthetic|DIR] [--lr 0.05]
-                                                                    [--out file]
+                                                                    [--global-avg-periods 4,16] [--out file]
 
 Each rank trains MNIST `cnn2` on its own `--partition label` shard (the samples sorted by class, cut into R equal
 blocks: each rank sees two or three of the ten classes) with constant-lr SGD, batch 32 per rank, once with plain
-decent, once with --gradient-tracking and once with --exact-diffusion, from the same seed.  After --steps steps it
+decent, once with --gradient-tracking, once with --exact-diffusion and once per --global-avg-period P in
+--global-avg-periods (every P-th step an exact average over all ranks), from the same seed.  After --steps steps it
 reports, per run:
   consensus   sqrt(mean_r ||theta_r - theta_bar||^2) / ||theta_bar||, before the final average
   local_acc   the test accuracy of every rank's own model, before the final average
@@ -30,12 +31,12 @@ from eventgrad_b200.engine.trainer import Trainer  # noqa: E402
 from eventgrad_b200.utils.dist import init_distributed, shutdown  # noqa: E402
 
 
-def run(a, env, tracking: bool, ed: bool = False) -> dict:
+def run(a, env, tracking: bool, ed: bool = False, P: int = 0) -> dict:
     n_train = 32 * a.steps * env.world          # one epoch of a.steps steps
     cfg = preset("decent", device="cpu", backend="gloo", model="cnn2", batch_mode="per_rank", batch_size=32,
                  sampler="random", partition="label", lr=a.lr, momentum=0.0, epochs=1, max_steps=a.steps,
                  train_samples=n_train, test_samples=a.test_samples, quiet=True, gradient_tracking=tracking,
-                 exact_diffusion=ed)
+                 exact_diffusion=ed, global_avg_period=P)
     if a.data == "synthetic":
         train, test = synthetic_source("mnist", n_train), synthetic_source("mnist", a.test_samples, train=False)
     else:
@@ -56,7 +57,8 @@ def run(a, env, tracking: bool, ed: bool = False) -> dict:
     dist.all_gather_object(accs, local)
     dist.all_gather_object(cls, classes)
     res = tr.finalize(evaluate=True)
-    out = {"gradient_tracking": tracking, "exact_diffusion": ed, "world": env.world, "steps": tr.steps_done, "lr": a.lr, "data": a.data,
+    out = {"gradient_tracking": tracking, "exact_diffusion": ed, "global_avg_period": P, "world": env.world,
+           "steps": tr.steps_done, "lr": a.lr, "data": a.data,
            "consensus": round(consensus, 6), "local_acc": [round(x, 2) for x in accs],
            "avg_acc": round(float(res.get("test_acc", float("nan"))), 2) if env.rank == 0 else None,
            "classes_per_rank": cls}
@@ -70,10 +72,13 @@ def main():
     ap.add_argument("--lr", type=float, default=0.05)
     ap.add_argument("--data", default="synthetic")
     ap.add_argument("--test-samples", type=int, default=2000)
+    ap.add_argument("--global-avg-periods", default="4,16", help="comma-separated P of the global-averaging runs")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     env = init_distributed("cpu")
-    lines = [json.dumps(run(a, env, t, ed)) for t, ed in ((False, False), (True, False), (False, True))]
+    runs = [(False, False, 0), (True, False, 0), (False, True, 0)]
+    runs += [(False, False, int(P)) for P in a.global_avg_periods.split(",") if P]
+    lines = [json.dumps(run(a, env, t, ed, P)) for t, ed, P in runs]
     if env.rank == 0:
         print("\n".join(lines), flush=True)
         if a.out:

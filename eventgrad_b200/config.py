@@ -84,6 +84,8 @@ class TrainConfig:
                                      # between are serial SGD steps with no exchange (local / periodic D-PSGD)
     exact_diffusion: bool = False    # decent on the ring: exact diffusion (D^2 on (I + W) / 2): SGD before the push,
                                      # gossip phi = p + theta - psi; no heterogeneity bias at decent's bytes
+    global_avg_period: int = 0       # decent on the ring / a static graph: every P-th step (P >= 2) averages theta over
+                                     # all ranks exactly in place of the gossip mix (Gossip-PGA); 0 = off
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -267,6 +269,38 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError("--exact-diffusion does not support file_write: the reference's log format records "
                                  "the received theta, and exact diffusion receives phi")
+        P = self.global_avg_period
+        if isinstance(P, bool) or not isinstance(P, int) or P < 0:
+            raise ValueError(f"--global-avg-period must be an integer >= 0, got {P!r}")
+        if P == 1:
+            raise ValueError("--global-avg-period 1 averages at every step and leaves no gossip: use algo cent")
+        if P:
+            # periodic global averaging exists for decent in the fused single-kernel ring / static-graph step (the gated
+            # all-reduce of csrc/allreduce.cu before csrc/gossip.cu, csrc/gossip_graph.cu), the torch.distributed
+            # backends and the simulator
+            h = f"--global-avg-period {P}"
+            if self.algo != "decent":
+                raise ValueError(f"{h} needs algo decent, got {self.algo!r}")
+            if str(self.topology).strip().lower() == "onepeer-exp":
+                raise ValueError(f"{h} does not support topology onepeer-exp: it already reaches the exact average "
+                                 "every tau steps at power-of-two R, and its per-slot WAR bound has no rule for skipped "
+                                 "steps")
+            if self.gradient_tracking:
+                raise ValueError(f"{h} does not support --gradient-tracking")
+            if self.exact_diffusion:
+                raise ValueError(f"{h} does not support --exact-diffusion")
+            if self.compress != "none":
+                raise ValueError(f"{h} does not support --compress int8")
+            if self.local_steps > 1:
+                raise ValueError(f"{h} does not support --local-steps {self.local_steps}")
+            if self.backend == "refport":
+                raise ValueError(f"{h} is not supported by --backend refport")
+            for name in ("overlap_push", "double_buffer", "ce_push"):
+                if getattr(self, name):
+                    raise ValueError(f"{h} does not support {name} (fused single-kernel step only)")
+            if self.file_write:
+                raise ValueError(f"{h} does not support file_write: the reference's log format records a neighbour "
+                                 "exchange at every step")
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
@@ -317,7 +351,7 @@ class TrainConfig:
             kw["overlap_push"] = bool(cuda and p2p and world >= 2 and c.algo in ("decent", "event")
                                       and not bool(c.double_buffer) and c.ring_topology and c.compress == "none"
                                       and not c.gradient_tracking and c.local_steps == 1
-                                      and not c.exact_diffusion)
+                                      and not c.exact_diffusion and not c.global_avg_period)
         return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
@@ -403,6 +437,9 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
                    help="decent on the ring: exact diffusion (D^2 on (I + W)/2): step before the push and gossip "
                         "phi = p + theta - psi; removes the bias of constant-lr D-PSGD under heterogeneous data at "
                         "decent's bytes")
+    p.add_argument("--global-avg-period", type=int, default=None, metavar="P",
+                   help="decent on the ring or a static graph: every P-th step (P >= 2) replaces the gossip mix with "
+                        "an exact average of the parameters over all ranks (Gossip-PGA; default 0: off)")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

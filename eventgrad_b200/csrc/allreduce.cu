@@ -99,6 +99,9 @@ __device__ __forceinline__ void nvls_broadcast_tile(float* mc, const F8& a) {
 template <bool kMom>
 __global__ void __launch_bounds__(EG_THREADS, 4) EG_AR_SYM(allreduce_kernel)(const AllReduceParams p) {
   const int b = blockIdx.x, G = gridDim.x, tid = threadIdx.x;
+  // step gate (--global-avg-period): not an averaging step -> no barrier, no load, no store, no counter; uniform over
+  // the grid and, through the equal pass counters, over the ranks (PROTOCOL.md 1.11)
+  if (p.gate_period > 0 && (*p.gate_pass + 1) % p.gate_period != 0) return;
   const uint32_t seq = (uint32_t)(*p.step_ctr) + 1u;
   // SGD mode: training step of this launch (the rank's device pass counter, advanced in the tail below)
   const int step = (p.pass_num != nullptr) ? *p.pass_num + 1 : 0;
@@ -159,6 +162,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_AR_SYM(allreduce_kernel)(con
 
 #ifndef EG_NVLS
 cudaError_t launch_allreduce(const AllReduceParams& p, int grid, cudaStream_t s) {
+  if (p.gate_period < 0 || (p.gate_period > 0 && p.gate_pass == nullptr)) return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_ALLREDUCE, 1);
   if (p.mode == 1 && p.mu != 0.f && p.mom != nullptr)
     allreduce_kernel<true><<<grid, EG_THREADS, 0, s>>>(p);
@@ -171,6 +175,7 @@ cudaError_t launch_allreduce(const AllReduceParams& p, int grid, cudaStream_t s)
 cudaError_t launch_allreduce_nvls(const AllReduceParams& p, int grid, cudaStream_t s) {
   eg_count_launch(EG_FAM_ALLREDUCE, 1);
   if (!p.two_shot || p.mc_local == nullptr) return cudaErrorInvalidValue;
+  if (p.gate_period < 0 || (p.gate_period > 0 && p.gate_pass == nullptr)) return cudaErrorInvalidValue;
   if (p.mode == 1 && p.mu != 0.f && p.mom != nullptr)
     allreduce_kernel_nvls<true><<<grid, EG_THREADS, 0, s>>>(p);
   else

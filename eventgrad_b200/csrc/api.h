@@ -59,7 +59,10 @@ struct SparseParams;
 // shadow, zero grad) accumulating per-warp sum-of-squares -> last CTA evaluates the trigger FSM
 // for step k+1 from those partials.  Replaces, per step, 86x{norm.item(), 2 MPI_Put, 2 memcpy,
 // add_, add_, div_} + optimizer.step() of the reference.
-struct GossipParams {
+// GossipCore is the block every step kernel reads; GossipParams appends the fields that only the ring and graph kernels
+// read.  The int8, tracking and exact-diffusion kernels take GossipCore followed by their own slots (their launchers
+// slice it out of GossipParams), so those slots keep the offsets they had when GossipCore was all of GossipParams.
+struct GossipCore {
   float* theta;
   float* grad;
   float* mom;               // may be null when mu == 0
@@ -117,6 +120,14 @@ struct GossipParams {
   // here, and the norm-on-write partials are sum (theta_{k+1} - sent)^2; spevent: the sparse `prev` (written by the
   // compaction, never by the step kernel).  null: the norm rule, no extra loads or stores
   float* sent;
+};
+
+struct GossipParams : GossipCore {
+  // periodic global averaging (--global-avg-period P >= 2, decent on the ring and on static graphs): at step k with P
+  // dividing k the gated all-reduce launched just before the step kernel has already replaced theta by the rank mean,
+  // and the step kernel takes the plain SGD step (no push, no flag, no ack, no mix).  0: off.  The WAR guard of the
+  // next gossip step waits for the ack of k - 1 (PROTOCOL.md 1.11)
+  int global_avg_period;
 };
 
 // Circulant gossip graph beyond the ring (csrc/gossip_graph.cu): the 2|O| inbox slots that replace the ring's
@@ -245,6 +256,12 @@ struct AllReduceParams {
   const float* lr_table;
   int lr_len;
   int* pass_num;
+  // step gate (--global-avg-period): gate_period > 0 makes every CTA read *gate_pass + 1, the 1-based step about to
+  // run, and return before its first cross-rank barrier unless gate_period divides it -- without touching step_ctr or
+  // the ticket, so a skipped launch leaves no trace.  gate_pass is the rank's gossip pass counter, which iter-sync keeps
+  // equal on every rank, so every rank skips the same launches.  0: every launch averages
+  const int* gate_pass;
+  int gate_period;
 };
 cudaError_t launch_allreduce(const AllReduceParams& p, int grid, cudaStream_t s);
 // experimental NVLink-SHARP variant (csrc/allreduce_nvls.cu): multimem.ld_reduce + multimem.st, two-shot only

@@ -65,7 +65,7 @@ static const std::unordered_map<std::string, Setter<GossipParams>> kGossip = {
     NUMF(GossipParams, send_ack), NUMF(GossipParams, zero_grad), NUMF(GossipParams, group_iters),
     PTRF(GossipParams, sparse), NUMF(GossipParams, need_norm), NUMF(GossipParams, phase), TAB_FIELDS(GossipParams),
     NUMF(GossipParams, wd), NUMF(GossipParams, nesterov), PTRF(GossipParams, lr_table), NUMF(GossipParams, lr_len),
-    NUMF(GossipParams, local_steps), PTRF(GossipParams, sent),
+    NUMF(GossipParams, local_steps), PTRF(GossipParams, sent), NUMF(GossipParams, global_avg_period),
     PTRF2(GossipParams, fsm, thres), PTRF2(GossipParams, fsm, last_norm), PTRF2(GossipParams, fsm, last_iter),
     PTRF2(GossipParams, fsm, slopes), PTRF2(GossipParams, fsm, fire), PTRF2(GossipParams, fsm, cur_norm),
     PTRF2(GossipParams, fsm, counters), PTRF2(GossipParams, fsm, pass_num), PTRF2(GossipParams, fsm, log_ring),
@@ -105,6 +105,7 @@ static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce
     NUMF(AllReduceParams, zero_after), PTRF(AllReduceParams, mc_local),
     NUMF(AllReduceParams, wd), NUMF(AllReduceParams, nesterov), PTRF(AllReduceParams, lr_table),
     NUMF(AllReduceParams, lr_len), PTRF(AllReduceParams, pass_num),
+    PTRF(AllReduceParams, gate_pass), NUMF(AllReduceParams, gate_period),
 };
 
 static const std::unordered_map<std::string, Setter<SparseParams>> kSparse = {

@@ -38,8 +38,9 @@ __global__ void ce_publish_pushed_kernel(const GossipParams p) {
 }
 
 cudaError_t launch_ce_push(const GossipParams& p, cudaStream_t s) {
-  // push_r null: 2-rank ring, one copy.  Every step pushes: no --local-steps
-  if (p.push_l == nullptr || p.fsm.enabled || p.local_steps > 1) return cudaErrorInvalidValue;
+  // push_r null: 2-rank ring, one copy.  Every step pushes: no --local-steps, no --global-avg-period
+  if (p.push_l == nullptr || p.fsm.enabled || p.local_steps > 1 || p.global_avg_period != 0)
+    return cudaErrorInvalidValue;
   const size_t nbytes = (size_t)p.tab.n_tiles * EG_TILE * sizeof(float);
   eg_count_launch(EG_FAM_GOSSIP, 2);
   ce_wait_acks_kernel<<<1, 32, 0, s>>>(p);

@@ -60,6 +60,12 @@
 // and acks only when H divides k; the other steps are the single-pass plain SGD step.  The WAR guard waits for the ack
 // of the previous round (k - H; one-peer: k - tau * H) and the one-peer slot is indexed by the round k / H (PROTOCOL.md
 // 1.9).
+// Periodic global averaging (GossipParams.global_avg_period = P >= 2, decent, ring and static-graph builds): at step k
+// with P dividing k, the gated all-reduce enqueued before this kernel (csrc/allreduce.cu, gate_period = P) has already
+// replaced theta by the rank mean, and this kernel takes the same single-pass plain SGD step as a local step.  The
+// other steps gossip; their WAR guard waits for the ack of the last step that gossiped (PROTOCOL.md 1.11).
+// The int8, tracking and exact-diffusion builds derive their parameter block from GossipCore, which has no
+// global_avg_period, so their slots keep their offsets; the launchers of every build but the ring and graph refuse P.
 #include "api.h"
 #include "common.cuh"
 #include "sparse_apply.cuh"
@@ -71,17 +77,17 @@ struct GraphStepParams : GossipParams {   // kernel parameter of the graph build
 };
 using StepParams = GraphStepParams;
 #elif defined(EG_Q8)
-struct Q8StepParams : GossipParams {      // kernel parameter of the q8 build: the ring block + the int8 slots
+struct Q8StepParams : GossipCore {        // kernel parameter of the q8 build: the ring block + the int8 slots
   Q8Slots q;
 };
 using StepParams = Q8StepParams;
 #elif defined(EG_GT)
-struct GtStepParams : GossipParams {      // kernel parameter of the tracking build: the ring block + the y slots
+struct GtStepParams : GossipCore {        // kernel parameter of the tracking build: the ring block + the y slots
   TrackSlots gt;
 };
 using StepParams = GtStepParams;
 #elif defined(EG_ED)
-struct EdStepParams : GossipParams {      // kernel parameter of the exact-diffusion build: the ring block + psi
+struct EdStepParams : GossipCore {        // kernel parameter of the exact-diffusion build: the ring block + psi
   EdSlots ed;
 };
 using StepParams = EdStepParams;
@@ -128,11 +134,19 @@ using StepParams = GossipParams;
 
 namespace egb {
 
-// Does 1-based step `step` gossip?  --local-steps H: iff H divides it.  Re-evaluated where it is needed instead of held
-// in a register across the tile loops
+#if EG_LOCAL_STEPS
+// Is 1-based step `step` a global-averaging step (--global-avg-period P: iff P divides it)?  The launchers refuse P = 1
+// and P < 0, so P > 0 means P >= 2
+__device__ __forceinline__ bool global_avg_step(const StepParams& p, int step) {
+  return p.global_avg_period > 0 && step % p.global_avg_period == 0;
+}
+#endif
+
+// Does 1-based step `step` gossip?  --local-steps H: iff H divides it; --global-avg-period P: iff P does not divide it.
+// Re-evaluated where it is needed instead of held in a register across the tile loops
 __device__ __forceinline__ bool gossip_step_comm(const StepParams& p, int step) {
 #if EG_LOCAL_STEPS
-  return p.local_steps <= 1 || step % p.local_steps == 0;
+  return (p.local_steps <= 1 || step % p.local_steps == 0) && !global_avg_step(p, step);
 #else
   return true;
 #endif
@@ -742,8 +756,9 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   const int b = blockIdx.x, G = gridDim.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int step = *p.fsm.pass_num + 1;
-  // --local-steps H: step k gossips iff H divides k, as round k / H; every other step is the serial SGD step.  A uniform
-  // branch on the device pass counter, which iter-sync keeps equal on every rank (PROTOCOL.md 1.9)
+  // --local-steps H: step k gossips iff H divides k, as round k / H; every other step is the serial SGD step.
+  // --global-avg-period P: a step with P dividing k is the serial SGD step on the averaged theta.  A uniform branch on
+  // the device pass counter, which iter-sync keeps equal on every rank (PROTOCOL.md 1.9, 1.11)
   const bool comm = gossip_step_comm(p, step);
 #if EG_LOCAL_STEPS
   const int H = max(p.local_steps, 1);
@@ -809,9 +824,12 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
     if (tid == 0) {
       // WAR guard: every peer I push into must have consumed what I last pushed into its slot before I overwrite
       // it -- at step-1 on a static graph, at step-period on a one-peer graph (slot m is written every period steps);
-      // with --local-steps H the last push into a slot was H (static) or period * H (one-peer) steps ago
+      // with --local-steps H the last push into a slot was H (static) or period * H (one-peer) steps ago; with
+      // --global-avg-period P one step ago, or two when the step before was an average (static graphs only)
       bool ok = true;
-      const int prev = max(step - (p.g.period ? p.g.period : 1) * H, 0);   // the first round(s) wait for nothing
+      int last = step - (p.g.period ? p.g.period : 1) * H;
+      if (global_avg_step(p, step - 1)) last -= 1;
+      const int prev = max(last, 0);                                       // the first round(s) wait for nothing
 #pragma unroll
       for (int k = 0; k < EG_MAX_SLOTS; ++k)
         if (slot_on(p, k, slot)) ok = wait_ge(p.g.ack_from[k], (uint32_t)prev, p.status, p.timeout_ns) && ok;
@@ -823,9 +841,9 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
     __shared__ int s_ok;
     if (tid == 0) {
       // WAR guard: neighbours must have consumed what I pushed at step-1 (--local-steps H: at step-H, the last
-      // round) before I overwrite it
+      // round; --global-avg-period P: at step-2 when step-1 was an average) before I overwrite it
 #if EG_LOCAL_STEPS
-      const uint32_t prev = (uint32_t)max(step - H, 0);
+      const uint32_t prev = (uint32_t)max(step - H - (global_avg_step(p, step - 1) ? 1 : 0), 0);
 #else
       const uint32_t prev = (uint32_t)(step - 1);
 #endif
@@ -984,6 +1002,11 @@ cudaError_t launch_gossip_step(const GossipParams& p, int grid, cudaStream_t s) 
   // --local-steps: the fused dense step only (no split phases, no sparse records, no trigger, no drift copy)
   if (p.local_steps > 1 && (p.phase != 0 || p.sparse != nullptr || p.fsm.enabled || p.sent != nullptr))
     return cudaErrorInvalidValue;
+  // --global-avg-period: P >= 2 (P = 1 would average at every step), on the fused dense decent step with H = 1
+  if (p.global_avg_period < 0 || p.global_avg_period == 1) return cudaErrorInvalidValue;
+  if (p.global_avg_period > 1 && (p.phase != 0 || p.sparse != nullptr || p.fsm.enabled || p.sent != nullptr ||
+                                  p.local_steps > 1))
+    return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
     gossip_step_kernel<true><<<grid, EG_THREADS, 0, s>>>(p);
@@ -1022,6 +1045,11 @@ cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g,
                                       : (g.period >= 1 && g.period <= EG_MAX_SLOTS && g.n_slots == g.period);
   if (p.phase != 0 || p.sparse != nullptr || !p.do_push || !p.do_mix || !slots_ok) return cudaErrorInvalidValue;
   if (p.local_steps > 1 && (p.fsm.enabled || p.sent != nullptr)) return cudaErrorInvalidValue;   // decent only
+  // --global-avg-period: P >= 2, decent on a static graph with H = 1 (the one-peer graph's per-slot WAR bound k - tau
+  // has no rule for skipped steps)
+  if (p.global_avg_period < 0 || p.global_avg_period == 1) return cudaErrorInvalidValue;
+  if (p.global_avg_period > 1 && (p.fsm.enabled || p.sent != nullptr || p.local_steps > 1 || g.period > 0))
+    return cudaErrorInvalidValue;
   GraphStepParams q;
   static_cast<GossipParams&>(q) = p;
   q.g = g;
@@ -1049,10 +1077,11 @@ cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int g
   const bool ptrs = q.q_from_l && q.q_from_r && q.s_from_l && q.s_from_r && q.q_to_l && q.q_to_r && q.s_to_l &&
                     q.s_to_r && q.prev && q.rep_l && q.rep_r && p.flag_from_l && p.flag_from_r && p.flag_to_l &&
                     p.flag_to_r && p.ack_from_l && p.ack_from_r && p.ack_to_l && p.ack_to_r;
-  if (p.phase != 0 || !p.sync || p.sparse != nullptr || !p.do_push || !p.do_mix || !ptrs || p.local_steps > 1)
+  if (p.phase != 0 || !p.sync || p.sparse != nullptr || !p.do_push || !p.do_mix || !ptrs || p.local_steps > 1 ||
+      p.global_avg_period != 0)
     return cudaErrorInvalidValue;
   Q8StepParams k;
-  static_cast<GossipParams&>(k) = p;
+  static_cast<GossipCore&>(k) = p;   // no global_avg_period (refused above)
   k.q = q;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
@@ -1080,10 +1109,10 @@ cudaError_t launch_gossip_step_gt(const GossipParams& p, const TrackSlots& y, in
                     p.flag_from_l && p.flag_from_r && p.flag_to_l && p.flag_to_r && p.ack_from_l && p.ack_from_r &&
                     p.ack_to_l && p.ack_to_r;
   if (p.phase != 0 || !p.sync || p.sparse != nullptr || p.sent != nullptr || p.fsm.enabled || !p.do_push || !p.do_mix ||
-      !p.send_ack || !ptrs || p.local_steps > 1)
+      !p.send_ack || !ptrs || p.local_steps > 1 || p.global_avg_period != 0)
     return cudaErrorInvalidValue;
   GtStepParams k;
-  static_cast<GossipParams&>(k) = p;
+  static_cast<GossipCore&>(k) = p;   // no global_avg_period (refused above)
   k.gt = y;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
@@ -1109,10 +1138,10 @@ cudaError_t launch_gossip_step_ed(const GossipParams& p, const EdSlots& e, int g
   const bool ptrs = e.psi && p.inbox_l && p.inbox_r && p.push_l && p.flag_from_l && p.flag_from_r && p.flag_to_l &&
                     p.flag_to_r && p.ack_from_l && p.ack_from_r && p.ack_to_l && p.ack_to_r;
   if (p.phase != 0 || !p.sync || p.sparse != nullptr || p.sent != nullptr || p.fsm.enabled || !p.do_push || !p.do_mix ||
-      !p.send_ack || !ptrs || p.local_steps > 1)
+      !p.send_ack || !ptrs || p.local_steps > 1 || p.global_avg_period != 0)
     return cudaErrorInvalidValue;
   EdStepParams k;
-  static_cast<GossipParams&>(k) = p;
+  static_cast<GossipCore&>(k) = p;   // no global_avg_period (refused above)
   k.ed = e;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
@@ -1135,7 +1164,8 @@ int gossip_dbuf_max_grid(int device) {
 
 // Dense iter-sync exchange only (decent): every tensor fires every step, inboxes hold 2 slots.
 cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_t s) {
-  if (p.phase != 0 || !p.sync || !p.do_push || !p.do_mix || p.fsm.enabled || p.sent != nullptr || p.local_steps > 1)
+  if (p.phase != 0 || !p.sync || !p.do_push || !p.do_mix || p.fsm.enabled || p.sent != nullptr || p.local_steps > 1 ||
+      p.global_avg_period != 0)
     return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)

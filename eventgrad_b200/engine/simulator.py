@@ -14,7 +14,7 @@ import torch
 from ..parallel.arena import TensorTable
 from ..parallel.topology import Graph
 from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode,
-                                q8_encode, q8_msg_bytes, sgd_, topk_select, trigger_step)
+                                q8_encode, q8_msg_bytes, rank_mean, sgd_, topk_select, trigger_step)
 from .lr_schedule import lr_at
 
 
@@ -24,7 +24,7 @@ class RingSimulator:
                  topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
                  weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
                  offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1,
-                 exact_diffusion: bool = False):
+                 exact_diffusion: bool = False, global_avg_period: int = 0):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -45,7 +45,12 @@ class RingSimulator:
         psi, theta_0 at start.  Step k runs the unchanged optimizer on theta_k first, p = sgd(theta_k, g_k), then
         phi = p + (theta_k - psi), psi <- p, pushes phi (decent's bytes) and mixes
         theta_{k+1} = (phi + mix3_(phi, L, R)) / 2 on the received phi's.  sum_r theta_r = sum_r psi_r after every step.
-        At R = 1 the plain serial step runs.  Any dtype works (float64 for convergence studies)."""
+        At R = 1 the plain serial step runs.  Any dtype works (float64 for convergence studies).
+        `global_avg_period=P` (decent on the ring or a static circulant graph, P >= 2; Gossip-PGA): at step k with P
+        dividing k every rank takes theta' = ((theta_0 + theta_1) + ... + theta_{R-1}) / R (rank_mean) in place of the
+        mix and then its own SGD step with its own gradient and momentum; no push, the inboxes keep what the last gossip
+        step delivered.  Such a step counts n_elems * 4 bytes per rank (cent's convention for one all-reduce).  Every
+        other step is the decent step above.  0: off."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -72,6 +77,15 @@ class RingSimulator:
             raise ValueError("exact diffusion: decent on the ring, without compression, gradient tracking or local "
                              "steps, only")
         self.ed = bool(exact_diffusion) and world > 1
+        if isinstance(global_avg_period, bool) or int(global_avg_period) != global_avg_period or global_avg_period < 0:
+            raise ValueError(f"global_avg_period must be an integer >= 0, got {global_avg_period!r}")
+        if global_avg_period == 1:
+            raise ValueError("global_avg_period 1 averages at every step: that is algo cent")
+        if global_avg_period and (algo != "decent" or self.period or self.q8 or gradient_tracking or local_steps > 1
+                                  or exact_diffusion):
+            raise ValueError("global averaging: decent on the ring or a static graph, without compression, gradient "
+                             "tracking, local steps or exact diffusion, only")
+        self.global_avg_period = int(global_avg_period)
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -144,6 +158,10 @@ class RingSimulator:
         """Does 1-based step `step` gossip (local_steps H: iff H divides it)?"""
         return step % self.local_steps == 0
 
+    def global_avg_step(self, step: int) -> bool:
+        """Is 1-based step `step` a global-averaging step (global_avg_period P: iff P divides it)?"""
+        return self.global_avg_period > 0 and step % self.global_avg_period == 0
+
     def round_of(self, step: int) -> int:
         """Gossip round of a communicating step: the one-peer graph's active slot is indexed by it."""
         return step // self.local_steps
@@ -173,6 +191,8 @@ class RingSimulator:
             for r in range(R):                                 # serial step / local step of --local-steps
                 self._sgd(r, grads[r])
             return
+        if self.global_avg_step(self.pass_num):
+            return self._step_global_avg(grads)
         if self.ed:
             return self._step_ed(grads)
         rnd = self.round_of(self.pass_num)
@@ -263,6 +283,15 @@ class RingSimulator:
             tmix = mix3_(phis[r].clone(), self.inbox_l[r], self.inbox_r[r])
             self.theta[r].copy_(phis[r].add(tmix).div_(2))
 
+    def _step_global_avg(self, grads) -> None:
+        """Global-averaging step: theta_r <- sgd(rank_mean(theta), g_r) on every rank r."""
+        R, t = self.R, self.table
+        avg = rank_mean(self.theta)
+        for r in range(R):
+            self.theta[r].copy_(avg)
+            self._sgd(r, grads[r])
+            self.bytes[r] += t.n_elems * 4 if R > 1 else 0
+
     def final_average(self) -> torch.Tensor:
         return torch.stack(self.theta).sum(0) / self.R
 
@@ -277,8 +306,10 @@ class RingSimulator:
     def mixing_matrix(self, step: Optional[int] = None) -> torch.Tensor:
         """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD.  It depends on the 1-based step
         (default: the next one) on the one-peer graph, whose slot is that of the step's round, and under local_steps,
-        where a step that does not communicate has W = I."""
+        where a step that does not communicate has W = I.  A global-averaging step has W = 11^T / R."""
         k = self.pass_num + 1 if step is None else step
+        if self.global_avg_step(k):
+            return torch.full((self.R, self.R), 1.0 / self.R, dtype=torch.float64)
         if not self.communicates(k):
             return torch.eye(self.R, dtype=torch.float64)
         if self.period:

@@ -93,6 +93,19 @@ def check_local_steps_state(sd: Dict, local_steps: int, algo: str) -> None:
                          f"{int(local_steps)}; resume with the same --local-steps")
 
 
+def check_global_avg_state(sd: Dict, period: int, algo: str) -> None:
+    """Refuse to resume decent state saved under another --global-avg-period: the inboxes hold what the last gossip step
+    of that schedule delivered.  Checkpoints without a `global_avg_period` key never averaged (the key is written only
+    when P > 0, so checkpoints of runs without the feature keep their keys).  A resume at any step continues the cycle
+    by itself: which step averages is a function of the restored step counter."""
+    if algo != "decent":
+        return
+    saved = int(sd.get("global_avg_period", 0))
+    if saved != int(period):
+        raise ValueError(f"checkpoint was written with --global-avg-period {saved}, this run uses --global-avg-period "
+                         f"{int(period)}; resume with the same --global-avg-period")
+
+
 def check_exact_diffusion_state(sd: Dict, ed: bool, algo: str) -> None:
     """Refuse to resume decent state saved under the other --exact-diffusion setting: exact-diffusion state is psi, and
     its inboxes hold the neighbours' phi rather than their theta.  Checkpoints without an `exact_diffusion` key are plain

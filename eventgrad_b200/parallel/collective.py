@@ -15,6 +15,7 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
   --gradient-tracking (decent, ring): theta and y travel in one batched exchange; y_k = (y + yL + yR)/3 + g_k - g_prev,
           and SGD steps along y_k
   --local-steps H (decent): only every H-th step runs the exchange and mix; the others are the SGD update alone
+  --global-avg-period P (decent): every P-th step all_gathers theta, averages it in rank order and takes the SGD step
   --exact-diffusion (decent, ring): p = SGD(theta), phi = p + (theta - psi), psi <- p; phi travels in the ring exchange,
           and theta <- (phi + (phi + L + R)/3) / 2
 
@@ -31,10 +32,10 @@ from typing import List
 import torch
 import torch.distributed as dist
 
-from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_local_steps_state,
-                   check_topology_state, check_tracking_state, check_trigger_state)
+from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
+                   check_local_steps_state, check_topology_state, check_tracking_state, check_trigger_state)
 from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode, q8_encode,
-                      q8_msg_bytes, sgd_, topk_select, trigger_step)
+                      q8_msg_bytes, rank_mean, sgd_, topk_select, trigger_step)
 
 
 class CollectiveBackend(CommBackend):
@@ -92,6 +93,8 @@ class CollectiveBackend(CommBackend):
             self.psi = arena.theta.clone()
         # --local-steps H (decent): step k gossips iff H divides k, as round k / H; the other steps are _opt() alone
         self.local_steps = int(getattr(cfg, "local_steps", 1)) if cfg.algo == "decent" else 1
+        # --global-avg-period P (decent): step k with P dividing k averages theta over all ranks instead of gossiping
+        self.global_avg_period = int(getattr(cfg, "global_avg_period", 0)) if cfg.algo == "decent" else 0
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
             self.last_recv_norm_l, self.last_recv_norm_r = z(), z()
@@ -173,6 +176,8 @@ class CollectiveBackend(CommBackend):
             self._step_cent()
         elif not self.comm_enabled or self.pass_num % self.local_steps:
             self._opt()                                # serial step / local step of --local-steps
+        elif self.global_avg_period and self.pass_num % self.global_avg_period == 0:
+            self._step_global_avg()
         elif algo == "decent":
             self._step_decent()
         elif algo == "event":
@@ -205,6 +210,17 @@ class CollectiveBackend(CommBackend):
         self._exchange([a.theta], [a.theta], [self.inbox_l], [self.inbox_r])
         self.bytes += 2 * a.table.n_elems * 4
         mix3_(a.theta, self.inbox_l, self.inbox_r)
+        self._opt()
+
+    def _step_global_avg(self) -> None:
+        """Global-averaging step, the simulator's ops: theta <- rank_mean(every rank's theta), then SGD on the own
+        gradient and momentum.  all_gather gives every rank the same R tensors, so every rank forms the same mean."""
+        a = self.arena
+        if self.ring.world > 1:
+            parts = [torch.empty_like(a.theta) for _ in range(self.ring.world)]
+            dist.all_gather(parts, a.theta, group=self.group)
+            a.theta.copy_(rank_mean(parts))
+            self.bytes += a.table.n_elems * 4
         self._opt()
 
     def _step_tracking(self) -> None:
@@ -454,6 +470,8 @@ class CollectiveBackend(CommBackend):
         if self.cfg.algo == "decent":
             sd["gradient_tracking"] = self.gt
             sd["local_steps"] = self.local_steps
+            if self.global_avg_period:
+                sd["global_avg_period"] = self.global_avg_period
             sd["exact_diffusion"] = self.ed
             if self.gt:
                 for k in ("y", "g_prev", "y_in_l", "y_in_r"):
@@ -483,6 +501,7 @@ class CollectiveBackend(CommBackend):
         check_compress_state(sd, self.compress, self.cfg.algo)
         check_tracking_state(sd, self.gt, self.cfg.algo)
         check_local_steps_state(sd, self.local_steps, self.cfg.algo)
+        check_global_avg_state(sd, self.global_avg_period, self.cfg.algo)
         check_exact_diffusion_state(sd, self.ed, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
         if self.ed:

@@ -14,6 +14,9 @@ Per training step, after backward():
            y_k = (y + yL + yR)/3 + g_k - g_prev and steps along y_k)
            (--exact-diffusion, decent on the ring: csrc/gossip_ed.cu runs SGD in the push stage, pushes
            phi = p + theta_k - psi, psi <- p, and mixes theta = (phi + (phi + L + R)/3) / 2)
+           (--global-avg-period P, decent on the ring / a static graph: TWO launches per step, the two-shot all-reduce
+           of theta gated on "P divides the step" (a no-op launch otherwise), then the step kernel, which takes the plain
+           SGD step at an averaging step)
   spevent  batched segmented radix-select top-k + compaction straight into the neighbours'
            inboxes, scatter of arrived records into replicas, then the dense mix+SGD kernel
 No NCCL/MPI call, no separate elementwise kernel and no host synchronisation on that path
@@ -26,8 +29,8 @@ from typing import List
 import torch
 
 from .arena import TILE, ParamArena, TensorTable
-from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_local_steps_state,
-                   check_topology_state, check_tracking_state, check_trigger_state)
+from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
+                   check_local_steps_state, check_topology_state, check_tracking_state, check_trigger_state)
 from .topology import Graph
 from .trigger import q8_msg_bytes
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
@@ -54,7 +57,8 @@ def _wants_dbuf(cfg) -> bool:
     return ((db is None or bool(db)) and cfg.algo == "decent" and cfg.sync_mode == "iter"
             and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True)
             and not _wants_q8(cfg) and not getattr(cfg, "gradient_tracking", False)
-            and getattr(cfg, "local_steps", 1) == 1 and not getattr(cfg, "exact_diffusion", False))
+            and getattr(cfg, "local_steps", 1) == 1 and not getattr(cfg, "exact_diffusion", False)
+            and not getattr(cfg, "global_avg_period", 0))
 
 
 def _wants_q8(cfg) -> bool:
@@ -213,6 +217,14 @@ class P2PBackend(CommBackend):
         if getattr(cfg, "local_steps", 1) > 1 and (cfg.algo != "decent" or self.overlap or self.q8 or self.gt
                                                    or self.ed or getattr(cfg, "ce_push", False) or self.want_logs):
             raise ValueError("p2p backend: --local-steps runs decent on the fused single-kernel step only")
+        # --global-avg-period P (decent): the gated all-reduce of theta, then the fused single-slot ring / static-graph
+        # step; both take "does P divide this step" from the device pass counter, so one captured pair serves the cycle
+        self.global_avg_period = int(getattr(cfg, "global_avg_period", 0)) if cfg.algo == "decent" else 0
+        if getattr(cfg, "global_avg_period", 0) and (
+                cfg.algo != "decent" or self.overlap or self.q8 or self.gt or self.ed or self.local_steps > 1
+                or getattr(cfg, "ce_push", False) or self.want_logs or getattr(self.graph, "period", 0)):
+            raise ValueError("p2p backend: --global-avg-period runs decent on the fused single-kernel ring / static "
+                             "graph step only")
         self.dbuf = _wants_dbuf(cfg) and self.do_comm
         self.ce_push = bool(getattr(cfg, "ce_push", False)) and self.overlap and cfg.algo == "decent" and self.sync
         self.nvls = self.nvls_step = False      # set in connect() when the window has a multicast mapping
@@ -307,7 +319,7 @@ class P2PBackend(CommBackend):
         self._grads_alive = None
         self.host_bytes = 0
         self._connected = False
-        self.gp = self.ap = self.ap_avg = self.sp = self.gs = self.qs = self.ts = self.es = None
+        self.gp = self.ap = self.ap_avg = self.ap_pga = self.sp = self.gs = self.qs = self.ts = self.es = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
@@ -366,6 +378,7 @@ class P2PBackend(CommBackend):
                 "fsm.metric": 1 if self.drift else 0,
                 "sent": P(self.sent) if (self.drift and self.do_comm) else 0,
                 "local_steps": self.local_steps,
+                "global_avg_period": self.global_avg_period if self.do_comm else 0,
             })
             if self.graph is None:
                 gp.update({
@@ -487,6 +500,16 @@ class P2PBackend(CommBackend):
         av.update({"peer_bufs": P(self.d_peer_theta), "local": P(a.theta), "mode": 0, "zero_after": 0,
                    "two_shot": 1})
         self.ap_avg = av
+        # --global-avg-period: the same average, gated on the gossip pass counter (the step kernel that follows it in
+        # the stream advances that counter).  It shares the launch counter, the ticket and ar_flags with the final
+        # average: a gated-off launch leaves all three untouched, so they stay equal on every rank
+        self.ap_pga = None
+        if self.global_avg_period and self.do_comm and W > 1:
+            pga = C.AllReduceParams()
+            pga.update(common)
+            pga.update({"peer_bufs": P(self.d_peer_theta), "local": P(a.theta), "mode": 0, "zero_after": 0,
+                        "two_shot": 1, "gate_pass": P(self.d_pass), "gate_period": self.global_avg_period})
+            self.ap_pga = pga
         # EXPERIMENTAL NVLS: multicast mappings of the same buffers (0 unless the window is a SymmWindow on
         # a fabric with multicast support) -> csrc/allreduce_nvls.cu for the two-shot launches
         mc_grad = win.mc_addr("grad") if hasattr(win, "mc_addr") else 0
@@ -495,6 +518,8 @@ class P2PBackend(CommBackend):
         if self.nvls:
             ap.update({"mc_local": mc_grad})
             av.update({"mc_local": mc_theta})
+            if self.ap_pga is not None:
+                self.ap_pga.update({"mc_local": mc_theta})
         self.nvls_step = self.nvls and t.n_padded * 4 > ONE_SHOT_MAX_BYTES
         self._connected = True
         self._apply_lr_table()
@@ -603,6 +628,9 @@ class P2PBackend(CommBackend):
                 else:
                     C.gossip_step(self.gp, self.grid, s)       # plain fused SGD
                 return
+            if self.ap_pga is not None:
+                # the average comes first: the step kernel of an averaging step runs SGD on the averaged theta
+                (C.allreduce_nvls if self.nvls else C.allreduce)(self.ap_pga, self.grid, s)
             if self.sparse and self.do_comm:
                 if not self.overlap:
                     C.sparse_select_push(self.sp, self.grid, s)        # 3 launches: hist, candidates, compaction
@@ -631,6 +659,9 @@ class P2PBackend(CommBackend):
             self.host_bytes += 2 * sum(self.msg_bytes)
         elif self.gt:
             self.host_bytes += 2 * 2 * self.table.n_elems * 4      # theta and y, to both neighbours
+        elif self.global_avg_period and self.do_comm and self.pass_num % self.global_avg_period == 0:
+            # --global-avg-period P: an averaging step counts one all-reduce of theta (cent's convention)
+            self.host_bytes += self.table.n_elems * 4 if self.ring.world > 1 else 0
         elif self.cfg.algo == "decent" and self.do_comm and self.pass_num % self.local_steps == 0:
             # --local-steps H: only every H-th step sends
             self.host_bytes += getattr(self.ring, "fanout", 2) * self.table.n_elems * 4
@@ -719,6 +750,8 @@ class P2PBackend(CommBackend):
             sd["gradient_tracking"] = self.gt
             sd["local_steps"] = self.local_steps
             sd["exact_diffusion"] = self.ed
+            if self.global_avg_period:
+                sd["global_avg_period"] = self.global_avg_period
             if self.ed:
                 sd["psi"] = self.psi.cpu().clone()
             if self.gt:
@@ -741,6 +774,7 @@ class P2PBackend(CommBackend):
         check_tracking_state(sd, self.gt, self.cfg.algo)
         check_local_steps_state(sd, self.local_steps, self.cfg.algo)
         check_exact_diffusion_state(sd, self.ed, self.cfg.algo)
+        check_global_avg_state(sd, self.global_avg_period, self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
@@ -767,7 +801,10 @@ class P2PBackend(CommBackend):
             self._drained = self.pass_num          # log rows of the steps before the checkpoint are not replayed
         # NOTE: handshake counters (flags / acks) restart from pass_num on every rank.  Under --local-steps H the next
         # gossip step k is the first multiple of H above pass_num, so the WAR bound k - H (one-peer: k - tau * H) is at
-        # most pass_num, and only that round's pushes reach the flag value k
+        # most pass_num, and only that round's pushes reach the flag value k.  Under --global-avg-period P the next gossip
+        # step k waits for the ack of k - 1 or k - 2, both <= pass_num.  The all-reduce launch counter (ar_ctr) and the
+        # ar_flags block are not part of the checkpoint: a new process starts both at zero on every rank, and a backend
+        # that keeps running keeps them equal on every rank, since every rank ran the same averages
         if self.gossip:
             self._init_norms(run_fsm=False)
             self._reset_handshake(self.pass_num)

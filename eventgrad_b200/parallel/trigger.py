@@ -132,6 +132,17 @@ def mix2_(theta: torch.Tensor, slot: torch.Tensor) -> torch.Tensor:
 
 
 @torch.no_grad()
+def rank_mean(thetas) -> torch.Tensor:
+    """((theta_0 + theta_1) + ... + theta_{R-1}) / R as a new tensor: one rounded add per rank in rank order, then one
+    true division -- reduce_tile of csrc/allreduce.cu, the average of --global-avg-period.  The divisor is a 0-dim
+    tensor on the data's device, so CUDA divides instead of multiplying by a rounded 1/R."""
+    acc = thetas[0].clone()
+    for x in thetas[1:]:
+        acc.add_(x)
+    return acc.div_(torch.tensor(float(len(thetas)), dtype=acc.dtype, device=acc.device))
+
+
+@torch.no_grad()
 def sgd_(theta: torch.Tensor, grad: torch.Tensor, mom, lr: float, mu: float, wd: float = 0.0,
          nesterov: bool = False) -> None:
     """torch.optim.SGD step with dampening 0 (dcifar10/event/event.cpp:196-200; zero momentum buffer ==
