@@ -86,6 +86,8 @@ class TrainConfig:
                                      # gossip phi = p + theta - psi; no heterogeneity bias at decent's bytes
     global_avg_period: int = 0       # decent on the ring / a static graph: every P-th step (P >= 2) averages theta over
                                      # all ranks exactly in place of the gossip mix (Gossip-PGA); 0 = off
+    quasi_global_momentum: bool = False  # decent/event/spevent, momentum > 0: the momentum buffer follows each rank's
+                                     # parameter displacement (mix included) instead of its gradient (QG-DSGDm)
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -301,6 +303,30 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError(f"{h} does not support file_write: the reference's log format records a neighbour "
                                  "exchange at every step")
+        if self.quasi_global_momentum:
+            # quasi-global momentum exists in the ring, double-buffered and graph step kernels (csrc/gossip.cu), the
+            # torch.distributed backends and the simulator
+            h = "--quasi-global-momentum"
+            if self.algo == "cent":
+                raise ValueError(f"{h} needs a gossip algorithm (decent, event or spevent), got algo cent")
+            if self.momentum == 0.0:
+                raise ValueError(f"{h} needs --momentum > 0")
+            if self.sync_mode != "iter":
+                raise ValueError(f"{h} needs --sync-mode iter: an async mix of a torn or stale inbox would enter the "
+                                 "momentum buffer")
+            if self.compress != "none":
+                raise ValueError(f"{h} does not support --compress int8")
+            if self.gradient_tracking:
+                raise ValueError(f"{h} does not support --gradient-tracking")
+            if self.exact_diffusion:
+                raise ValueError(f"{h} does not support --exact-diffusion")
+            if self.global_avg_period:
+                raise ValueError(f"{h} does not support --global-avg-period: the gated all-reduce overwrites theta_k "
+                                 "before the step kernel reads it")
+            if self.backend == "refport":
+                raise ValueError(f"{h} is not supported by --backend refport")
+            if self.ce_push:
+                raise ValueError(f"{h} does not support ce_push")
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
@@ -440,6 +466,10 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--global-avg-period", type=int, default=None, metavar="P",
                    help="decent on the ring or a static graph: every P-th step (P >= 2) replaces the gossip mix with "
                         "an exact average of the parameters over all ranks (Gossip-PGA; default 0: off)")
+    p.add_argument("--quasi-global-momentum", action="store_true", default=None,
+                   help="decent/event/spevent with --momentum > 0: build each rank's momentum from its own parameter "
+                        "displacement (mix included) instead of its gradient (QG-DSGDm); removes momentum's "
+                        "1/(1 - mu) amplification of the heterogeneity bias at unchanged bytes")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

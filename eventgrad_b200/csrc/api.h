@@ -128,7 +128,14 @@ struct GossipParams : GossipCore {
   // and the step kernel takes the plain SGD step (no push, no flag, no ack, no mix).  0: off.  The WAR guard of the
   // next gossip step waits for the ack of k - 1 (PROTOCOL.md 1.11)
   int global_avg_period;
+  // quasi-global momentum (--quasi-global-momentum, decent/event/spevent on the ring, the double-buffered ring and
+  // circulant / one-peer graphs; needs mu > 0 and iter-sync): `mom` holds m_hat, built from the step's own parameter
+  // displacement theta_k - theta_{k+1} instead of the gradient (qg_sgd_elem in common.cuh).  0: the plain sgd_elem.
+  // It fills the tail padding after global_avg_period, so the size of this block is unchanged
+  int quasi_global;
 };
+static_assert(sizeof(GossipParams) == sizeof(GossipCore) + 8, "GossipParams: global_avg_period and quasi_global fill "
+                                                              "the 8 bytes after GossipCore");
 
 // Circulant gossip graph beyond the ring (csrc/gossip_graph.cu): the 2|O| inbox slots that replace the ring's
 // left/right pointers.  A separate block, passed to the graph kernel next to GossipParams, so the ring kernels'

@@ -66,6 +66,7 @@ static const std::unordered_map<std::string, Setter<GossipParams>> kGossip = {
     PTRF(GossipParams, sparse), NUMF(GossipParams, need_norm), NUMF(GossipParams, phase), TAB_FIELDS(GossipParams),
     NUMF(GossipParams, wd), NUMF(GossipParams, nesterov), PTRF(GossipParams, lr_table), NUMF(GossipParams, lr_len),
     NUMF(GossipParams, local_steps), PTRF(GossipParams, sent), NUMF(GossipParams, global_avg_period),
+    NUMF(GossipParams, quasi_global),
     PTRF2(GossipParams, fsm, thres), PTRF2(GossipParams, fsm, last_norm), PTRF2(GossipParams, fsm, last_iter),
     PTRF2(GossipParams, fsm, slopes), PTRF2(GossipParams, fsm, fire), PTRF2(GossipParams, fsm, cur_norm),
     PTRF2(GossipParams, fsm, counters), PTRF2(GossipParams, fsm, pass_num), PTRF2(GossipParams, fsm, log_ring),

@@ -141,4 +141,19 @@ __device__ __forceinline__ float sgd_elem(float th, float g, float& m, float lr,
   return __fmaf_rn(d, -lr, th);
 }
 
+// Quasi-global momentum (QG-DSGDm, Lin et al. 2021; parallel/trigger.py:qg_sgd_ is the oracle).  `th` is the step's
+// mix theta' of theta_k (theta_k when the step does not mix), `dk` = theta_k - theta' (rounded), `mh` the buffer m_hat,
+// c = 1 - mu in fp32:
+//   a = mu*m_hat;  d as sgd_elem;  m = a + d;  s = nesterov ? fma(m, mu, d) : m;  theta'' = fma(s, -lr, theta')
+//   lr != 0: m_hat = a + c*((theta_k - theta') / lr + s), the step's own displacement (theta_k - theta'') / lr written as
+//   mix displacement plus step direction, so lr*s is never subtracted back out of a rounded theta''
+__device__ __forceinline__ float qg_sgd_elem(float dk, float th, float g, float& mh, float lr, float mu, float c,
+                                             float wd, int nesterov) {
+  const float a = __fmul_rn(mh, mu);
+  const float d = (wd != 0.f) ? __fmaf_rn(th, wd, g) : g;
+  const float m = __fadd_rn(a, d);
+  const float s = nesterov ? __fmaf_rn(m, mu, d) : m;
+  if (lr != 0.f) mh = __fadd_rn(a, __fmul_rn(c, __fadd_rn(__fdiv_rn(dk, lr), s)));
+  return __fmaf_rn(s, -lr, th);
+}
 }  // namespace egb

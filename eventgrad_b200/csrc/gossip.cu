@@ -131,6 +131,17 @@ using StepParams = GossipParams;
 #else
 #define EG_LOCAL_STEPS 1
 #endif
+// Quasi-global momentum (GossipParams.quasi_global) exists in the ring, double-buffered and graph builds; the int8,
+// tracking and exact-diffusion builds take GossipCore, which has no such field, and their launchers reject it
+#if defined(EG_Q8) || defined(EG_GT) || defined(EG_ED)
+#define EG_QG 0
+#else
+#define EG_QG 1
+#endif
+#ifdef EG_GRAPH
+static_assert(offsetof(egb::GraphStepParams, g) == sizeof(egb::GossipCore) + 8,
+              "GraphSlots moved: quasi_global must stay in GossipParams' tail padding");
+#endif
 
 namespace egb {
 
@@ -512,7 +523,7 @@ __device__ __forceinline__ void ed_push_stage(const StepParams& p, const TileInf
 
 // mix + SGD + norm-on-write for one tile. `th` already holds theta_k for this thread's 8 floats.  `mix`: p.do_mix of
 // a gossip step, false on a local step of --local-steps (plain SGD); the q8 and tracking builds always mix
-template <bool kMom>
+template <bool kMom, bool kQG>
 __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileInfo& ti, size_t base, F8 th,
                                          int lane, int warp, int step, int slot, bool mix) {
 #ifdef EG_GRAPH
@@ -599,9 +610,12 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
 #else
   const bool logrecv = (p.tile_ss_l != nullptr);
   float ssl = 0.f, ssr = 0.f;
-  // issue every load of the tile before the first dependent FP op (5 x 32 B in flight per lane)
+  // issue every load of the tile before the first dependent FP op (5 x 32 B in flight per lane).  Quasi-global momentum
+  // loads the inboxes after the gradient and momentum instead, as the graph build stages its slots: it re-reads theta_k
+  // after the mix and would not fit in 64 registers otherwise
+  constexpr bool qg = kMom && kQG;
   F8 L, R, m;
-  if (mix) {
+  if (mix && !qg) {
 #ifdef EG_DBUF
     L = ld_f8_cg(p.inbox_l + EG_SLOT_OFF(p, step) + base);
     R = ld_f8_cg(p.inbox_r + EG_SLOT_OFF(p, step) + base);
@@ -613,6 +627,15 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
   const F8 g = load_grad(p, ti, base, threadIdx.x);
   if (kMom) m = ld_f8(p.mom + base);
   if (mix) {
+    if (qg) {
+#ifdef EG_DBUF
+      L = ld_f8_cg(p.inbox_l + EG_SLOT_OFF(p, step) + base);
+      R = ld_f8_cg(p.inbox_r + EG_SLOT_OFF(p, step) + base);
+#else
+      L = ld_f8_cg(p.inbox_l + base);
+      R = ld_f8_cg(p.inbox_r + base);
+#endif
+    }
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       th.v[e] = __fdiv_rn(__fadd_rn(__fadd_rn(th.v[e], L.v[e]), R.v[e]), 3.0f);
@@ -633,10 +656,26 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
   // learning rate of this step, looked up per tile (an L1 hit) rather than held in a register across the loop
   const float lr = sched_lr(p.lr_table, p.lr_len, p.lr, step);
   float ss = 0.f;
+#if EG_QG
+  if (kMom && kQG) {
+    // quasi-global momentum needs theta_k, which the mix has overwritten in `th` (the graph build accumulates the slots
+    // into it).  This thread has not stored this slice of theta yet, and nothing else stores theta during the step (the
+    // pipeline, the split step and the sparse prologue write only inboxes), so p.theta still holds theta_k
+    const F8 tk = ld_f8(p.theta + base);
+    const float c = __fsub_rn(1.f, p.mu);
 #pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    th.v[e] = sgd_elem<kMom>(th.v[e], g.v[e], m.v[e], lr, p.mu, p.wd, p.nesterov);
-    ss = __fmaf_rn(th.v[e], th.v[e], ss);
+    for (int e = 0; e < 8; ++e) {
+      th.v[e] = qg_sgd_elem(__fsub_rn(tk.v[e], th.v[e]), th.v[e], g.v[e], m.v[e], lr, p.mu, c, p.wd, p.nesterov);
+      ss = __fmaf_rn(th.v[e], th.v[e], ss);
+    }
+  } else
+#endif
+  {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      th.v[e] = sgd_elem<kMom>(th.v[e], g.v[e], m.v[e], lr, p.mu, p.wd, p.nesterov);
+      ss = __fmaf_rn(th.v[e], th.v[e], ss);
+    }
   }
   if (kMom) st_f8(p.mom + base, m);
   st_f8(p.theta + base, th);
@@ -751,8 +790,15 @@ __device__ __forceinline__ void push_phase(const StepParams& p, int step) {
   }
 }
 
+#if EG_QG
+template <bool kMom, bool kQG>   // kQG: quasi-global momentum, an instance of its own (see DESIGN §4)
+#else
 template <bool kMom>
+#endif
 __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(const StepParams p) {
+#if !EG_QG
+  constexpr bool kQG = false;
+#endif
   const int b = blockIdx.x, G = gridDim.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int step = *p.fsm.pass_num + 1;
@@ -810,7 +856,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
       const TileInfo ti = tile_info(p, s_ti, j, t);
       const F8 th = ld_f8(p.theta + base);
       if (push && (ti.flags & 1)) push_tile(p, base, th, slot);
-      mix_tile<kMom>(p, t, ti, base, th, lane, warp, step, slot, p.do_mix != 0 && comm);
+      mix_tile<kMom, kQG>(p, t, ti, base, th, lane, warp, step, slot, p.do_mix != 0 && comm);
     }
   } else {
     // ---------------- iter-sync: per-WARP software pipeline, no block barriers ------------------
@@ -906,8 +952,8 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         // the fired bits lane 0 observed, to the whole warp
         const int sides = __shfl_sync(0xffffffffu, (int)((fl & 1u) | ((fr & 1u) << 1)), 0);
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
-        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, sides,
-                       p.do_mix != 0);
+        mix_tile<kMom, kQG>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step,
+                            sides, p.do_mix != 0);
 #else
         if (lane == 0) {
 #ifdef EG_GRAPH
@@ -924,13 +970,13 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
 #ifdef EG_GT
         // the tracking mix loads theta itself, after the y stage: held from here it would spill
-        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot, p.do_mix != 0);
+        mix_tile<kMom, kQG>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot, p.do_mix != 0);
 #elif defined(EG_ED)
         // the exact-diffusion mix loads phi itself
-        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot, p.do_mix != 0);
+        mix_tile<kMom, kQG>(p, t2, tile_info(p, s_ti, j - D, t2), base, F8{}, lane, warp, step, slot, p.do_mix != 0);
 #else
-        mix_tile<kMom>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step, slot,
-                       p.do_mix != 0);
+        mix_tile<kMom, kQG>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step,
+                            slot, p.do_mix != 0);
 #endif
 #endif
       }
@@ -938,6 +984,12 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   }
   if (p.need_norm) cta_finish_tensors(p, s_ti, step + 1, p.do_mix != 0, true);
   grid_tail(p, step, slot);
+}
+
+// Quasi-global momentum needs a momentum buffer (mu > 0), iter-sync (an async mix of a stale inbox would enter m_hat),
+// and no global average (the gated all-reduce overwrites theta_k before the step kernel reads it back)
+static inline bool qg_rejected(const GossipParams& p) {
+  return p.quasi_global != 0 && (p.mu == 0.f || p.mom == nullptr || !p.sync || p.global_avg_period != 0);
 }
 
 #if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT) && !defined(EG_ED)
@@ -991,8 +1043,10 @@ int gossip_max_grid(int device) {
   int sms = 0, per_sm = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
   int per_sm2 = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gossip_step_kernel<true>, EG_THREADS, 0);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm2, gossip_step_kernel<false>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gossip_step_kernel<true, false>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm2, gossip_step_kernel<false, false>, EG_THREADS, 0);
+  if (per_sm2 < per_sm) per_sm = per_sm2;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm2, gossip_step_kernel<true, true>, EG_THREADS, 0);
   if (per_sm2 < per_sm) per_sm = per_sm2;
   if (per_sm < 1) per_sm = 1;
   return sms * per_sm;
@@ -1007,11 +1061,15 @@ cudaError_t launch_gossip_step(const GossipParams& p, int grid, cudaStream_t s) 
   if (p.global_avg_period > 1 && (p.phase != 0 || p.sparse != nullptr || p.fsm.enabled || p.sent != nullptr ||
                                   p.local_steps > 1))
     return cudaErrorInvalidValue;
+  if (qg_rejected(p)) return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
-    gossip_step_kernel<true><<<grid, EG_THREADS, 0, s>>>(p);
+    if (p.quasi_global)
+      gossip_step_kernel<true, true><<<grid, EG_THREADS, 0, s>>>(p);
+    else
+      gossip_step_kernel<true, false><<<grid, EG_THREADS, 0, s>>>(p);
   else
-    gossip_step_kernel<false><<<grid, EG_THREADS, 0, s>>>(p);
+    gossip_step_kernel<false, false><<<grid, EG_THREADS, 0, s>>>(p);
   return cudaGetLastError();
 }
 
@@ -1031,8 +1089,10 @@ cudaError_t launch_fsm_decide(const FsmDev& f, const TableDev& t, const float* e
 int gossip_graph_max_grid(int device) {
   int sms = 0, a = 0, b = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_graph<true>, EG_THREADS, 0);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_graph<false>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_graph<true, false>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_graph<false, false>, EG_THREADS, 0);
+  if (b < a) a = b;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_graph<true, true>, EG_THREADS, 0);
   if (b < a) a = b;
   if (a < 1) a = 1;
   return sms * a;
@@ -1050,14 +1110,18 @@ cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g,
   if (p.global_avg_period < 0 || p.global_avg_period == 1) return cudaErrorInvalidValue;
   if (p.global_avg_period > 1 && (p.fsm.enabled || p.sent != nullptr || p.local_steps > 1 || g.period > 0))
     return cudaErrorInvalidValue;
+  if (qg_rejected(p)) return cudaErrorInvalidValue;
   GraphStepParams q;
   static_cast<GossipParams&>(q) = p;
   q.g = g;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
-    gossip_step_kernel_graph<true><<<grid, EG_THREADS, 0, s>>>(q);
+    if (p.quasi_global)
+      gossip_step_kernel_graph<true, true><<<grid, EG_THREADS, 0, s>>>(q);
+    else
+      gossip_step_kernel_graph<true, false><<<grid, EG_THREADS, 0, s>>>(q);
   else
-    gossip_step_kernel_graph<false><<<grid, EG_THREADS, 0, s>>>(q);
+    gossip_step_kernel_graph<false, false><<<grid, EG_THREADS, 0, s>>>(q);
   return cudaGetLastError();
 }
 
@@ -1078,10 +1142,10 @@ cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int g
                     q.s_to_r && q.prev && q.rep_l && q.rep_r && p.flag_from_l && p.flag_from_r && p.flag_to_l &&
                     p.flag_to_r && p.ack_from_l && p.ack_from_r && p.ack_to_l && p.ack_to_r;
   if (p.phase != 0 || !p.sync || p.sparse != nullptr || !p.do_push || !p.do_mix || !ptrs || p.local_steps > 1 ||
-      p.global_avg_period != 0)
+      p.global_avg_period != 0 || p.quasi_global != 0)
     return cudaErrorInvalidValue;
   Q8StepParams k;
-  static_cast<GossipCore&>(k) = p;   // no global_avg_period (refused above)
+  static_cast<GossipCore&>(k) = p;   // no global_avg_period, no quasi_global (refused above)
   k.q = q;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
@@ -1109,10 +1173,10 @@ cudaError_t launch_gossip_step_gt(const GossipParams& p, const TrackSlots& y, in
                     p.flag_from_l && p.flag_from_r && p.flag_to_l && p.flag_to_r && p.ack_from_l && p.ack_from_r &&
                     p.ack_to_l && p.ack_to_r;
   if (p.phase != 0 || !p.sync || p.sparse != nullptr || p.sent != nullptr || p.fsm.enabled || !p.do_push || !p.do_mix ||
-      !p.send_ack || !ptrs || p.local_steps > 1 || p.global_avg_period != 0)
+      !p.send_ack || !ptrs || p.local_steps > 1 || p.global_avg_period != 0 || p.quasi_global != 0)
     return cudaErrorInvalidValue;
   GtStepParams k;
-  static_cast<GossipCore&>(k) = p;   // no global_avg_period (refused above)
+  static_cast<GossipCore&>(k) = p;   // no global_avg_period, no quasi_global (refused above)
   k.gt = y;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
@@ -1138,10 +1202,10 @@ cudaError_t launch_gossip_step_ed(const GossipParams& p, const EdSlots& e, int g
   const bool ptrs = e.psi && p.inbox_l && p.inbox_r && p.push_l && p.flag_from_l && p.flag_from_r && p.flag_to_l &&
                     p.flag_to_r && p.ack_from_l && p.ack_from_r && p.ack_to_l && p.ack_to_r;
   if (p.phase != 0 || !p.sync || p.sparse != nullptr || p.sent != nullptr || p.fsm.enabled || !p.do_push || !p.do_mix ||
-      !p.send_ack || !ptrs || p.local_steps > 1 || p.global_avg_period != 0)
+      !p.send_ack || !ptrs || p.local_steps > 1 || p.global_avg_period != 0 || p.quasi_global != 0)
     return cudaErrorInvalidValue;
   EdStepParams k;
-  static_cast<GossipCore&>(k) = p;   // no global_avg_period (refused above)
+  static_cast<GossipCore&>(k) = p;   // no global_avg_period, no quasi_global (refused above)
   k.ed = e;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
@@ -1155,8 +1219,10 @@ cudaError_t launch_gossip_step_ed(const GossipParams& p, const EdSlots& e, int g
 int gossip_dbuf_max_grid(int device) {
   int sms = 0, a = 0, b = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_dbuf<true>, EG_THREADS, 0);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_dbuf<false>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_dbuf<true, false>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_dbuf<false, false>, EG_THREADS, 0);
+  if (b < a) a = b;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_dbuf<true, true>, EG_THREADS, 0);
   if (b < a) a = b;
   if (a < 1) a = 1;
   return sms * a;
@@ -1165,13 +1231,16 @@ int gossip_dbuf_max_grid(int device) {
 // Dense iter-sync exchange only (decent): every tensor fires every step, inboxes hold 2 slots.
 cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_t s) {
   if (p.phase != 0 || !p.sync || !p.do_push || !p.do_mix || p.fsm.enabled || p.sent != nullptr || p.local_steps > 1 ||
-      p.global_avg_period != 0)
+      p.global_avg_period != 0 || qg_rejected(p))
     return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_GOSSIP, 1);
   if (p.mu != 0.f && p.mom != nullptr)
-    gossip_step_kernel_dbuf<true><<<grid, EG_THREADS, 0, s>>>(p);
+    if (p.quasi_global)
+      gossip_step_kernel_dbuf<true, true><<<grid, EG_THREADS, 0, s>>>(p);
+    else
+      gossip_step_kernel_dbuf<true, false><<<grid, EG_THREADS, 0, s>>>(p);
   else
-    gossip_step_kernel_dbuf<false><<<grid, EG_THREADS, 0, s>>>(p);
+    gossip_step_kernel_dbuf<false, false><<<grid, EG_THREADS, 0, s>>>(p);
   return cudaGetLastError();
 }
 #endif

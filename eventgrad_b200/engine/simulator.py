@@ -14,7 +14,7 @@ import torch
 from ..parallel.arena import TensorTable
 from ..parallel.topology import Graph
 from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode,
-                                q8_encode, q8_msg_bytes, rank_mean, sgd_, topk_select, trigger_step)
+                                q8_encode, q8_msg_bytes, qg_sgd_, rank_mean, sgd_, topk_select, trigger_step)
 from .lr_schedule import lr_at
 
 
@@ -24,7 +24,7 @@ class RingSimulator:
                  topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
                  weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
                  offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1,
-                 exact_diffusion: bool = False, global_avg_period: int = 0):
+                 exact_diffusion: bool = False, global_avg_period: int = 0, quasi_global: bool = False):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -50,7 +50,11 @@ class RingSimulator:
         dividing k every rank takes theta' = ((theta_0 + theta_1) + ... + theta_{R-1}) / R (rank_mean) in place of the
         mix and then its own SGD step with its own gradient and momentum; no push, the inboxes keep what the last gossip
         step delivered.  Such a step counts n_elems * 4 bytes per rank (cent's convention for one all-reduce).  Every
-        other step is the decent step above.  0: off."""
+        other step is the decent step above.  0: off.
+        `quasi_global=True` (decent, event, spevent; momentum > 0; QG-DSGDm): the momentum buffers hold m_hat.  Every
+        step of a rank -- gossip, local or serial -- snapshots theta_k first and runs qg_sgd_(theta', theta_k, ...) where
+        the other steps run sgd_, so m_hat follows the parameter displacement theta_k - theta_{k+1} instead of the
+        gradient.  Bytes and events are unchanged."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -86,6 +90,11 @@ class RingSimulator:
             raise ValueError("global averaging: decent on the ring or a static graph, without compression, gradient "
                              "tracking, local steps or exact diffusion, only")
         self.global_avg_period = int(global_avg_period)
+        if quasi_global and (algo == "cent" or momentum == 0.0 or self.q8 or gradient_tracking or exact_diffusion
+                             or global_avg_period):
+            raise ValueError("quasi-global momentum: decent, event or spevent with momentum > 0, without compression, "
+                             "gradient tracking, exact diffusion or global averaging, only")
+        self.qg = bool(quasi_global)
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -152,6 +161,9 @@ class RingSimulator:
 
     def _sgd(self, r, grad):
         lr = lr_at(self.lr_table, self.pass_num, self.lr)
+        if self.qg:
+            qg_sgd_(self.theta[r], self.theta_k[r], grad, self.mom[r], lr, self.mu, self.wd, self.nesterov)
+            return
         sgd_(self.theta[r], grad, self.mom[r], lr, self.mu, self.wd, self.nesterov)
 
     def communicates(self, step: int) -> bool:
@@ -181,6 +193,8 @@ class RingSimulator:
         under the drift metric) so the FSM logic can be compared exactly while norm accuracy is tested separately."""
         R, t = self.R, self.table
         self.pass_num += 1
+        if self.qg:
+            self.theta_k = [th.clone() for th in self.theta]      # before any mix of this step
         if self.algo == "cent":
             g = torch.stack(list(grads)).sum(0) / R if R > 1 else grads[0]
             for r in range(R):

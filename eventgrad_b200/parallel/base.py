@@ -106,6 +106,20 @@ def check_global_avg_state(sd: Dict, period: int, algo: str) -> None:
                          f"{int(period)}; resume with the same --global-avg-period")
 
 
+def check_qg_state(sd: Dict, qg: bool, algo: str) -> None:
+    """Refuse to resume gossip state saved under the other --quasi-global-momentum setting: the momentum buffer holds
+    m_hat with it and the heavy-ball m without it.  The key is written only when the feature is on, so checkpoints of
+    runs without it keep their keys."""
+    if algo not in ("decent", "event", "spevent"):
+        return
+    saved = bool(sd.get("quasi_global_momentum", False))
+    if saved != bool(qg):
+        have = "with" if saved else "without"
+        run = "with" if qg else "without"
+        raise ValueError(f"checkpoint was written {have} --quasi-global-momentum, this run is {run} it: its momentum "
+                         "buffer holds " + ("m_hat" if saved else "the heavy-ball momentum") +
+                         "; resume with the same --quasi-global-momentum setting")
+
 def check_exact_diffusion_state(sd: Dict, ed: bool, algo: str) -> None:
     """Refuse to resume decent state saved under the other --exact-diffusion setting: exact-diffusion state is psi, and
     its inboxes hold the neighbours' phi rather than their theta.  Checkpoints without an `exact_diffusion` key are plain

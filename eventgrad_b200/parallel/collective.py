@@ -18,6 +18,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
   --global-avg-period P (decent): every P-th step all_gathers theta, averages it in rank order and takes the SGD step
   --exact-diffusion (decent, ring): p = SGD(theta), phi = p + (theta - psi), psi <- p; phi travels in the ring exchange,
           and theta <- (phi + (phi + L + R)/3) / 2
+  --quasi-global-momentum (decent/event/spevent): theta_k is snapshotted before the exchange and every SGD update is
+          qg_sgd_, whose momentum follows theta_k - theta_{k+1}
 
 torch.distributed has no one-sided RMA, so the "window" is emulated with an iteration-
 synchronous exchange: first the fire masks, then a payload holding only the fired tensors.
@@ -33,9 +35,10 @@ import torch
 import torch.distributed as dist
 
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
-                   check_local_steps_state, check_topology_state, check_tracking_state, check_trigger_state)
+                   check_local_steps_state, check_qg_state, check_topology_state, check_tracking_state,
+                   check_trigger_state)
 from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode, q8_encode,
-                      q8_msg_bytes, rank_mean, sgd_, topk_select, trigger_step)
+                      q8_msg_bytes, qg_sgd_, rank_mean, sgd_, topk_select, trigger_step)
 
 
 class CollectiveBackend(CommBackend):
@@ -95,6 +98,10 @@ class CollectiveBackend(CommBackend):
         self.local_steps = int(getattr(cfg, "local_steps", 1)) if cfg.algo == "decent" else 1
         # --global-avg-period P (decent): step k with P dividing k averages theta over all ranks instead of gossiping
         self.global_avg_period = int(getattr(cfg, "global_avg_period", 0)) if cfg.algo == "decent" else 0
+        # --quasi-global-momentum: step() snapshots theta_k, and _opt() runs qg_sgd_ on it (every step, also local and
+        # serial ones)
+        self.qg = gossip and bool(getattr(cfg, "quasi_global_momentum", False))
+        self.theta_k = None
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
             self.last_recv_norm_l, self.last_recv_norm_r = z(), z()
@@ -165,6 +172,10 @@ class CollectiveBackend(CommBackend):
 
     def _opt(self) -> None:
         a, cfg = self.arena, self.cfg
+        if self.qg:
+            qg_sgd_(a.theta, self.theta_k, a.grad, a.mom, self.step_lr(self.pass_num), cfg.momentum, cfg.weight_decay,
+                    cfg.nesterov)
+            return
         sgd_(a.theta, a.grad, a.mom, self.step_lr(self.pass_num), cfg.momentum, cfg.weight_decay, cfg.nesterov)
 
     # ------------------------------------------------------------------ step
@@ -172,6 +183,8 @@ class CollectiveBackend(CommBackend):
     def step(self) -> None:
         self.pass_num += 1
         algo = self.cfg.algo
+        if self.qg:
+            self.theta_k = self.arena.theta.clone()    # before the exchange and the mix
         if algo == "cent":
             self._step_cent()
         elif not self.comm_enabled or self.pass_num % self.local_steps:
@@ -478,6 +491,8 @@ class CollectiveBackend(CommBackend):
                     sd[k] = getattr(self, k).cpu().clone()
             if self.ed:
                 sd["psi"] = self.psi.cpu().clone()
+        if self.qg:
+            sd["quasi_global_momentum"] = True      # the arena's momentum holds m_hat
         if self.cfg.algo in ("decent", "event"):
             sd["compress"] = self.compress          # int8: prev / rep_l / rep_r are saved above
         if self.cfg.algo in ("event", "spevent"):
@@ -503,6 +518,7 @@ class CollectiveBackend(CommBackend):
         check_local_steps_state(sd, self.local_steps, self.cfg.algo)
         check_global_avg_state(sd, self.global_avg_period, self.cfg.algo)
         check_exact_diffusion_state(sd, self.ed, self.cfg.algo)
+        check_qg_state(sd, self.qg, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
         if self.ed:
             self.psi.copy_(sd["psi"].to(self.psi.device))

@@ -30,7 +30,8 @@ import torch
 
 from .arena import TILE, ParamArena, TensorTable
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
-                   check_local_steps_state, check_topology_state, check_tracking_state, check_trigger_state)
+                   check_local_steps_state, check_qg_state, check_topology_state, check_tracking_state,
+                   check_trigger_state)
 from .topology import Graph
 from .trigger import q8_msg_bytes
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
@@ -225,6 +226,14 @@ class P2PBackend(CommBackend):
                 or getattr(cfg, "ce_push", False) or self.want_logs or getattr(self.graph, "period", 0)):
             raise ValueError("p2p backend: --global-avg-period runs decent on the fused single-kernel ring / static "
                              "graph step only")
+        # --quasi-global-momentum: the ring, double-buffered and graph step kernels update m_hat from theta_k (re-read
+        # after the mix) at every step, gossip, local or serial alike
+        self.qg = self.gossip and bool(getattr(cfg, "quasi_global_momentum", False))
+        if self.qg and (cfg.momentum == 0 or not self.sync or self.q8 or self.gt or self.ed or self.global_avg_period
+                        or getattr(cfg, "ce_push", False)):
+            raise ValueError("p2p backend: --quasi-global-momentum runs the ring, double-buffered and graph step "
+                             "kernels with momentum and iter-sync, without int8, tracking, exact diffusion, global "
+                             "averaging or ce_push")
         self.dbuf = _wants_dbuf(cfg) and self.do_comm
         self.ce_push = bool(getattr(cfg, "ce_push", False)) and self.overlap and cfg.algo == "decent" and self.sync
         self.nvls = self.nvls_step = False      # set in connect() when the window has a multicast mapping
@@ -379,6 +388,7 @@ class P2PBackend(CommBackend):
                 "sent": P(self.sent) if (self.drift and self.do_comm) else 0,
                 "local_steps": self.local_steps,
                 "global_avg_period": self.global_avg_period if self.do_comm else 0,
+                "quasi_global": 1 if self.qg else 0,
             })
             if self.graph is None:
                 gp.update({
@@ -733,6 +743,8 @@ class P2PBackend(CommBackend):
     def state_dict(self):
         torch.cuda.synchronize(self.dev)
         sd = {"pass_num": self.pass_num, "host_bytes": self.host_bytes}
+        if self.qg:
+            sd["quasi_global_momentum"] = True     # the arena's momentum holds m_hat
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
             sd[k] = getattr(self, k).cpu().clone()
         if self.cfg.algo in ("decent", "event") and self.graph is not None:
@@ -775,6 +787,7 @@ class P2PBackend(CommBackend):
         check_local_steps_state(sd, self.local_steps, self.cfg.algo)
         check_exact_diffusion_state(sd, self.ed, self.cfg.algo)
         check_global_avg_state(sd, self.global_avg_period, self.cfg.algo)
+        check_qg_state(sd, self.qg, self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):

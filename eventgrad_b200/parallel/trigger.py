@@ -156,6 +156,30 @@ def sgd_(theta: torch.Tensor, grad: torch.Tensor, mom, lr: float, mu: float, wd:
     theta.add_(d, alpha=-lr)
 
 
+
+@torch.no_grad()
+def qg_sgd_(theta: torch.Tensor, theta_k: torch.Tensor, grad: torch.Tensor, mom: torch.Tensor, lr: float, mu: float,
+            wd: float = 0.0, nesterov: bool = False) -> None:
+    """Quasi-global momentum step (QG-DSGDm, Lin, Kong, Stich and Jaggi 2021), op for op as qg_sgd_elem of
+    csrc/common.cuh.  `theta` holds the step's mix theta' of `theta_k` (theta_k itself when the step does not mix) and
+    receives theta''; `mom` holds m_hat, which is built from the step's own displacement instead of the gradient:
+        a = mu*m_hat ;  d = grad + wd*theta' (wd != 0) ;  m = a + d ;  s = d + mu*m (nesterov) or m ;
+        theta'' = theta' - lr*s ;  lr != 0: m_hat = a + (1 - mu)*((theta_k - theta') / lr + s), else m_hat is kept
+    (theta_k - theta'')/lr is written as mix displacement plus step direction, so lr*s is never subtracted back out of a
+    rounded theta''.  1 - mu is formed in the tensors' dtype and the division takes a 0-dim tensor divisor, so CUDA
+    divides instead of multiplying by a rounded 1/lr.  At a fixed point the displacement is zero and m_hat decays to 0:
+    no 1/(1 - mu) amplification of the heterogeneity bias."""
+    d = grad.add(theta, alpha=wd) if wd != 0.0 else grad
+    a = mom.mul(mu)
+    m = a.add(d)
+    s = d.add(m, alpha=mu) if nesterov else m
+    q = theta_k.sub(theta)
+    theta.add_(s, alpha=-lr)
+    if float(torch.tensor(lr, dtype=theta.dtype)) != 0.0:
+        q.div_(torch.tensor(lr, dtype=q.dtype, device=q.device)).add_(s)
+        c = float(torch.tensor(1.0, dtype=theta.dtype).sub_(mu))
+        mom.copy_(a.add_(q.mul_(c)))
+
 Q8_BLOCK = 256          # elements per int8 scale: one warp's slice of a 2048-float tile (never straddles tensors)
 COMPRESS = ("none", "int8")
 
