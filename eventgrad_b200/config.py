@@ -88,6 +88,11 @@ class TrainConfig:
                                      # all ranks exactly in place of the gossip mix (Gossip-PGA); 0 = off
     quasi_global_momentum: bool = False  # decent/event/spevent, momentum > 0: the momentum buffer follows each rank's
                                      # parameter displacement (mix included) instead of its gradient (QG-DSGDm)
+    slowmo_period: int = 0           # decent on the ring / a static graph: every tau-th step (tau >= 2) averages theta
+                                     # exactly and takes a slow heavy-ball step on the average from where the cycle
+                                     # started (SlowMo); base: gossip (local_steps 1) or local SGD (local_steps tau); 0 = off
+    slowmo_beta: float = 0.5         # SlowMo slow momentum, 0 <= beta < 1
+    slowmo_lr: float = 1.0           # SlowMo slow learning rate, alpha > 0
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -327,6 +332,52 @@ class TrainConfig:
                 raise ValueError(f"{h} is not supported by --backend refport")
             if self.ce_push:
                 raise ValueError(f"{h} does not support ce_push")
+        tau = self.slowmo_period
+        if isinstance(tau, bool) or not isinstance(tau, int) or tau < 0:
+            raise ValueError(f"--slowmo-period must be an integer >= 0, got {tau!r}")
+        if tau == 1:
+            raise ValueError("--slowmo-period 1 averages at every step and leaves no base step: use algo cent")
+        if tau:
+            # SlowMo exists for decent in the fused single-kernel ring / static-graph step (the gated sync kernel of
+            # csrc/allreduce.cu before csrc/gossip.cu, csrc/gossip_graph.cu), the torch.distributed backends and the
+            # simulator
+            h = f"--slowmo-period {tau}"
+            if not (isinstance(self.slowmo_beta, (int, float)) and 0.0 <= self.slowmo_beta < 1.0):
+                raise ValueError(f"--slowmo-beta must be in [0, 1), got {self.slowmo_beta!r}")
+            if not (isinstance(self.slowmo_lr, (int, float)) and self.slowmo_lr > 0.0):
+                raise ValueError(f"--slowmo-lr must be > 0, got {self.slowmo_lr!r}")
+            if not self.lr > 0.0:
+                raise ValueError(f"{h} needs --lr > 0: the slow momentum is (x - theta_bar) / lr")
+            if self.algo == "cent":
+                raise ValueError(f"{h} needs algo decent: cent has its own all-reduce step")
+            if self.algo in ("event", "spevent"):
+                raise ValueError(f"{h} needs algo decent, got {self.algo!r}: the trigger's last_norm / sent state has no "
+                                 "defined meaning across the jump of theta at a sync")
+            if str(self.topology).strip().lower() == "onepeer-exp":
+                raise ValueError(f"{h} does not support topology onepeer-exp: its per-slot WAR bound has no rule for "
+                                 "skipped steps")
+            if self.local_steps not in (1, tau):
+                raise ValueError(f"{h} needs --local-steps 1 (gossip base) or {tau} (local SGD base), got "
+                                 f"--local-steps {self.local_steps}")
+            if self.global_avg_period:
+                raise ValueError(f"{h} does not support --global-avg-period: both replace the mix at the same steps")
+            if self.gradient_tracking:
+                raise ValueError(f"{h} does not support --gradient-tracking")
+            if self.exact_diffusion:
+                raise ValueError(f"{h} does not support --exact-diffusion")
+            if self.compress != "none":
+                raise ValueError(f"{h} does not support --compress int8")
+            if self.quasi_global_momentum:
+                raise ValueError(f"{h} does not support --quasi-global-momentum: the sync overwrites theta_k before the "
+                                 "step kernel reads it back")
+            if self.backend == "refport":
+                raise ValueError(f"{h} is not supported by --backend refport")
+            for name in ("overlap_push", "double_buffer", "ce_push"):
+                if getattr(self, name):
+                    raise ValueError(f"{h} does not support {name} (fused single-kernel step only)")
+            if self.file_write:
+                raise ValueError(f"{h} does not support file_write: the reference's log format records a neighbour "
+                                 "exchange at every step")
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
@@ -377,7 +428,8 @@ class TrainConfig:
             kw["overlap_push"] = bool(cuda and p2p and world >= 2 and c.algo in ("decent", "event")
                                       and not bool(c.double_buffer) and c.ring_topology and c.compress == "none"
                                       and not c.gradient_tracking and c.local_steps == 1
-                                      and not c.exact_diffusion and not c.global_avg_period)
+                                      and not c.exact_diffusion and not c.global_avg_period
+                                      and not c.slowmo_period)
         return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
@@ -470,6 +522,15 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
                    help="decent/event/spevent with --momentum > 0: build each rank's momentum from its own parameter "
                         "displacement (mix included) instead of its gradient (QG-DSGDm); removes momentum's "
                         "1/(1 - mu) amplification of the heterogeneity bias at unchanged bytes")
+    p.add_argument("--slowmo-period", type=int, default=None, metavar="TAU",
+                   help="decent on the ring or a static graph: every TAU-th step (TAU >= 2) averages the parameters "
+                        "exactly and takes a slow heavy-ball step on the average from where the cycle started (SlowMo); "
+                        "the base steps gossip (--local-steps 1) or are local SGD (--local-steps TAU) (default 0: off)")
+    p.add_argument("--slowmo-beta", type=float, default=None, metavar="BETA",
+                   help="SlowMo slow momentum, 0 <= BETA < 1 (default 0.5; 0 with --slowmo-lr 1 is plain periodic "
+                        "averaging)")
+    p.add_argument("--slowmo-lr", type=float, default=None, metavar="ALPHA",
+                   help="SlowMo slow learning rate, ALPHA > 0 (default 1.0)")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

@@ -161,6 +161,67 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_AR_SYM(allreduce_kernel)(con
 }
 
 #ifndef EG_NVLS
+// SlowMo sync (--slowmo-period tau): the gated two-shot average of theta, then the outer heavy-ball update of the
+// identical x and u on every rank, one persistent launch.  Every op is an fp32 round-to-nearest intrinsic, so nothing
+// is contracted and parallel/trigger.py:slowmo_sync_ reproduces it bit for bit.
+__global__ void __launch_bounds__(EG_THREADS, 4) slowmo_sync_kernel(const SlowMoParams p) {
+  const int b = blockIdx.x, G = gridDim.x, tid = threadIdx.x;
+  // step gate: not a sync step -> no barrier, no load, no store, no counter (PROTOCOL.md 1.11, 1.13)
+  const int step = *p.gate_pass + 1;
+  if (step % p.gate_period != 0) return;
+  const uint32_t seq = (uint32_t)(*p.step_ctr) + 1u;
+  const float lr = sched_lr(p.lr_table, p.lr_len, p.lr, step);
+  const float c = __fmul_rn(p.alpha, lr);
+
+  cta_barrier_all_ranks(p, 0, b, G, seq);                 // every rank's theta is final
+  int j = 0;
+  for (int t = b; t < p.n_tiles; t += G, ++j) {
+    if ((b + j) % p.world != p.rank) continue;            // tile owner
+    const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
+    const F8 avg = reduce_tile(p, base);
+    for (int r = 0; r < p.world; ++r) st_f8(p.peer_bufs[r] + base, avg);
+  }
+  // every owner has stored theta_bar into my theta, and has finished reading my theta (its reads precede its arrival)
+  cta_barrier_all_ranks(p, 1, b, G, seq);
+  for (int t = b; t < p.n_tiles; t += G) {
+    const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
+    F8 x = ld_f8_cg(p.local + base);                      // theta_bar, stored by its owner
+    if (lr != 0.f) {
+      const F8 xo = ld_f8(p.x + base);
+      F8 u = ld_f8(p.u + base);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float q = __fdiv_rn(__fsub_rn(xo.v[e], x.v[e]), lr);
+        u.v[e] = __fadd_rn(__fmul_rn(p.beta, u.v[e]), q);
+        x.v[e] = __fmaf_rn(u.v[e], -c, xo.v[e]);
+      }
+      st_f8(p.u + base, u);
+    }
+    st_f8(p.x + base, x);
+    st_f8(p.local + base, x);
+    if (p.shadow != nullptr) st_bf16x8(p.shadow + base, x);
+  }
+  __syncthreads();
+  if (tid == 0) {
+    __threadfence();
+    const unsigned prev = atomicAdd(p.ticket, 1u);
+    if (prev == gridDim.x - 1) {
+      *p.ticket = 0u;
+      *p.step_ctr = (int)seq;
+    }
+  }
+}
+
+cudaError_t launch_slowmo_sync(const SlowMoParams& p, int grid, cudaStream_t s) {
+  // the peer-load two-shot average only; tau >= 2 on a pass counter; beta in [0, 1), alpha > 0
+  if (p.gate_period < 2 || p.gate_pass == nullptr || !p.two_shot || p.mode != 0 || p.x == nullptr ||
+      p.u == nullptr || !(p.beta >= 0.f && p.beta < 1.f) || !(p.alpha > 0.f))
+    return cudaErrorInvalidValue;
+  eg_count_launch(EG_FAM_ALLREDUCE, 1);
+  slowmo_sync_kernel<<<grid, EG_THREADS, 0, s>>>(p);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_allreduce(const AllReduceParams& p, int grid, cudaStream_t s) {
   if (p.gate_period < 0 || (p.gate_period > 0 && p.gate_pass == nullptr)) return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_ALLREDUCE, 1);

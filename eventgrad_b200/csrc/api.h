@@ -271,6 +271,20 @@ struct AllReduceParams {
   int gate_period;
 };
 cudaError_t launch_allreduce(const AllReduceParams& p, int grid, cudaStream_t s);
+// SlowMo (--slowmo-period tau, decent; csrc/allreduce.cu): the all-reduce block followed by the outer iterate x and
+// the slow momentum u (arena-sized, local device memory, identical on every rank) and the slow momentum / learning rate.
+// The sync kernel is gated like the --global-avg-period all-reduce (gate_pass, gate_period = tau): at step k with tau
+// dividing k it averages theta two-shot into every rank's theta window, then every rank applies, tile by tile,
+//   lr != 0:  u <- beta*u + (x - theta_bar) / lr ;  x <- fma(u, -alpha*lr, x)        lr == 0:  x <- theta_bar
+// and stores theta <- x (and the bf16 shadow when set).  A separate struct, so AllReduceParams and the all-reduce
+// instances keep their layout and code
+struct SlowMoParams : AllReduceParams {
+  float* x;
+  float* u;
+  float beta;
+  float alpha;
+};
+cudaError_t launch_slowmo_sync(const SlowMoParams& p, int grid, cudaStream_t s);
 // experimental NVLink-SHARP variant (csrc/allreduce_nvls.cu): multimem.ld_reduce + multimem.st, two-shot only
 cudaError_t launch_allreduce_nvls(const AllReduceParams& p, int grid, cudaStream_t s);
 

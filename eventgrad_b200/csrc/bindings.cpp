@@ -109,6 +109,17 @@ static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce
     PTRF(AllReduceParams, gate_pass), NUMF(AllReduceParams, gate_period),
 };
 
+// SlowMoParams: every AllReduceParams field plus the SlowMo block
+static const std::unordered_map<std::string, Setter<SlowMoParams>> kSlowMo = [] {
+  std::unordered_map<std::string, Setter<SlowMoParams>> m;
+  for (const auto& kv : kAllReduce) {
+    const Setter<AllReduceParams> f = kv.second;
+    m.emplace(kv.first, [f](SlowMoParams& p, py::object v) { f(p, v); });
+  }
+  m.insert({PTRF(SlowMoParams, x), PTRF(SlowMoParams, u), NUMF(SlowMoParams, beta), NUMF(SlowMoParams, alpha)});
+  return m;
+}();
+
 static const std::unordered_map<std::string, Setter<SparseParams>> kSparse = {
     PTRF(SparseParams, theta), PTRF(SparseParams, prev), PTRF(SparseParams, rep_l), PTRF(SparseParams, rep_r),
     PTRF(SparseParams, rec_from_l), PTRF(SparseParams, rec_from_r), PTRF(SparseParams, rec_to_l),
@@ -186,6 +197,7 @@ PYBIND11_MODULE(_C, m) {
   bind_params<TrackSlots>(m, "TrackSlots", kTrack);
   bind_params<EdSlots>(m, "EdSlots", kEd);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
+  bind_params<SlowMoParams>(m, "SlowMoParams", kSlowMo);
   bind_params<SparseParams>(m, "SparseParams", kSparse);
   bind_params<BnParams>(m, "BnParams", kBn);
 
@@ -227,6 +239,9 @@ PYBIND11_MODULE(_C, m) {
   });
   m.def("allreduce", [](const AllReduceParams& p, int grid, uintptr_t s) {
     check(launch_allreduce(p, grid, S(s)), "allreduce");
+  });
+  m.def("slowmo_sync", [](const SlowMoParams& p, int grid, uintptr_t s) {
+    check(launch_slowmo_sync(p, grid, S(s)), "slowmo_sync");
   });
   m.def("allreduce_nvls", [](const AllReduceParams& p, int grid, uintptr_t s) {
     check(launch_allreduce_nvls(p, grid, S(s)), "allreduce_nvls");

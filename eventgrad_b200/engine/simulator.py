@@ -14,7 +14,8 @@ import torch
 from ..parallel.arena import TensorTable
 from ..parallel.topology import Graph
 from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode,
-                                q8_encode, q8_msg_bytes, qg_sgd_, rank_mean, sgd_, topk_select, trigger_step)
+                                q8_encode, q8_msg_bytes, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
+                                trigger_step)
 from .lr_schedule import lr_at
 
 
@@ -24,7 +25,8 @@ class RingSimulator:
                  topk_percent: float = 10.0, serial_skip: bool = True, sparse_init=None,
                  weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
                  offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1,
-                 exact_diffusion: bool = False, global_avg_period: int = 0, quasi_global: bool = False):
+                 exact_diffusion: bool = False, global_avg_period: int = 0, quasi_global: bool = False,
+                 slowmo_period: int = 0, slowmo_beta: float = 0.5, slowmo_lr: float = 1.0):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -54,7 +56,13 @@ class RingSimulator:
         `quasi_global=True` (decent, event, spevent; momentum > 0; QG-DSGDm): the momentum buffers hold m_hat.  Every
         step of a rank -- gossip, local or serial -- snapshots theta_k first and runs qg_sgd_(theta', theta_k, ...) where
         the other steps run sgd_, so m_hat follows the parameter displacement theta_k - theta_{k+1} instead of the
-        gradient.  Bytes and events are unchanged."""
+        gradient.  Bytes and events are unchanged.
+        `slowmo_period=tau` (decent on the ring or a static circulant graph, tau >= 2; SlowMo, Wang et al. 2020): every
+        rank also keeps the outer iterate x (theta_0 at start) and the slow momentum u (zero at start), identical on every
+        rank.  At step k with tau dividing k every rank forms avg = rank_mean(theta), runs slowmo_sync_(x, u, avg, lr_k,
+        `slowmo_beta`, `slowmo_lr`), sets theta <- x and takes its own SGD step; such a step counts n_elems * 4 bytes per
+        rank (0 at R = 1, where the outer update still runs on the rank's own theta).  The other steps are the base:
+        decent's gossip step with local_steps = 1, the serial SGD step with local_steps = tau (local SGD).  0: off."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -95,6 +103,21 @@ class RingSimulator:
             raise ValueError("quasi-global momentum: decent, event or spevent with momentum > 0, without compression, "
                              "gradient tracking, exact diffusion or global averaging, only")
         self.qg = bool(quasi_global)
+        tau = slowmo_period
+        if isinstance(tau, bool) or int(tau) != tau or tau < 0 or tau == 1:
+            raise ValueError(f"slowmo_period must be 0 or an integer >= 2, got {tau!r}")
+        if tau:
+            if not (0.0 <= slowmo_beta < 1.0) or not slowmo_lr > 0.0 or not lr > 0.0:
+                raise ValueError("slowmo: slowmo_beta in [0, 1), slowmo_lr > 0 and lr > 0 only")
+            if (algo != "decent" or self.period or self.q8 or gradient_tracking or exact_diffusion or global_avg_period
+                    or quasi_global or local_steps not in (1, tau)):
+                raise ValueError("slowmo: decent on the ring or a static graph with local_steps 1 or slowmo_period, "
+                                 "without compression, gradient tracking, exact diffusion, global averaging or "
+                                 "quasi-global momentum, only")
+        self.slowmo_period, self.slowmo_beta, self.slowmo_lr = int(tau), float(slowmo_beta), float(slowmo_lr)
+        if self.slowmo_period:
+            self.slowmo_x = [theta0.clone() for _ in range(world)]
+            self.slowmo_u = [torch.zeros_like(theta0) for _ in range(world)]
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -174,6 +197,10 @@ class RingSimulator:
         """Is 1-based step `step` a global-averaging step (global_avg_period P: iff P divides it)?"""
         return self.global_avg_period > 0 and step % self.global_avg_period == 0
 
+    def slowmo_step(self, step: int) -> bool:
+        """Is 1-based step `step` a SlowMo sync step (slowmo_period tau: iff tau divides it)?"""
+        return self.slowmo_period > 0 and step % self.slowmo_period == 0
+
     def round_of(self, step: int) -> int:
         """Gossip round of a communicating step: the one-peer graph's active slot is indexed by it."""
         return step // self.local_steps
@@ -201,6 +228,8 @@ class RingSimulator:
                 self._sgd(r, g)
                 self.bytes[r] += t.n_elems * 4 if R > 1 else 0
             return
+        if self.slowmo_step(self.pass_num):
+            return self._step_slowmo(grads)
         if (R == 1 and self.serial_skip) or not self.communicates(self.pass_num):
             for r in range(R):                                 # serial step / local step of --local-steps
                 self._sgd(r, grads[r])
@@ -306,6 +335,18 @@ class RingSimulator:
             self._sgd(r, grads[r])
             self.bytes[r] += t.n_elems * 4 if R > 1 else 0
 
+    def _step_slowmo(self, grads) -> None:
+        """SlowMo sync step: avg = rank_mean(theta); on every rank r the outer update of x_r, u_r, theta_r <- x_r, then
+        sgd(theta_r, g_r).  Every rank runs the update on the same inputs, so x and u stay identical across ranks."""
+        R, t = self.R, self.table
+        avg = rank_mean(self.theta)
+        lr = lr_at(self.lr_table, self.pass_num, self.lr)
+        for r in range(R):
+            slowmo_sync_(self.slowmo_x[r], self.slowmo_u[r], avg, lr, self.slowmo_beta, self.slowmo_lr)
+            self.theta[r].copy_(self.slowmo_x[r])
+            self._sgd(r, grads[r])
+            self.bytes[r] += t.n_elems * 4 if R > 1 else 0
+
     def final_average(self) -> torch.Tensor:
         return torch.stack(self.theta).sum(0) / self.R
 
@@ -320,9 +361,10 @@ class RingSimulator:
     def mixing_matrix(self, step: Optional[int] = None) -> torch.Tensor:
         """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD.  It depends on the 1-based step
         (default: the next one) on the one-peer graph, whose slot is that of the step's round, and under local_steps,
-        where a step that does not communicate has W = I.  A global-averaging step has W = 11^T / R."""
+        where a step that does not communicate has W = I.  A global-averaging step has W = 11^T / R, and so does the
+        average of a SlowMo sync step (before its outer update)."""
         k = self.pass_num + 1 if step is None else step
-        if self.global_avg_step(k):
+        if self.global_avg_step(k) or self.slowmo_step(k):
             return torch.full((self.R, self.R), 1.0 / self.R, dtype=torch.float64)
         if not self.communicates(k):
             return torch.eye(self.R, dtype=torch.float64)

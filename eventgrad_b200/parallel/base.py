@@ -106,6 +106,29 @@ def check_global_avg_state(sd: Dict, period: int, algo: str) -> None:
                          f"{int(period)}; resume with the same --global-avg-period")
 
 
+def slowmo_state(be) -> Dict:
+    """Checkpoint entries of a decent backend under --slowmo-period (none when the feature is off, so other checkpoints
+    keep their keys): the settings and the outer iterate x and slow momentum u, on the CPU."""
+    if not be.slowmo_period:
+        return {}
+    return {"slowmo_period": be.slowmo_period, "slowmo_beta": be.slowmo_beta, "slowmo_lr": be.slowmo_lr,
+            "slowmo_x": be.slowmo_x.cpu().clone(), "slowmo_u": be.slowmo_u.cpu().clone()}
+
+
+def check_slowmo_state(sd: Dict, period: int, beta: float, alpha: float, algo: str) -> None:
+    """Refuse to resume decent state saved under other --slowmo-period / --slowmo-beta / --slowmo-lr settings, in either
+    direction: x and u belong to that schedule.  Checkpoints without a `slowmo_period` key never ran SlowMo.  A resume at
+    any step continues the cycle by itself: which step syncs is a function of the restored step counter."""
+    if algo != "decent":
+        return
+    saved = (int(sd.get("slowmo_period", 0)), float(sd.get("slowmo_beta", beta)), float(sd.get("slowmo_lr", alpha)))
+    run = (int(period), float(beta), float(alpha))
+    if saved[0] != run[0] or (run[0] and saved != run):
+        fmt = lambda s: f"--slowmo-period {s[0]}" + (f" --slowmo-beta {s[1]} --slowmo-lr {s[2]}" if s[0] else "")
+        raise ValueError(f"checkpoint was written with {fmt(saved)}, this run uses {fmt(run)}; resume with the same "
+                         "--slowmo-period, --slowmo-beta and --slowmo-lr")
+
+
 def check_qg_state(sd: Dict, qg: bool, algo: str) -> None:
     """Refuse to resume gossip state saved under the other --quasi-global-momentum setting: the momentum buffer holds
     m_hat with it and the heavy-ball m without it.  The key is written only when the feature is on, so checkpoints of

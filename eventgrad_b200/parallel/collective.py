@@ -16,6 +16,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
           and SGD steps along y_k
   --local-steps H (decent): only every H-th step runs the exchange and mix; the others are the SGD update alone
   --global-avg-period P (decent): every P-th step all_gathers theta, averages it in rank order and takes the SGD step
+  --slowmo-period tau (decent): every tau-th step all_gathers theta, averages it in rank order, applies slowmo_sync_ to
+          the outer iterate x and slow momentum u, sets theta <- x and takes the SGD step
   --exact-diffusion (decent, ring): p = SGD(theta), phi = p + (theta - psi), psi <- p; phi travels in the ring exchange,
           and theta <- (phi + (phi + L + R)/3) / 2
   --quasi-global-momentum (decent/event/spevent): theta_k is snapshotted before the exchange and every SGD update is
@@ -35,10 +37,10 @@ import torch
 import torch.distributed as dist
 
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
-                   check_local_steps_state, check_qg_state, check_topology_state, check_tracking_state,
-                   check_trigger_state)
+                   check_local_steps_state, check_qg_state, check_slowmo_state, check_topology_state,
+                   check_tracking_state, check_trigger_state, slowmo_state)
 from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode, q8_encode,
-                      q8_msg_bytes, qg_sgd_, rank_mean, sgd_, topk_select, trigger_step)
+                      q8_msg_bytes, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select, trigger_step)
 
 
 class CollectiveBackend(CommBackend):
@@ -101,6 +103,13 @@ class CollectiveBackend(CommBackend):
         # --quasi-global-momentum: step() snapshots theta_k, and _opt() runs qg_sgd_ on it (every step, also local and
         # serial ones)
         self.qg = gossip and bool(getattr(cfg, "quasi_global_momentum", False))
+        # --slowmo-period tau (decent): step k with tau dividing k averages theta over all ranks, then the outer update of
+        # x (theta_0 at start) and u (zero at start), identical on every rank; the other steps are the base steps
+        self.slowmo_period = int(getattr(cfg, "slowmo_period", 0)) if cfg.algo == "decent" else 0
+        self.slowmo_beta = float(getattr(cfg, "slowmo_beta", 0.5))
+        self.slowmo_lr = float(getattr(cfg, "slowmo_lr", 1.0))
+        if self.slowmo_period:
+            self.slowmo_x, self.slowmo_u = arena.theta.clone(), torch.zeros_like(arena.theta)
         self.theta_k = None
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
@@ -187,6 +196,8 @@ class CollectiveBackend(CommBackend):
             self.theta_k = self.arena.theta.clone()    # before the exchange and the mix
         if algo == "cent":
             self._step_cent()
+        elif self.slowmo_period and self.pass_num % self.slowmo_period == 0:
+            self._step_slowmo()                        # also at R = 1: the outer update on the own theta
         elif not self.comm_enabled or self.pass_num % self.local_steps:
             self._opt()                                # serial step / local step of --local-steps
         elif self.global_avg_period and self.pass_num % self.global_avg_period == 0:
@@ -234,6 +245,22 @@ class CollectiveBackend(CommBackend):
             dist.all_gather(parts, a.theta, group=self.group)
             a.theta.copy_(rank_mean(parts))
             self.bytes += a.table.n_elems * 4
+        self._opt()
+
+    def _step_slowmo(self) -> None:
+        """SlowMo sync step, the simulator's ops: avg = rank_mean(every rank's theta), slowmo_sync_(x, u, avg), theta <- x,
+        then SGD on the own gradient and momentum.  Every rank forms the same mean and runs the same update, so x and u
+        stay identical across ranks."""
+        a = self.arena
+        if self.ring.world > 1:
+            parts = [torch.empty_like(a.theta) for _ in range(self.ring.world)]
+            dist.all_gather(parts, a.theta, group=self.group)
+            self.bytes += a.table.n_elems * 4
+        else:
+            parts = [a.theta]
+        slowmo_sync_(self.slowmo_x, self.slowmo_u, rank_mean(parts), self.step_lr(self.pass_num), self.slowmo_beta,
+                     self.slowmo_lr)
+        a.theta.copy_(self.slowmo_x)
         self._opt()
 
     def _step_tracking(self) -> None:
@@ -486,6 +513,7 @@ class CollectiveBackend(CommBackend):
             if self.global_avg_period:
                 sd["global_avg_period"] = self.global_avg_period
             sd["exact_diffusion"] = self.ed
+            sd.update(slowmo_state(self))
             if self.gt:
                 for k in ("y", "g_prev", "y_in_l", "y_in_r"):
                     sd[k] = getattr(self, k).cpu().clone()
@@ -519,7 +547,11 @@ class CollectiveBackend(CommBackend):
         check_global_avg_state(sd, self.global_avg_period, self.cfg.algo)
         check_exact_diffusion_state(sd, self.ed, self.cfg.algo)
         check_qg_state(sd, self.qg, self.cfg.algo)
+        check_slowmo_state(sd, self.slowmo_period, self.slowmo_beta, self.slowmo_lr, self.cfg.algo)
         self.state.load_state_dict(sd["fsm"])
+        if self.slowmo_period:
+            self.slowmo_x.copy_(sd["slowmo_x"].to(self.slowmo_x.device))
+            self.slowmo_u.copy_(sd["slowmo_u"].to(self.slowmo_u.device))
         if self.ed:
             self.psi.copy_(sd["psi"].to(self.psi.device))
         if self.gt:

@@ -17,6 +17,10 @@ Per training step, after backward():
            (--global-avg-period P, decent on the ring / a static graph: TWO launches per step, the two-shot all-reduce
            of theta gated on "P divides the step" (a no-op launch otherwise), then the step kernel, which takes the plain
            SGD step at an averaging step)
+           (--slowmo-period tau, decent on the ring / a static graph: TWO launches per step, the SlowMo sync kernel of
+           csrc/allreduce.cu gated on "tau divides the step" -- the two-shot average plus the outer update of x and u --
+           then the step kernel: the gossip step (local_steps 1, which takes the plain SGD step at a sync step) or the
+           serial step (local_steps tau, local SGD))
   spevent  batched segmented radix-select top-k + compaction straight into the neighbours'
            inboxes, scatter of arrived records into replicas, then the dense mix+SGD kernel
 No NCCL/MPI call, no separate elementwise kernel and no host synchronisation on that path
@@ -30,7 +34,7 @@ import torch
 
 from .arena import TILE, ParamArena, TensorTable
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
-                   check_local_steps_state, check_qg_state, check_topology_state, check_tracking_state,
+                   check_local_steps_state, check_slowmo_state, slowmo_state, check_qg_state, check_topology_state, check_tracking_state,
                    check_trigger_state)
 from .topology import Graph
 from .trigger import q8_msg_bytes
@@ -59,7 +63,7 @@ def _wants_dbuf(cfg) -> bool:
             and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True)
             and not _wants_q8(cfg) and not getattr(cfg, "gradient_tracking", False)
             and getattr(cfg, "local_steps", 1) == 1 and not getattr(cfg, "exact_diffusion", False)
-            and not getattr(cfg, "global_avg_period", 0))
+            and not getattr(cfg, "global_avg_period", 0) and not getattr(cfg, "slowmo_period", 0))
 
 
 def _wants_q8(cfg) -> bool:
@@ -234,6 +238,19 @@ class P2PBackend(CommBackend):
             raise ValueError("p2p backend: --quasi-global-momentum runs the ring, double-buffered and graph step "
                              "kernels with momentum and iter-sync, without int8, tracking, exact diffusion, global "
                              "averaging or ce_push")
+        # --slowmo-period tau (decent): the gated SlowMo sync kernel, then the fused single-slot ring / static-graph step
+        # as the gossip base (local_steps 1) or the serial step as the local-SGD base (local_steps tau, on every
+        # topology: that base never exchanges).  x and u live in local device memory, identical on every rank
+        self.slowmo_period = int(getattr(cfg, "slowmo_period", 0)) if cfg.algo == "decent" else 0
+        self.slowmo_beta = float(getattr(cfg, "slowmo_beta", 0.5))
+        self.slowmo_lr = float(getattr(cfg, "slowmo_lr", 1.0))
+        self.slowmo_local = bool(self.slowmo_period) and self.local_steps == self.slowmo_period
+        if self.slowmo_period and (self.overlap or self.q8 or self.gt or self.ed or self.qg or self.global_avg_period
+                                   or self.local_steps not in (1, self.slowmo_period) or getattr(cfg, "ce_push", False)
+                                   or self.want_logs or getattr(self.graph, "period", 0)):
+            raise ValueError("p2p backend: --slowmo-period runs decent on the fused single-kernel ring / static graph "
+                             "step with --local-steps 1 or tau only")
+        self.slowmo_x = self.slowmo_u = None
         self.dbuf = _wants_dbuf(cfg) and self.do_comm
         self.ce_push = bool(getattr(cfg, "ce_push", False)) and self.overlap and cfg.algo == "decent" and self.sync
         self.nvls = self.nvls_step = False      # set in connect() when the window has a multicast mapping
@@ -319,6 +336,8 @@ class P2PBackend(CommBackend):
         if self.drift:
             self.sent = self.prev if (self.sparse or self.q8) else zf(t.n_padded)
         self.ar_ctr = zi(1)
+        if self.slowmo_period:
+            self.slowmo_x, self.slowmo_u = arena.theta.clone(), zf(t.n_padded)
         # gradient pointer table (table mode): device arrays + rotating pinned staging
         self.table_mode = bool(getattr(arena, "table_mode", False)) and cfg.algo != "cent"
         self.d_gptr = torch.zeros(t.n_tensors, dtype=torch.int64, device=dev)
@@ -328,7 +347,7 @@ class P2PBackend(CommBackend):
         self._grads_alive = None
         self.host_bytes = 0
         self._connected = False
-        self.gp = self.ap = self.ap_avg = self.ap_pga = self.sp = self.gs = self.qs = self.ts = self.es = None
+        self.gp = self.ap = self.ap_avg = self.ap_pga = self.sm = self.sp = self.gs = self.qs = self.ts = self.es = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
@@ -387,9 +406,13 @@ class P2PBackend(CommBackend):
                 "fsm.metric": 1 if self.drift else 0,
                 "sent": P(self.sent) if (self.drift and self.do_comm) else 0,
                 "local_steps": self.local_steps,
-                "global_avg_period": self.global_avg_period if self.do_comm else 0,
+                "global_avg_period": (self.global_avg_period or (0 if self.slowmo_local else self.slowmo_period))
+                                     if self.do_comm else 0,
                 "quasi_global": 1 if self.qg else 0,
             })
+            if self.slowmo_local:
+                # local-SGD base: every step the step kernel runs is the serial step -- no push, mix, flag or ack
+                gp.update({"do_mix": 0, "do_push": 0, "send_ack": 0, "local_steps": 1})
             if self.graph is None:
                 gp.update({
                     "flag_from_l": win.addr("flag_from_l"), "flag_from_r": win.addr("flag_from_r"),
@@ -520,6 +543,18 @@ class P2PBackend(CommBackend):
             pga.update({"peer_bufs": P(self.d_peer_theta), "local": P(a.theta), "mode": 0, "zero_after": 0,
                         "two_shot": 1, "gate_pass": P(self.d_pass), "gate_period": self.global_avg_period})
             self.ap_pga = pga
+        # --slowmo-period: the SlowMo sync kernel, gated on the gossip pass counter like ap_pga, sharing the launch
+        # counter, the ticket and ar_flags with the final average.  It runs at R = 1 too (a world of one)
+        self.sm = None
+        if self.slowmo_period:
+            sm = C.SlowMoParams()
+            sm.update(common)
+            sm.update({"peer_bufs": P(self.d_peer_theta), "local": P(a.theta), "mode": 0, "zero_after": 0,
+                       "two_shot": 1, "gate_pass": P(self.d_pass), "gate_period": self.slowmo_period,
+                       "shadow": P(getattr(a, "shadow", None)) if self.table_mode else 0,
+                       "x": P(self.slowmo_x), "u": P(self.slowmo_u), "beta": self.slowmo_beta,
+                       "alpha": self.slowmo_lr})
+            self.sm = sm
         # EXPERIMENTAL NVLS: multicast mappings of the same buffers (0 unless the window is a SymmWindow on
         # a fabric with multicast support) -> csrc/allreduce_nvls.cu for the two-shot launches
         mc_grad = win.mc_addr("grad") if hasattr(win, "mc_addr") else 0
@@ -555,6 +590,8 @@ class P2PBackend(CommBackend):
                "lr_len": 0 if self.d_lr is None else int(self.d_lr.numel())}
         self.gp.update(upd)
         self.ap.update(upd)
+        if self.sm is not None:
+            self.sm.update(upd)
 
     def set_sparse_init(self, prev, rep_l, rep_r) -> None:
         super().set_sparse_init(prev, rep_l, rep_r)
@@ -641,6 +678,9 @@ class P2PBackend(CommBackend):
             if self.ap_pga is not None:
                 # the average comes first: the step kernel of an averaging step runs SGD on the averaged theta
                 (C.allreduce_nvls if self.nvls else C.allreduce)(self.ap_pga, self.grid, s)
+            if self.sm is not None:
+                # the sync comes first: the step kernel of a sync step runs SGD on theta <- x
+                C.slowmo_sync(self.sm, self.grid, s)
             if self.sparse and self.do_comm:
                 if not self.overlap:
                     C.sparse_select_push(self.sp, self.grid, s)        # 3 launches: hist, candidates, compaction
@@ -655,7 +695,7 @@ class P2PBackend(CommBackend):
                 C.gossip_step_phase(self.gp, 2, self.grid, s)
             elif self.dbuf:
                 C.gossip_step_dbuf(self.gp, self.grid, s)
-            elif self.graph is not None and self.do_comm:
+            elif self.graph is not None and self.do_comm and not self.slowmo_local:
                 C.gossip_step_graph(self.gp, self.gs, self.grid, s)
             else:
                 C.gossip_step(self.gp, self.grid, s)
@@ -669,6 +709,11 @@ class P2PBackend(CommBackend):
             self.host_bytes += 2 * sum(self.msg_bytes)
         elif self.gt:
             self.host_bytes += 2 * 2 * self.table.n_elems * 4      # theta and y, to both neighbours
+        elif self.slowmo_period and self.pass_num % self.slowmo_period == 0:
+            # --slowmo-period tau: a sync step counts one all-reduce of theta (cent's convention)
+            self.host_bytes += self.table.n_elems * 4 if self.ring.world > 1 else 0
+        elif self.slowmo_local:
+            pass                                                  # local-SGD base: no exchange
         elif self.global_avg_period and self.do_comm and self.pass_num % self.global_avg_period == 0:
             # --global-avg-period P: an averaging step counts one all-reduce of theta (cent's convention)
             self.host_bytes += self.table.n_elems * 4 if self.ring.world > 1 else 0
@@ -764,6 +809,7 @@ class P2PBackend(CommBackend):
             sd["exact_diffusion"] = self.ed
             if self.global_avg_period:
                 sd["global_avg_period"] = self.global_avg_period
+            sd.update(slowmo_state(self))
             if self.ed:
                 sd["psi"] = self.psi.cpu().clone()
             if self.gt:
@@ -788,6 +834,7 @@ class P2PBackend(CommBackend):
         check_exact_diffusion_state(sd, self.ed, self.cfg.algo)
         check_global_avg_state(sd, self.global_avg_period, self.cfg.algo)
         check_qg_state(sd, self.qg, self.cfg.algo)
+        check_slowmo_state(sd, self.slowmo_period, self.slowmo_beta, self.slowmo_lr, self.cfg.algo)
         self.pass_num = int(sd["pass_num"])
         self.host_bytes = int(sd.get("host_bytes", 0))
         for k in ("thres", "last_norm", "last_iter", "slopes", "fire", "cur_norm", "counters", "d_pass"):
@@ -810,12 +857,16 @@ class P2PBackend(CommBackend):
             self.win.view("y_in_r", torch.float32).copy_(sd["y_in_r"].to(self.dev))
         if self.ed:
             self.psi.copy_(sd["psi"].to(self.dev))
+        if self.slowmo_period:
+            self.slowmo_x.copy_(sd["slowmo_x"].to(self.dev))
+            self.slowmo_u.copy_(sd["slowmo_u"].to(self.dev))
         if self.log_ring is not None:
             self._drained = self.pass_num          # log rows of the steps before the checkpoint are not replayed
         # NOTE: handshake counters (flags / acks) restart from pass_num on every rank.  Under --local-steps H the next
         # gossip step k is the first multiple of H above pass_num, so the WAR bound k - H (one-peer: k - tau * H) is at
         # most pass_num, and only that round's pushes reach the flag value k.  Under --global-avg-period P the next gossip
-        # step k waits for the ack of k - 1 or k - 2, both <= pass_num.  The all-reduce launch counter (ar_ctr) and the
+        # step k waits for the ack of k - 1 or k - 2, both <= pass_num; so does a gossip step under --slowmo-period with
+        # --local-steps 1, whose step kernel sees tau as its averaging period.  The all-reduce launch counter (ar_ctr) and the
         # ar_flags block are not part of the checkpoint: a new process starts both at zero on every rank, and a backend
         # that keeps running keeps them equal on every rank, since every rank ran the same averages
         if self.gossip:

@@ -180,6 +180,26 @@ def qg_sgd_(theta: torch.Tensor, theta_k: torch.Tensor, grad: torch.Tensor, mom:
         c = float(torch.tensor(1.0, dtype=theta.dtype).sub_(mu))
         mom.copy_(a.add_(q.mul_(c)))
 
+@torch.no_grad()
+def slowmo_sync_(x: torch.Tensor, u: torch.Tensor, avg: torch.Tensor, lr: float, beta: float, alpha: float) -> None:
+    """SlowMo's outer update at a sync step (Wang, Tantia, Ballas and Rabbat 2020), op for op as slowmo_sync_kernel of
+    csrc/allreduce.cu.  `avg` is the exact average theta_bar of the ranks' parameters, `x` the outer iterate (where the
+    cycle started) and `u` the slow momentum:
+        lr != 0:  q = (x - avg) / lr ;  u = beta*u + q ;  x = x - (alpha*lr)*u  (one fma)        lr == 0:  x = avg
+    lr, beta and alpha are rounded to the tensors' dtype once; alpha*lr is one rounded product, and the division takes a
+    0-dim tensor divisor, so CUDA divides instead of multiplying by a rounded 1/lr.  The caller then sets theta <- x."""
+    dt = x.dtype
+    lr_t = torch.tensor(lr, dtype=dt)
+    if float(lr_t) == 0.0:
+        x.copy_(avg)
+        return
+    b = float(torch.tensor(beta, dtype=dt))
+    c = float(torch.tensor(alpha, dtype=dt) * lr_t)
+    q = x.sub(avg).div_(lr_t.to(x.device))
+    u.mul_(b).add_(q)
+    x.add_(u, alpha=-c)
+
+
 Q8_BLOCK = 256          # elements per int8 scale: one warp's slice of a 2048-float tile (never straddles tensors)
 COMPRESS = ("none", "int8")
 

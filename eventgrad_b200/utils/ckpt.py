@@ -11,7 +11,9 @@ check_compress_state; decent: the `gradient_tracking` setting, and under --gradi
 period, checked on resume by check_local_steps_state; decent: the `exact_diffusion` setting, and under
 --exact-diffusion `psi`, checked on resume by check_exact_diffusion_state; decent with --global-avg-period P > 0: the
 `global_avg_period`, checked on resume by check_global_avg_state; decent/event/spevent with --quasi-global-momentum:
-`quasi_global_momentum`, checked on resume by check_qg_state), BN buffers, RNG state
+`quasi_global_momentum`, checked on resume by check_qg_state; decent with --slowmo-period tau > 0: `slowmo_period`,
+`slowmo_beta`, `slowmo_lr`, the outer iterate `slowmo_x` and the slow momentum `slowmo_u`, checked on resume by
+check_slowmo_state), BN buffers, RNG state
 (global + the loader's private augmentation generator), step counter and epoch.  Only tensors / numbers / strings / lists / dicts are stored, so
 files are read back with `weights_only=True` (no pickle code execution from a user-supplied --resume path).  The
 ranks' models differ between consensus rounds, so a decentralized run can only be resumed
