@@ -11,6 +11,7 @@ After --steps steps it reports, per run:
   loss             the last training step's loss, per rank
   bytes_per_rank   what each rank sent
   consensus        sqrt(mean_r ||theta_r - theta_bar||^2) / ||theta_bar||, before the final average
+                   (the Trainer's --consensus-every measurement, consensus_before_final_average)
   local_acc        the test accuracy of every rank's own model, before the final average
   avg_acc          the test accuracy of the averaged model
 The default data is the project's synthetic MNIST (class templates plus noise), which is known to be too easy to
@@ -21,6 +22,7 @@ import argparse
 import json
 import os
 import sys
+import tempfile
 
 import torch
 import torch.distributed as dist
@@ -31,12 +33,16 @@ from eventgrad_b200.data import load_source, synthetic_source  # noqa: E402
 from eventgrad_b200.engine.trainer import Trainer  # noqa: E402
 from eventgrad_b200.utils.dist import init_distributed, shutdown  # noqa: E402
 
+# the Trainer's consensus.csv files: not wanted here, kept out of the working directory
+_LOGS = tempfile.TemporaryDirectory(prefix="consensus_logs_")
+
 
 def run(a, env, name: str, **kw) -> dict:
     n_train = 32 * a.steps * env.world          # one epoch of a.steps steps
     cfg = preset("decent", device="cpu", backend="gloo", model="cnn2", batch_mode="per_rank", batch_size=32,
                  sampler="random", lr=a.lr, momentum=0.9, epochs=1, max_steps=a.steps, train_samples=n_train,
-                 test_samples=a.test_samples, quiet=True, partition="label", **kw)
+                 test_samples=a.test_samples, quiet=True, consensus_every=a.steps, log_dir=_LOGS.name,
+                 partition="label", **kw)
     if a.data == "synthetic":
         train, test = synthetic_source("mnist", n_train), synthetic_source("mnist", a.test_samples, train=False)
     else:
@@ -45,11 +51,6 @@ def run(a, env, name: str, **kw) -> dict:
     torch.manual_seed(0)
     tr = Trainer(cfg, env, train_source=train, test_source=test)
     tr.fit()
-    th = tr.arena.theta.detach().clone()
-    allth = [torch.empty_like(th) for _ in range(env.world)]
-    dist.all_gather(allth, th)
-    bar = torch.stack(allth).mean(0)
-    consensus = float(torch.stack([(x - bar).pow(2).sum() for x in allth]).mean().sqrt() / bar.norm())
     local = float(tr.evaluate()["test_acc"])
     accs = [None] * env.world
     sent = [None] * env.world
@@ -58,6 +59,7 @@ def run(a, env, name: str, **kw) -> dict:
     dist.all_gather_object(accs, local)
     dist.all_gather_object(sent, int(tr.backend.bytes_sent()))
     res = tr.finalize(evaluate=True)
+    consensus = res["consensus_before_final_average"]
     out = {"run": name, "world": env.world, "steps": tr.steps_done, "lr": a.lr, "data": a.data,
            "loss": [round(x, 4) for x in losses], "bytes_per_rank": sent,
            "consensus": round(consensus, 6), "local_acc": [round(x, 2) for x in accs],

@@ -11,6 +11,7 @@ decent, once with --gradient-tracking, once with --exact-diffusion and once per 
 --global-avg-periods (every P-th step an exact average over all ranks), from the same seed.  After --steps steps it
 reports, per run:
   consensus   sqrt(mean_r ||theta_r - theta_bar||^2) / ||theta_bar||, before the final average
+              (the Trainer's --consensus-every measurement, consensus_before_final_average)
   local_acc   the test accuracy of every rank's own model, before the final average
   avg_acc     the test accuracy of the averaged model
 The default data is the project's synthetic MNIST (class templates plus noise), which may be too easy to separate the
@@ -20,6 +21,7 @@ import argparse
 import json
 import os
 import sys
+import tempfile
 
 import torch
 import torch.distributed as dist
@@ -30,13 +32,16 @@ from eventgrad_b200.data import load_source, synthetic_source  # noqa: E402
 from eventgrad_b200.engine.trainer import Trainer  # noqa: E402
 from eventgrad_b200.utils.dist import init_distributed, shutdown  # noqa: E402
 
+# the Trainer's consensus.csv files: not wanted here, kept out of the working directory
+_LOGS = tempfile.TemporaryDirectory(prefix="consensus_logs_")
+
 
 def run(a, env, tracking: bool, ed: bool = False, P: int = 0) -> dict:
     n_train = 32 * a.steps * env.world          # one epoch of a.steps steps
     cfg = preset("decent", device="cpu", backend="gloo", model="cnn2", batch_mode="per_rank", batch_size=32,
                  sampler="random", partition="label", lr=a.lr, momentum=0.0, epochs=1, max_steps=a.steps,
-                 train_samples=n_train, test_samples=a.test_samples, quiet=True, gradient_tracking=tracking,
-                 exact_diffusion=ed, global_avg_period=P)
+                 train_samples=n_train, test_samples=a.test_samples, quiet=True, consensus_every=a.steps,
+                 log_dir=_LOGS.name, gradient_tracking=tracking, exact_diffusion=ed, global_avg_period=P)
     if a.data == "synthetic":
         train, test = synthetic_source("mnist", n_train), synthetic_source("mnist", a.test_samples, train=False)
     else:
@@ -46,17 +51,13 @@ def run(a, env, tracking: bool, ed: bool = False, P: int = 0) -> dict:
     tr = Trainer(cfg, env, train_source=train, test_source=test)
     classes = sorted(set(train.labels[tr.sampler.indices()].tolist()))
     tr.fit()
-    th = tr.arena.theta.detach().clone()
-    allth = [torch.empty_like(th) for _ in range(env.world)]
-    dist.all_gather(allth, th)
-    bar = torch.stack(allth).mean(0)
-    consensus = float(torch.stack([(x - bar).pow(2).sum() for x in allth]).mean().sqrt() / bar.norm())
     local = float(tr.evaluate()["test_acc"])
     accs = [None] * env.world
     cls = [None] * env.world
     dist.all_gather_object(accs, local)
     dist.all_gather_object(cls, classes)
     res = tr.finalize(evaluate=True)
+    consensus = res["consensus_before_final_average"]
     out = {"gradient_tracking": tracking, "exact_diffusion": ed, "global_avg_period": P, "world": env.world,
            "steps": tr.steps_done, "lr": a.lr, "data": a.data,
            "consensus": round(consensus, 6), "local_acc": [round(x, 2) for x in accs],

@@ -93,6 +93,8 @@ class TrainConfig:
                                      # started (SlowMo); base: gossip (local_steps 1) or local SGD (local_steps tau); 0 = off
     slowmo_beta: float = 0.5         # SlowMo slow momentum, 0 <= beta < 1
     slowmo_lr: float = 1.0           # SlowMo slow learning rate, alpha > 0
+    consensus_every: int = 0         # gossip algorithms: every N-th step measure the consensus distance
+                                     # sqrt(sum_r ||theta_r - theta_bar||^2 / R) per tensor (read-only); 0 = off
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -378,6 +380,18 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError(f"{h} does not support file_write: the reference's log format records a neighbour "
                                  "exchange at every step")
+        N = self.consensus_every
+        if isinstance(N, bool) or not isinstance(N, int) or N < 0:
+            raise ValueError(f"--consensus-every must be an integer >= 0, got {N!r}")
+        if N:
+            h = f"--consensus-every {N}"
+            if self.algo == "cent":
+                raise ValueError(f"{h} needs a gossip algorithm: cent keeps theta identical on every rank")
+            if self.sync_mode != "iter":
+                raise ValueError(f"{h} needs --sync-mode iter: a measurement waits for every rank, and async mode "
+                                 "promises no cross-rank waits in the step loop")
+            if self.backend == "refport":
+                raise ValueError(f"{h} is not supported by --backend refport")
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
@@ -531,6 +545,10 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
                         "averaging)")
     p.add_argument("--slowmo-lr", type=float, default=None, metavar="ALPHA",
                    help="SlowMo slow learning rate, ALPHA > 0 (default 1.0)")
+    p.add_argument("--consensus-every", type=int, default=None, metavar="N",
+                   help="decent/event/spevent: after every N-th step measure how far the ranks' parameters are from "
+                        "their average, per tensor, without changing training; rank 0 prints the relative distance "
+                        "per epoch and --log-dir gets consensus.csv and consensus_tensors.csv (default 0: off)")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

@@ -222,6 +222,107 @@ cudaError_t launch_slowmo_sync(const SlowMoParams& p, int grid, cudaStream_t s) 
   return cudaGetLastError();
 }
 
+// Consensus distance (--consensus-every N): after step k with N dividing k, per tensor
+// D_i = sum_r ||theta_r,i - theta_bar_i||^2 and A_i = ||theta_bar_i||^2, one persistent launch after the step kernel.
+// theta is only read; the owner of a tile reads it from every rank twice (the mean, then the deviations), so no rank's
+// copy is held in registers.  Every sum has a fixed order, so every rank and every run gets the same bits, and
+// parallel/trigger.py:consensus_stats is the oracle (fp64 sums in another order: equal to rounding).
+__global__ void __launch_bounds__(EG_THREADS, 4) consensus_kernel(const ConsensusParams p) {
+  const int b = blockIdx.x, G = gridDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // step gate: not a measurement step -> no barrier, no load, no store, no counter (PROTOCOL.md 1.14)
+  const int step = *p.gate_pass;
+  if (step % p.gate_period != 0) return;
+  const uint32_t seq = (uint32_t)(*p.step_ctr) + 1u;
+
+  cta_barrier_all_ranks(p, 0, b, G, seq);                 // every rank's theta_k is final
+  int j = 0;
+  for (int t = b; t < p.n_tiles; t += G, ++j) {
+    if ((b + j) % p.world != p.rank) continue;            // tile owner
+    const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
+    const F8 avg = reduce_tile(p, base);
+    const int i = p.tile_tensor[t];
+    // real elements of the tensor from `base` on (<= 0: all padding)
+    const int lim = p.t_numel[i] - (t - p.t_tile_start[i]) * EG_TILE - tid * EG_VEC;
+    double d = 0.0, a = 0.0;
+#pragma unroll
+    for (int e = 0; e < 8; ++e)
+      if (e < lim) a = fma((double)avg.v[e], (double)avg.v[e], a);
+    for (int r = 0; r < p.world; ++r) {
+      const F8 x = ld_f8_cg(p.peer_bufs[r] + base);
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        if (e < lim) {
+          const double q = (double)x.v[e] - (double)avg.v[e];
+          d = fma(q, q, d);
+        }
+    }
+    d = warp_sum_d(d);
+    a = warp_sum_d(a);
+    if (lane == 0) {
+      const size_t o = ((size_t)t * EG_WARPS + warp) * 2;
+      for (int r = 0; r < p.world; ++r) {
+        p.peer_part[r][o] = d;
+        p.peer_part[r][o + 1] = a;
+      }
+    }
+  }
+  // every owner of my tile set has stored its partials into my buffer, and no peer reads my theta any more
+  cta_barrier_all_ranks(p, 1, b, G, seq);
+  __shared__ int s_last;
+  if (tid == 0) {
+    __threadfence();
+    s_last = atomicAdd(p.ticket, 1u) == (unsigned)G - 1u;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  // last CTA: every CTA of this rank has passed barrier 1, so every partial has arrived.  Warp w reduces tensors
+  // w, w + 8, ...: lane l sums the tensor's (tile, warp) partials l, l + 32, ..., then the butterfly
+  __threadfence();
+  const int row = *p.ring_ctr % p.cap;
+  for (int i = warp; i < p.n_tensors; i += EG_WARPS) {
+    const int lo = p.t_tile_start[i] * EG_WARPS, n = p.t_tile_count[i] * EG_WARPS;
+    double d = 0.0, a = 0.0;
+    for (int k = lane; k < n; k += 32) {
+      d += __ldcg(p.part + (size_t)(lo + k) * 2);
+      a += __ldcg(p.part + (size_t)(lo + k) * 2 + 1);
+    }
+    d = warp_sum_d(d);
+    a = warp_sum_d(a);
+    if (lane == 0) {
+      p.ring[((size_t)row * p.n_tensors + i) * 2] = d;
+      p.ring[((size_t)row * p.n_tensors + i) * 2 + 1] = a;
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    p.ring_step[row] = step;
+    *p.ring_ctr += 1;
+    *p.ticket = 0u;
+    *p.step_ctr = (int)seq;
+  }
+}
+
+// Co-resident CTAs of the consensus kernel.  The occupancy query also loads the kernel: it is enqueued behind step
+// kernels that spin on peer ranks, and a lazy load at its first launch could wait for those kernels to finish
+int consensus_max_grid(int device) {
+  int sms = 0, per_sm = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, consensus_kernel, EG_THREADS, 0);
+  return sms * (per_sm < 1 ? 1 : per_sm);
+}
+
+cudaError_t launch_consensus(const ConsensusParams& p, int grid, cudaStream_t s) {
+  // the peer-load two-shot tile ownership only; N >= 1 on a pass counter; the partial buffers, the ring and its
+  // counters set; a ring of at least one row
+  if (p.gate_period < 1 || p.gate_pass == nullptr || !p.two_shot || p.peer_part == nullptr || p.part == nullptr ||
+      p.ring == nullptr || p.ring_step == nullptr || p.ring_ctr == nullptr || p.cap < 1 || p.tile_tensor == nullptr ||
+      p.t_tile_start == nullptr || p.t_tile_count == nullptr || p.t_numel == nullptr || p.n_tensors < 1)
+    return cudaErrorInvalidValue;
+  eg_count_launch(EG_FAM_ALLREDUCE, 1);
+  consensus_kernel<<<grid, EG_THREADS, 0, s>>>(p);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_allreduce(const AllReduceParams& p, int grid, cudaStream_t s) {
   if (p.gate_period < 0 || (p.gate_period > 0 && p.gate_pass == nullptr)) return cudaErrorInvalidValue;
   eg_count_launch(EG_FAM_ALLREDUCE, 1);

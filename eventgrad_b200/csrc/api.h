@@ -285,6 +285,29 @@ struct SlowMoParams : AllReduceParams {
   float alpha;
 };
 cudaError_t launch_slowmo_sync(const SlowMoParams& p, int grid, cudaStream_t s);
+// Consensus distance (--consensus-every N; csrc/allreduce.cu): the all-reduce block (two-shot, peer_bufs = every
+// rank's theta, gate_pass = the gossip pass counter, gate_period = N) followed by the arena's tensor table, the
+// partial buffers and the measurement ring.  After step k with N dividing k (k = *gate_pass, the step that just
+// completed) every tile owner forms theta_bar with reduce_tile's rounding and, over the tile's real elements, in fp64,
+//   D = sum_r (theta_r - theta_bar)^2        A = theta_bar^2
+// per (tile, warp); it stores both into every rank's partial buffer, and the last CTA of every rank reduces them per
+// tensor into ring row (*ring_ctr mod cap): [n_tensors][2] doubles, ring_step[row] = k.  theta is only read.  A
+// separate struct, so AllReduceParams and the all-reduce instances keep their layout and code
+struct ConsensusParams : AllReduceParams {
+  double* const* peer_part;  // device array [world]: each rank's partial buffer [n_tiles][EG_WARPS][2] (peer-mapped)
+  const double* part;        // == peer_part[rank]
+  const int* tile_tensor;    // [n_tiles]
+  const int* t_tile_start;   // [n_tensors]
+  const int* t_tile_count;
+  const int* t_numel;
+  int n_tensors;
+  double* ring;              // [cap][n_tensors][2] (local)
+  int* ring_step;            // [cap]
+  int* ring_ctr;             // measurements written so far
+  int cap;
+};
+int consensus_max_grid(int device);  // co-resident CTAs; also loads the kernel before any step kernel spins
+cudaError_t launch_consensus(const ConsensusParams& p, int grid, cudaStream_t s);
 // experimental NVLink-SHARP variant (csrc/allreduce_nvls.cu): multimem.ld_reduce + multimem.st, two-shot only
 cudaError_t launch_allreduce_nvls(const AllReduceParams& p, int grid, cudaStream_t s);
 

@@ -120,6 +120,20 @@ static const std::unordered_map<std::string, Setter<SlowMoParams>> kSlowMo = [] 
   return m;
 }();
 
+// ConsensusParams: every AllReduceParams field plus the table, the partial buffers and the ring
+static const std::unordered_map<std::string, Setter<ConsensusParams>> kConsensus = [] {
+  std::unordered_map<std::string, Setter<ConsensusParams>> m;
+  for (const auto& kv : kAllReduce) {
+    const Setter<AllReduceParams> f = kv.second;
+    m.emplace(kv.first, [f](ConsensusParams& p, py::object v) { f(p, v); });
+  }
+  m.insert({PTRF(ConsensusParams, peer_part), PTRF(ConsensusParams, part), PTRF(ConsensusParams, tile_tensor),
+            PTRF(ConsensusParams, t_tile_start), PTRF(ConsensusParams, t_tile_count), PTRF(ConsensusParams, t_numel),
+            NUMF(ConsensusParams, n_tensors), PTRF(ConsensusParams, ring), PTRF(ConsensusParams, ring_step),
+            PTRF(ConsensusParams, ring_ctr), NUMF(ConsensusParams, cap)});
+  return m;
+}();
+
 static const std::unordered_map<std::string, Setter<SparseParams>> kSparse = {
     PTRF(SparseParams, theta), PTRF(SparseParams, prev), PTRF(SparseParams, rep_l), PTRF(SparseParams, rep_r),
     PTRF(SparseParams, rec_from_l), PTRF(SparseParams, rec_from_r), PTRF(SparseParams, rec_to_l),
@@ -198,6 +212,7 @@ PYBIND11_MODULE(_C, m) {
   bind_params<EdSlots>(m, "EdSlots", kEd);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
   bind_params<SlowMoParams>(m, "SlowMoParams", kSlowMo);
+  bind_params<ConsensusParams>(m, "ConsensusParams", kConsensus);
   bind_params<SparseParams>(m, "SparseParams", kSparse);
   bind_params<BnParams>(m, "BnParams", kBn);
 
@@ -242,6 +257,10 @@ PYBIND11_MODULE(_C, m) {
   });
   m.def("slowmo_sync", [](const SlowMoParams& p, int grid, uintptr_t s) {
     check(launch_slowmo_sync(p, grid, S(s)), "slowmo_sync");
+  });
+  m.def("consensus_max_grid", &consensus_max_grid);
+  m.def("consensus", [](const ConsensusParams& p, int grid, uintptr_t s) {
+    check(launch_consensus(p, grid, S(s)), "consensus");
   });
   m.def("allreduce_nvls", [](const AllReduceParams& p, int grid, uintptr_t s) {
     check(launch_allreduce_nvls(p, grid, S(s)), "allreduce_nvls");

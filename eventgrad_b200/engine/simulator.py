@@ -7,15 +7,15 @@ baseline and the fused CUDA kernels are all tested against this.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
 from ..parallel.arena import TensorTable
 from ..parallel.topology import Graph
-from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode,
-                                q8_encode, q8_msg_bytes, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
-                                trigger_step)
+from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, consensus_stats, drift_norms, mix2_, mix3_,
+                                mixk_, q8_decode, q8_encode, q8_msg_bytes, qg_sgd_, rank_mean, sgd_, slowmo_sync_,
+                                topk_select, trigger_step)
 from .lr_schedule import lr_at
 
 
@@ -26,7 +26,8 @@ class RingSimulator:
                  weight_decay: float = 0.0, nesterov: bool = False, lr_table: Optional[torch.Tensor] = None,
                  offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1,
                  exact_diffusion: bool = False, global_avg_period: int = 0, quasi_global: bool = False,
-                 slowmo_period: int = 0, slowmo_beta: float = 0.5, slowmo_lr: float = 1.0):
+                 slowmo_period: int = 0, slowmo_beta: float = 0.5, slowmo_lr: float = 1.0,
+                 consensus_every: int = 0):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -62,7 +63,11 @@ class RingSimulator:
         rank.  At step k with tau dividing k every rank forms avg = rank_mean(theta), runs slowmo_sync_(x, u, avg, lr_k,
         `slowmo_beta`, `slowmo_lr`), sets theta <- x and takes its own SGD step; such a step counts n_elems * 4 bytes per
         rank (0 at R = 1, where the outer update still runs on the rank's own theta).  The other steps are the base:
-        decent's gossip step with local_steps = 1, the serial SGD step with local_steps = tau (local SGD).  0: off."""
+        decent's gossip step with local_steps = 1, the serial SGD step with local_steps = tau (local SGD).  0: off.
+        `consensus_every=N` (decent, event, spevent): after step k with N dividing k, append (k, D, A) of
+        consensus_stats(theta, table) to `self.consensus` -- D_i = sum_r ||theta_r,i - theta_bar_i||^2 and
+        A_i = ||theta_bar_i||^2 in float64, theta_bar = rank_mean(theta).  Read-only: training is unchanged.  At R = 1
+        every measurement is zero.  0: off."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -118,6 +123,12 @@ class RingSimulator:
         if self.slowmo_period:
             self.slowmo_x = [theta0.clone() for _ in range(world)]
             self.slowmo_u = [torch.zeros_like(theta0) for _ in range(world)]
+        if isinstance(consensus_every, bool) or int(consensus_every) != consensus_every or consensus_every < 0:
+            raise ValueError(f"consensus_every must be an integer >= 0, got {consensus_every!r}")
+        if consensus_every and algo == "cent":
+            raise ValueError("consensus distance: cent keeps theta identical on every rank")
+        self.consensus_every = int(consensus_every)
+        self.consensus: List[Tuple[int, torch.Tensor, torch.Tensor]] = []
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
         self.lr, self.mu = lr, momentum
@@ -214,6 +225,20 @@ class RingSimulator:
     @torch.no_grad()
     def step(self, grads: Sequence[torch.Tensor], fires: Optional[Sequence[torch.Tensor]] = None,
              norms: Optional[Sequence[torch.Tensor]] = None) -> None:
+        """One training step of every rank (_step), then the consensus measurement when N divides the step."""
+        self._step(grads, fires, norms)
+        if self.consensus_every and self.pass_num % self.consensus_every == 0:
+            self.consensus.append((self.pass_num, *self.consensus_stats()))
+
+    def consensus_stats(self):
+        """(D, A) of the ranks' current theta (parallel/trigger.py:consensus_stats); zeros at R = 1."""
+        if self.R == 1:
+            z = torch.zeros(self.table.n_tensors, dtype=torch.float64)
+            return z, z.clone()
+        return consensus_stats(self.theta, self.table)
+
+    def _step(self, grads: Sequence[torch.Tensor], fires: Optional[Sequence[torch.Tensor]] = None,
+              norms: Optional[Sequence[torch.Tensor]] = None) -> None:
         """`fires` (optional, one bool mask per rank) overrides the trigger decisions -- used to
         compare the data path of a kernel bit-for-bit under the kernel's own decisions; `norms`
         (optional, one [sz] tensor per rank) replaces the oracle's own norm computation (trigger_norms: the drift

@@ -15,6 +15,7 @@ What is different by design:
 """
 from __future__ import annotations
 
+import os
 import time
 from typing import Optional
 
@@ -25,6 +26,7 @@ from ..config import TrainConfig
 from ..data import BatchLoader, ShardSampler, eval_batches, load_source, per_rank_batch
 from ..models import build_model
 from ..parallel import Graph, ParamArena, Ring, make_backend
+from ..parallel.trigger import consensus_values
 from ..utils.ckpt import ckpt_path, load_checkpoint, save_checkpoint
 from ..utils.dist import DistEnv, barrier
 from ..utils.logfiles import RefLogWriter
@@ -99,6 +101,10 @@ class Trainer:
         if not lr_schedule.is_constant(cfg):
             # one lr per step of the run, indexed by the backend's (device) pass counter -- also after a resume
             self.backend.set_lr_table(lr_schedule.lr_table(cfg, len(self.loader)))
+        if cfg.consensus_every:
+            # the measurements are drained at every epoch boundary: room for one epoch's worth
+            self.backend.set_consensus_capacity(len(self.loader) // cfg.consensus_every + 1)
+        self.consensus_last = None                # (step, distance, relative) of the latest measurement
         self.logw = RefLogWriter(cfg.log_dir, env.rank, cfg.algo, cfg.dataset, bool(cfg.file_write))
         self.timer = PhaseTimer(dev, enabled=bool(cfg.phase_timers))
         self.correct = torch.zeros((), dtype=torch.int64, device=dev)
@@ -278,6 +284,8 @@ class Trainer:
                 else:
                     print(f"Accuracy in epoch {self.epoch} - {acc:g}", flush=True)     # event.cpp:489
             self.last_train_acc = acc
+            if cfg.consensus_every:
+                self._drain_consensus()
             if cfg.file_write:
                 self.logw.write_steps(self.backend.drain_logs())
                 for pn, l in ep_losses:
@@ -298,6 +306,37 @@ class Trainer:
             if env.rank == 0 and not cfg.quiet:
                 print("phase timers (ms/call): " + ", ".join(f"{k}={v:.3f}" for k, v in ms.items()), flush=True)
             self.phase_ms = ms
+
+    def _drain_consensus(self) -> None:
+        """Epoch boundary under --consensus-every: take the epoch's measurements from the backend, print the latest
+        relative distance (rank 0) and append them to consensus.csv / consensus_tensors.csv in --log-dir (rank 0;
+        every rank holds the same values)."""
+        rows = self.backend.drain_consensus()
+        if not rows:
+            return
+        R, names = self.env.world, self.arena.table.names
+        vals = [(k, *consensus_values(D, A, R)) for k, D, A in rows]
+        self.consensus_last = vals[-1]
+        if self.env.rank != 0:
+            return
+        if not self.cfg.quiet:
+            print(f"Consensus distance in epoch {self.epoch} - {vals[-1][2]:g}", flush=True)
+        os.makedirs(self.cfg.log_dir, exist_ok=True)
+        for fname, header, lines in (
+                ("consensus.csv", "step,distance,relative", [f"{k},{d!r},{r!r}" for k, d, r in vals]),
+                ("consensus_tensors.csv", "step,tensor,sq_dist,sq_norm_mean",
+                 [f"{k},{names[i]},{float(D[i])!r},{float(A[i])!r}" for k, D, A in rows for i in range(len(names))])):
+            path = os.path.join(self.cfg.log_dir, fname)
+            if not self._consensus_files_open:
+                # a fresh run starts the files; a resumed one appends to what the run before it wrote
+                if not self.cfg.resume or not os.path.exists(path):
+                    with open(path, "w") as f:
+                        f.write(header + "\n")
+            with open(path, "a") as f:
+                f.write("".join(line + "\n" for line in lines))
+        self._consensus_files_open = True
+
+    _consensus_files_open = False
 
     def _check_device_status(self) -> None:
         """Raise if a device-side wait timed out (sticky status words of the fused kernels): a wedged
@@ -320,7 +359,14 @@ class Trainer:
             print(f"No of events in rank {env.rank} - {self.backend.num_events()}", flush=True)
         res["events_rank"] = self.backend.num_events()
         res["bytes_sent_rank"] = self.backend.bytes_sent()
+        if cfg.consensus_every:
+            res["consensus_last"] = None if self.consensus_last is None else self.consensus_last[2]
         if cfg.algo != "cent":
+            if cfg.consensus_every:
+                # one more, ungated measurement of the models the final average is about to merge
+                barrier(env)
+                D, A = self.backend.measure_consensus()
+                res["consensus_before_final_average"] = consensus_values(D, A, env.world)[1]
             # ranks may be skewed here (async mode has no per-step handshake; a slow checkpoint write or autotune on
             # one rank): meet on the host first so nobody spins in the all-reduce kernel against its device timeout
             barrier(env)

@@ -91,6 +91,29 @@ class LocalWorld:
         for be in self.backends:
             be.check_status()
 
+    def measure_consensus(self):
+        """One ungated consensus measurement (--consensus-every) of every rank's current theta, all R launches in
+        flight together; returns each rank's (D, A)."""
+        cur = torch.cuda.current_stream(self.device)
+        for st in self.streams:
+            st.wait_stream(cur)
+        for r in range(self.world):
+            with torch.cuda.stream(self.streams[r]):
+                self.backends[r].launch_consensus_now()
+        for st in self.streams:
+            cur.wait_stream(st)
+        torch.cuda.synchronize(self.device)
+        out = []
+        for be in self.backends:
+            be.check_status()
+            if not be.cons:
+                out.append(be.measure_consensus())          # R = 1: zeros, nothing launched
+                continue
+            rows = be.drain_consensus()
+            be._cons_held = rows[:-1]
+            out.append(rows[-1][1:])
+        return out
+
     def close(self) -> None:
         torch.cuda.synchronize(self.device)
         for be in self.backends:

@@ -212,6 +212,19 @@ class CommBackend:
         out, self.logs = self.logs, []
         return out
 
+    # -- consensus distance (--consensus-every N) -----------------------------------------
+    def set_consensus_capacity(self, cap: int) -> None:
+        """Measurements kept between two drains (the p2p backend's device ring); the host-side backends keep all."""
+
+    def drain_consensus(self) -> List:
+        """Measurements since the last drain, oldest first: (step, D, A) with D and A float64 CPU tensors [n_tensors]
+        (parallel/trigger.py:consensus_stats)."""
+        return []
+
+    def measure_consensus(self):
+        """(D, A) of the current parameters, measured now whatever the step; every rank must call it."""
+        raise NotImplementedError
+
     def synchronize(self) -> None:
         pass
 

@@ -20,6 +20,7 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
           the outer iterate x and slow momentum u, sets theta <- x and takes the SGD step
   --exact-diffusion (decent, ring): p = SGD(theta), phi = p + (theta - psi), psi <- p; phi travels in the ring exchange,
           and theta <- (phi + (phi + L + R)/3) / 2
+  --consensus-every N (decent/event/spevent): after every N-th step all_gathers theta and records consensus_stats
   --quasi-global-momentum (decent/event/spevent): theta_k is snapshotted before the exchange and every SGD update is
           qg_sgd_, whose momentum follows theta_k - theta_{k+1}
 
@@ -39,8 +40,9 @@ import torch.distributed as dist
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
                    check_local_steps_state, check_qg_state, check_slowmo_state, check_topology_state,
                    check_tracking_state, check_trigger_state, slowmo_state)
-from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, drift_norms, mix2_, mix3_, mixk_, q8_decode, q8_encode,
-                      q8_msg_bytes, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select, trigger_step)
+from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, consensus_stats, drift_norms, mix2_, mix3_, mixk_,
+                      q8_decode, q8_encode, q8_msg_bytes, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
+                      trigger_step)
 
 
 class CollectiveBackend(CommBackend):
@@ -110,6 +112,10 @@ class CollectiveBackend(CommBackend):
         self.slowmo_lr = float(getattr(cfg, "slowmo_lr", 1.0))
         if self.slowmo_period:
             self.slowmo_x, self.slowmo_u = arena.theta.clone(), torch.zeros_like(arena.theta)
+        # --consensus-every N: after step k with N dividing k, (k, D, A) of every rank's theta; the all_gather is not
+        # counted in bytes_sent
+        self.consensus_every = int(getattr(cfg, "consensus_every", 0)) if gossip else 0
+        self.consensus_rows = []
         self.theta_k = None
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
@@ -208,6 +214,22 @@ class CollectiveBackend(CommBackend):
             self._step_event()
         else:
             self._step_spevent()
+        if self.consensus_every and self.pass_num % self.consensus_every == 0:
+            self.consensus_rows.append((self.pass_num, *self.measure_consensus()))
+
+    def measure_consensus(self):
+        """(D, A) of every rank's current theta: all_gather, then consensus_stats (zeros at R = 1, no collective)."""
+        a = self.arena
+        if self.ring.world == 1:
+            z = torch.zeros(a.table.n_tensors, dtype=torch.float64)
+            return z, z.clone()
+        parts = [torch.empty_like(a.theta) for _ in range(self.ring.world)]
+        dist.all_gather(parts, a.theta, group=self.group)
+        return consensus_stats(parts, a.table)
+
+    def drain_consensus(self):
+        out, self.consensus_rows = self.consensus_rows, []
+        return out
 
     def _step_cent(self) -> None:
         a = self.arena

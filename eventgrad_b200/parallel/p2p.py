@@ -21,6 +21,9 @@ Per training step, after backward():
            csrc/allreduce.cu gated on "tau divides the step" -- the two-shot average plus the outer update of x and u --
            then the step kernel: the gossip step (local_steps 1, which takes the plain SGD step at a sync step) or the
            serial step (local_steps tau, local SGD))
+           (--consensus-every N, decent/event/spevent: one more launch per step after the step kernel, the
+           consensus kernel of csrc/allreduce.cu gated on "N divides the step that just completed"; it only reads theta
+           and writes per-tensor sums into a device ring that drain_consensus() reads at epoch boundaries)
   spevent  batched segmented radix-select top-k + compaction straight into the neighbours'
            inboxes, scatter of arrived records into replicas, then the dense mix+SGD kernel
 No NCCL/MPI call, no separate elementwise kernel and no host synchronisation on that path
@@ -89,6 +92,20 @@ def _graph_of(cfg, rank: int, world: int):
     return None if g.is_ring else g
 
 
+def _wants_consensus(cfg, world: int) -> bool:
+    """--consensus-every N on a gossip algorithm with peers: the consensus kernel runs, and the window gets its
+    partial buffer.  At R = 1 every measurement is zero and nothing is launched."""
+    return bool(getattr(cfg, "consensus_every", 0)) and cfg.algo in ("decent", "event", "spevent") and world > 1
+
+
+def _add_consensus(lay: Layout, table: TensorTable, cfg, world: int) -> Layout:
+    """The consensus kernel's partial buffer, last in the window and only with the flag on, so every other window
+    keeps its layout: two fp64 sums per (tile, warp), written by the tile's owner into every rank's copy."""
+    if _wants_consensus(cfg, world):
+        lay.add("cons_part", table.n_tiles * 8 * 2 * 8)
+    return lay
+
+
 def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None) -> Layout:
     lay = Layout()
     n = table.n_padded * 4
@@ -103,7 +120,7 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None)
             lay.add(f"flag_from_{k}", nflag)
             lay.add(f"ack_from_{k}", 256)
         lay.add("ar_flags", 3 * max_grid * world * 4)
-        return lay
+        return _add_consensus(lay, table, cfg, world)
     if _wants_q8(cfg):
         # int8 codes (one byte per arena element) and one fp32 scale per (tile, warp) block from each neighbour
         lay.add("q_from_l", table.n_padded)
@@ -134,7 +151,7 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None)
     lay.add("pushed_from_l", 256)
     lay.add("pushed_from_r", 256)
     lay.add("ar_flags", 3 * max_grid * world * 4)
-    return lay
+    return _add_consensus(lay, table, cfg, world)
 
 
 def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
@@ -155,6 +172,10 @@ def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
         max_grid = min(max_grid, C.gossip_gt_max_grid(env.device.index or 0))
     if _wants_ed(cfg, env.world):
         max_grid = min(max_grid, C.gossip_ed_max_grid(env.device.index or 0))
+    if _wants_consensus(cfg, env.world):
+        # the query loads the consensus kernel now: enqueued behind spinning step kernels, a lazy load at its first
+        # launch could wait for them to finish
+        max_grid = min(max_grid, C.consensus_max_grid(env.device.index or 0))
     lay = build_layout(table, cfg, env.world, max_grid, graph)
     symm = wants_symm_window(env) and bootstrap is None      # NVLS path: torch symmetric memory + multicast mapping
     win = (SymmWindow if symm else Window)(lay, env.rank, env.world, env.device)
@@ -251,6 +272,16 @@ class P2PBackend(CommBackend):
             raise ValueError("p2p backend: --slowmo-period runs decent on the fused single-kernel ring / static graph "
                              "step with --local-steps 1 or tau only")
         self.slowmo_x = self.slowmo_u = None
+        # --consensus-every N: the gated consensus kernel after the step kernel (R >= 2); its rows wait in a device
+        # ring of `cons_cap` rows until drain_consensus().  At R = 1 account_step() records the zero rows itself
+        self.consensus_every = int(getattr(cfg, "consensus_every", 0)) if self.gossip else 0
+        if self.consensus_every and not self.sync:
+            raise ValueError("p2p backend: --consensus-every needs iter-sync")
+        self.cons = _wants_consensus(cfg, ring.world)
+        self.cons_cap = 1024
+        self._cons_held = []           # rows read from the ring (or recorded at R = 1) and not yet returned
+        self._cons_drained = 0         # ring rows read so far
+        self.cp = self.cp_now = None
         self.dbuf = _wants_dbuf(cfg) and self.do_comm
         self.ce_push = bool(getattr(cfg, "ce_push", False)) and self.overlap and cfg.algo == "decent" and self.sync
         self.nvls = self.nvls_step = False      # set in connect() when the window has a multicast mapping
@@ -336,6 +367,10 @@ class P2PBackend(CommBackend):
         if self.drift:
             self.sent = self.prev if (self.sparse or self.q8) else zf(t.n_padded)
         self.ar_ctr = zi(1)
+        if self.cons:
+            self.cons_ring = torch.zeros(self.cons_cap * t.n_tensors * 2, dtype=torch.float64, device=dev)
+            self.cons_step, self.cons_ctr = zi(self.cons_cap), zi(1)
+            self.d_tile_count = i32(t.tile_count)
         if self.slowmo_period:
             self.slowmo_x, self.slowmo_u = arena.theta.clone(), zf(t.n_padded)
         # gradient pointer table (table mode): device arrays + rotating pinned staging
@@ -555,6 +590,22 @@ class P2PBackend(CommBackend):
                        "x": P(self.slowmo_x), "u": P(self.slowmo_u), "beta": self.slowmo_beta,
                        "alpha": self.slowmo_lr})
             self.sm = sm
+        # --consensus-every: the consensus kernel, gated on the gossip pass counter after the step kernel that advanced
+        # it, sharing the launch counter, the ticket and ar_flags with the final average.  cp_now is the same block with
+        # N = 1 (every launch measures): the ungated measurement of measure_consensus()
+        if self.cons:
+            self.d_peer_part = torch.tensor([win.addr("cons_part", r) for r in range(W)], dtype=torch.int64,
+                                            device=self.dev)
+            f = {"peer_bufs": P(self.d_peer_theta), "local": P(a.theta), "mode": 0, "zero_after": 0, "two_shot": 1,
+                 "gate_pass": P(self.d_pass), "peer_part": P(self.d_peer_part), "part": win.addr("cons_part"),
+                 "tile_tensor": P(self.d_tile_tensor), "t_tile_start": P(self.d_tile_start),
+                 "t_tile_count": P(self.d_tile_count), "t_numel": P(self.d_numel), "n_tensors": t.n_tensors}
+            self.cp, self.cp_now = C.ConsensusParams(), C.ConsensusParams()
+            for blk, n in ((self.cp, self.consensus_every), (self.cp_now, 1)):
+                blk.update(common)
+                blk.update(f)
+                blk.update({"gate_period": n})
+            self._set_cons_ring()
         # EXPERIMENTAL NVLS: multicast mappings of the same buffers (0 unless the window is a SymmWindow on
         # a fabric with multicast support) -> csrc/allreduce_nvls.cu for the two-shot launches
         mc_grad = win.mc_addr("grad") if hasattr(win, "mc_addr") else 0
@@ -574,6 +625,68 @@ class P2PBackend(CommBackend):
 
     def _stream(self) -> int:
         return torch.cuda.current_stream(self.dev).cuda_stream
+
+    # ------------------------------------------------------------------ consensus distance
+    def _set_cons_ring(self) -> None:
+        ring = {"ring": self.cons_ring.data_ptr(), "ring_step": self.cons_step.data_ptr(),
+                "ring_ctr": self.cons_ctr.data_ptr(), "cap": self.cons_cap}
+        self.cp.update(ring)
+        self.cp_now.update(ring)
+
+    def set_consensus_capacity(self, cap: int) -> None:
+        """Rows the device ring holds between two drain_consensus() calls (default 1024).  Call before the first step
+        (a graph captured earlier keeps the ring it was captured with)."""
+        cap = int(cap)
+        if cap < 1:
+            raise ValueError(f"consensus ring capacity must be >= 1, got {cap}")
+        if not self.cons or cap == self.cons_cap:
+            return
+        if self.pass_num or self._cons_drained:
+            raise RuntimeError("set_consensus_capacity must be called before the first step")
+        self.cons_cap = cap
+        self.cons_ring = torch.zeros(cap * self.table.n_tensors * 2, dtype=torch.float64, device=self.dev)
+        self.cons_step = torch.zeros(cap, dtype=torch.int32, device=self.dev)
+        if self._connected:
+            self._set_cons_ring()
+
+    def launch_consensus_now(self) -> None:
+        """Enqueue one ungated measurement of the current theta on the current stream (every rank must)."""
+        if self.cons:
+            with torch.cuda.device(self.dev):
+                self.C.consensus(self.cp_now, self.grid, self._stream())
+
+    def drain_consensus(self):
+        """The measurements since the last drain, oldest first: a list of (step, D, A), D and A float64 CPU tensors
+        [n_tensors] (parallel/trigger.py:consensus_stats).  One host synchronisation.  Raises when the ring overwrote
+        rows that were never drained."""
+        out, self._cons_held = self._cons_held, []
+        if not self.cons:
+            return out
+        torch.cuda.synchronize(self.dev)
+        ctr = int(self.cons_ctr.item())
+        n = ctr - self._cons_drained
+        if n > self.cons_cap:
+            raise RuntimeError(f"consensus ring overwrote {n - self.cons_cap} undrained measurements: drain at least "
+                               f"every {self.cons_cap} measurements (set_consensus_capacity)")
+        nt = self.table.n_tensors
+        ring = self.cons_ring.view(self.cons_cap, nt, 2).cpu()
+        steps = self.cons_step.cpu()
+        for j in range(self._cons_drained, ctr):
+            row = j % self.cons_cap
+            out.append((int(steps[row]), ring[row, :, 0].clone(), ring[row, :, 1].clone()))
+        self._cons_drained = ctr
+        return out
+
+    def measure_consensus(self):
+        """(D, A) of the current theta, measured now whatever the step: the kernel with N = 1 (zeros at R = 1).
+        Earlier undrained rows stay for the next drain_consensus()."""
+        if not self.cons:
+            z = torch.zeros(self.table.n_tensors, dtype=torch.float64)
+            return z, z.clone()
+        self.launch_consensus_now()
+        rows = self.drain_consensus()
+        self._cons_held = rows[:-1]
+        return rows[-1][1], rows[-1][2]
 
     # ------------------------------------------------------------------ learning-rate schedule
     def set_lr_table(self, table) -> None:
@@ -699,10 +812,16 @@ class P2PBackend(CommBackend):
                 C.gossip_step_graph(self.gp, self.gs, self.grid, s)
             else:
                 C.gossip_step(self.gp, self.grid, s)
+            if self.cp is not None:
+                # after the step kernel that completed the step: it measures theta_{k} when N divides k
+                C.consensus(self.cp, self.grid, s)
 
     def account_step(self) -> None:
         """Host-side bookkeeping of one executed step (after launch() or a graph replay)."""
         self.pass_num += 1
+        if self.consensus_every and not self.cons and self.pass_num % self.consensus_every == 0:
+            z = torch.zeros(self.table.n_tensors, dtype=torch.float64)     # R = 1: no launch, the distance is 0
+            self._cons_held.append((self.pass_num, z, z.clone()))
         if self.cfg.algo == "cent" and self.ring.world > 1:
             self.host_bytes += self.table.n_elems * 4
         elif self.cfg.algo == "decent" and self.do_comm and self.q8:
@@ -862,6 +981,9 @@ class P2PBackend(CommBackend):
             self.slowmo_u.copy_(sd["slowmo_u"].to(self.dev))
         if self.log_ring is not None:
             self._drained = self.pass_num          # log rows of the steps before the checkpoint are not replayed
+        if self.cons:
+            self._cons_drained = int(self.cons_ctr.item())     # nor are consensus rows
+        self._cons_held = []
         # NOTE: handshake counters (flags / acks) restart from pass_num on every rank.  Under --local-steps H the next
         # gossip step k is the first multiple of H above pass_num, so the WAR bound k - H (one-peer: k - tau * H) is at
         # most pass_num, and only that round's pushes reach the flag value k.  Under --global-avg-period P the next gossip

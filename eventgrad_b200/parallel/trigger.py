@@ -200,6 +200,33 @@ def slowmo_sync_(x: torch.Tensor, u: torch.Tensor, avg: torch.Tensor, lr: float,
     x.add_(u, alpha=-c)
 
 
+@torch.no_grad()
+def consensus_stats(thetas, table):
+    """Per-tensor consensus statistics of the ranks' flat arenas `thetas` (--consensus-every), the oracle of
+    consensus_kernel in csrc/allreduce.cu.  theta_bar = rank_mean(thetas) in the arenas' dtype (the average that
+    Gossip-PGA forms); then, over the numel real elements of tensor i (padding excluded), in float64:
+        D_i = sum_r ||theta_r,i - theta_bar_i||^2        A_i = ||theta_bar_i||^2
+    Returns (D, A), float64 CPU tensors of length n_tensors."""
+    avg = rank_mean(thetas).double()
+    xs = [t.double() for t in thetas]
+    D = torch.zeros(table.n_tensors, dtype=torch.float64)
+    A = torch.zeros(table.n_tensors, dtype=torch.float64)
+    for i, (o, n) in enumerate(zip(table.offsets, table.numels)):
+        a = avg[o:o + n]
+        A[i] = float(a.square().sum())
+        D[i] = float(sum(x[o:o + n].sub(a).square().sum() for x in xs))
+    return D, A
+
+
+def consensus_values(D, A, world: int):
+    """(distance, relative) of one measurement: distance = sqrt(sum_i D_i / R), relative = distance / sqrt(sum_i A_i),
+    the consensus distance sqrt(mean_r ||theta_r - theta_bar||^2) / ||theta_bar||.  relative is 0 when every rank holds
+    the zero vector."""
+    dist = (float(sum(float(d) for d in D)) / world) ** 0.5
+    norm = float(sum(float(a) for a in A)) ** 0.5
+    return dist, (dist / norm if norm > 0.0 else (0.0 if dist == 0.0 else float("inf")))
+
+
 Q8_BLOCK = 256          # elements per int8 scale: one warp's slice of a 2048-float tile (never straddles tensors)
 COMPRESS = ("none", "int8")
 
