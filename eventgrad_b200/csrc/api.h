@@ -5,6 +5,9 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+#include <utility>
+#include <vector>
+
 #define EG_TILE 2048     // fp32 elements per tile == parallel/arena.py:TILE
 #define EG_THREADS 256
 #define EG_MAX_SLOTS 8   // inbox slots of a circulant gossip graph: 2 per offset, <= 4 offsets (parallel/topology.py)
@@ -463,6 +466,7 @@ cudaError_t launch_split3(const float* src, __nv_bfloat16* dst, size_t n, cudaSt
 cudaError_t launch_split3_parity(const float* src, __nv_bfloat16* dst, int N, int H, int W, int C, cudaStream_t s);
 cudaError_t launch_split3_stem(const float* src, __nv_bfloat16* dst, int N, int H, int W, cudaStream_t s);
 cudaError_t launch_conv_wprep(const float* w, __nv_bfloat16* wp, __nv_bfloat16* wtp, int Co, int T, int Ci, cudaStream_t s);
+cudaError_t conv_graph_kernel_priorities(cudaGraph_t g, std::vector<std::pair<int, int>>* out);
 
 // ------------------------------------------------------------------ IPC window runtime
 // The RMA-window replacement (MPI_Alloc_mem + MPI_Win_create, event.cpp:138-147).

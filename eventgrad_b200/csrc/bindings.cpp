@@ -442,6 +442,11 @@ PYBIND11_MODULE(_C, m) {
     fill(p, taps);
     check(launch_conv_wgrad(p, reinterpret_cast<float*>(dw), splits, S(s)), "conv_wgrad");
   });
+  m.def("conv_graph_kernel_priorities", [](uintptr_t graph) {
+    std::vector<std::pair<int, int>> out;
+    check(conv_graph_kernel_priorities(reinterpret_cast<cudaGraph_t>(graph), &out), "conv_graph_kernel_priorities");
+    return out;
+  });
   m.def("decode_augment",
         [](uintptr_t in, uintptr_t out, uintptr_t oy, uintptr_t ox, uintptr_t flip, int B, int C, int H, int W,
            int pad, float scale, float mean, float inv_std, int out_bf16, int nhwc, uintptr_t s) {

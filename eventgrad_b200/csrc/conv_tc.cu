@@ -701,14 +701,34 @@ cudaError_t launch_conv_fprop(const ConvTcParams& p0, int sm_count, cudaStream_t
   return cudaGetLastError();
 }
 
+// The weight gradient runs at the device's lowest priority, also as a node of a captured graph (the attribute is
+// recorded on the kernel node).  It is off the critical path: nothing reads dw before the optimizer step, so when an
+// SM frees up, a pending CTA of the higher-priority work on the main stream (data gradients, BatchNorm) takes it first.
+static cudaLaunchConfig_t low_priority_config(dim3 grid, unsigned block, size_t smem, cudaStream_t s,
+                                              cudaLaunchAttribute* attr) {
+  int least = 0, greatest = 0;
+  cudaDeviceGetStreamPriorityRange(&least, &greatest);
+  attr->id = cudaLaunchAttributePriority;
+  attr->val.priority = least;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = dim3(block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = s;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+
 template <int NT, int STAGES>
 static cudaError_t wgrad_launch(const CUtensorMap& tmX, const CUtensorMap& tmG, const ConvTcParams& p, dim3 grid,
                                 cudaStream_t s) {
   const size_t smem = (size_t)STAGES * (3 * CV_APLANE + 3 * NT * 128) + 256 + 1024;
   cudaError_t e = cudaFuncSetAttribute(conv3x3_wgrad_kernel<NT, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  conv3x3_wgrad_kernel<NT, STAGES><<<grid, CV_THREADS, smem, s>>>(tmX, tmG, p);
-  return cudaGetLastError();
+  cudaLaunchAttribute prio;
+  cudaLaunchConfig_t cfg = low_priority_config(grid, CV_THREADS, smem, s, &prio);
+  return cudaLaunchKernelEx(&cfg, conv3x3_wgrad_kernel<NT, STAGES>, tmX, tmG, p);
 }
 
 // p.a = input planes [3][nsrc][N][H][W][Ca], p.b = dY planes [3][N][H][W][Cb], p.out = workspace
@@ -729,8 +749,50 @@ cudaError_t launch_conv_wgrad(const ConvTcParams& p0, float* dw, int splits, cud
   cudaError_t e = wgrad_launch<CV_WGRAD_NT, CV_STAGES(CV_WGRAD_NT)>(tmX, tmG, p, grid, s);
   if (e != cudaSuccess || splits == 1) return e;
   const int rows = p.ntaps * p.Ca;
-  conv_wgrad_reduce_kernel<<<dim3((rows + 31) / 32, p.Cb / 32), 256, 0, s>>>(p.out, dw, rows, p.Cb, splits);
-  return cudaGetLastError();
+  cudaLaunchAttribute prio;
+  cudaLaunchConfig_t cfg = low_priority_config(dim3((rows + 31) / 32, p.Cb / 32), 256, 0, s, &prio);
+  return cudaLaunchKernelEx(&cfg, conv_wgrad_reduce_kernel, (const float*)p.out, dw, rows, p.Cb, splits);
+}
+
+// (kind, priority) of every kernel node of a captured graph; kind: 1 = weight gradient (or its reduce), 2 = forward /
+// data gradient (or its reduce), 0 = any other kernel.  For tests: the priorities must be in the graph, not only in
+// eager launches.
+cudaError_t conv_graph_kernel_priorities(cudaGraph_t g, std::vector<std::pair<int, int>>* out) {
+  size_t n = 0;
+  cudaError_t e = cudaGraphGetNodes(g, nullptr, &n);
+  if (e != cudaSuccess) return e;
+  std::vector<cudaGraphNode_t> nodes(n);
+  if (n && (e = cudaGraphGetNodes(g, nodes.data(), &n)) != cudaSuccess) return e;
+  const void* wgrad_fns[] = {(const void*)conv3x3_wgrad_kernel<CV_WGRAD_NT, CV_STAGES(CV_WGRAD_NT)>,
+                             (const void*)conv_wgrad_reduce_kernel};
+  const void* fprop_fns[] = {(const void*)conv3x3_fprop_kernel<128, CV_STAGES(128), true>,
+                             (const void*)conv3x3_fprop_kernel<128, CV_STAGES(128), false>,
+                             (const void*)conv3x3_fprop_kernel<64, CV_STAGES(64), true>,
+                             (const void*)conv3x3_fprop_kernel<64, CV_STAGES(64), false>,
+                             (const void*)conv_fprop_reduce_kernel};
+  auto is = [](const void* f, const void* const* fns, int k) {
+    for (int i = 0; i < k; ++i) {
+      cudaFunction_t h = nullptr;
+      if (f == fns[i] || (cudaGetFuncBySymbol(&h, fns[i]) == cudaSuccess && f == (const void*)h)) return true;
+    }
+    return false;
+  };
+  for (size_t i = 0; i < n; ++i) {
+    cudaGraphNodeType t;
+    if ((e = cudaGraphNodeGetType(nodes[i], &t)) != cudaSuccess) return e;
+    if (t != cudaGraphNodeTypeKernel) continue;
+    cudaLaunchAttributeValue v = {};
+    if ((e = cudaGraphKernelNodeGetAttribute(nodes[i], cudaLaunchAttributePriority, &v)) != cudaSuccess) return e;
+    // a kernel that another library launched through the driver API has no runtime entry: it is none of ours
+    cudaKernelNodeParams kp = {};
+    int kind = 0;
+    if (cudaGraphKernelNodeGetParams(nodes[i], &kp) == cudaSuccess)
+      kind = is(kp.func, wgrad_fns, 2) ? 1 : is(kp.func, fprop_fns, 5) ? 2 : 0;
+    else
+      cudaGetLastError();
+    out->emplace_back(kind, v.priority);
+  }
+  return cudaSuccess;
 }
 
 static unsigned split_blocks(size_t n8) {

@@ -118,6 +118,7 @@ class Trainer:
         self.own_launches_total = 0               # ... summed over every step executed so far (replays included)
         self._graph_warm = {}
         self._side = None
+        self._capture_stream = None
         self._graph_keepalive = []
         self.train_time_s = 0.0
         if cfg.resume:
@@ -215,7 +216,11 @@ class Trainer:
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
             before = self._own_counts()
-            with torch.cuda.graph(g):
+            # captured at a higher priority than the default streams': every kernel node of the step outranks the
+            # weight gradients, which conv_tc launches at the lowest priority on a side stream
+            if self._capture_stream is None:
+                self._capture_stream = torch.cuda.Stream(self.device, priority=-1)
+            with torch.cuda.graph(g, stream=self._capture_stream):
                 if whole:
                     sloss = self._fwd_bwd_launch(sx, sy)
                 else:

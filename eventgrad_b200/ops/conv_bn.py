@@ -17,6 +17,7 @@ Results are bitwise identical to the separate `conv_tc.conv2d` + `FusedBNAct` op
 from __future__ import annotations
 
 import os
+import weakref
 from typing import Optional
 
 import torch
@@ -46,7 +47,7 @@ class _ConvBNFn(torch.autograd.Function):
     def forward(ctx, x, weight, gamma, beta, running_mean, running_var, nbt, residual, kind, momentum, eps, relu,
                 emit_planes, skip_in, skip_out):
         N, Ci, H, W = x.shape
-        ctx.kind, ctx.geom = kind, (N, Ci, H, W, weight.shape[0])
+        ctx.kind, ctx.geom, ctx.weight = kind, (N, Ci, H, W, weight.shape[0]), weakref.ref(weight)
         z, xp, wtp = conv_tc.conv_forward(x, weight, kind, ctx.needs_input_grad[0])
         z = z.permute(0, 3, 1, 2)                                       # conv output, logical NCHW, channels_last
         yp = torch.empty(3, z.numel(), dtype=torch.bfloat16, device=z.device) if emit_planes else None
@@ -77,7 +78,7 @@ class _ConvBNFn(torch.autograd.Function):
         if ctx.skip_in is not None:
             addend, addmask = ctx.skip_in.take()
         dx, dw = conv_tc.conv_backward(xp, wtp, gp, ctx.geom, ctx.kind, ctx.needs_input_grad[0],
-                                       ctx.needs_input_grad[1], z.device, addend, addmask)
+                                       ctx.needs_input_grad[1], z.device, addend, addmask, ctx.weight())
         return dx, dw, dgamma, dbeta, None, None, None, dres, None, None, None, None, None, None, None
 
 

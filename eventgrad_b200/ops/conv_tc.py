@@ -19,6 +19,7 @@ Eligibility: CUDA, fp32, channels_last activations, no bias / dilation / groups,
 from __future__ import annotations
 
 import os
+import weakref
 
 import torch
 import torch.nn.functional as F
@@ -149,8 +150,8 @@ def wprep(w_oti: torch.Tensor, transposed: bool):
 
 
 KSPLIT = os.environ.get("EGB_CONV_KSPLIT", "1") != "0"
-# weight gradient on a side stream, concurrent with the data gradient of the same layer (two branches inside the step's
-# CUDA graph): both kernels leave SMs idle at small per-GPU batches
+# weight gradient on a side stream, concurrent with the data gradient of the same layer and, when the join can wait for
+# the end of the backward (_fork_wgrad.join), with the layers after it (branches inside the step's CUDA graph)
 PAR_BWD = os.environ.get("EGB_CONV_PAR_BWD", "1") != "0"
 _SIDE = {}
 
@@ -179,12 +180,48 @@ class _fork_wgrad:
             self.ctx.__exit__(*a)
         return False
 
-    def join(self, *tensors):
-        if self.on:
+    def join(self, dw, weight, *read):
+        """Order the wgrad's result `dw` before its readers.  When the only reader is the AccumulateGrad of a leaf
+        weight without a preset .grad (it steals dw as the new .grad, no kernel), the wait is deferred to the end of
+        the backward pass (`_join_at_end`), so the side stream keeps running under the following layers' work.
+        Otherwise (preset .grad: AccumulateGrad adds dw in place; hooks; a non-leaf weight; outside a backward pass)
+        the current stream waits here.  `read`: the tensors the wgrad reads, kept alive for the side stream (dw and
+        the split workspace were allocated on the side stream, which orders their reuse there)."""
+        if not self.on:
+            return
+        dw.record_stream(self.cur)
+        if _defer_ok(dw, weight):
+            for t in read:
+                t.record_stream(self.side)
+            _join_at_end(self.cur, self.side)
+        else:
             self.cur.wait_stream(self.side)
-            for t in tensors:
-                if t is not None:
-                    t.record_stream(self.cur)
+
+
+def _defer_ok(dw, w) -> bool:
+    return (w is not None and w.is_leaf and w.requires_grad and w.grad is None and not w._backward_hooks
+            and not getattr(w, "_post_accumulate_grad_hooks", None) and dw.stride() == w.stride()
+            and torch._C._current_graph_task_id() != -1)
+
+
+# backward pass (autograd graph task id) -> {(current stream, side stream)} still to be joined at its end
+_PENDING = {}
+
+
+def _join_at_end(cur, side) -> None:
+    """Make `cur` wait for `side` when the running backward pass ends: from a callback of the autograd engine, which
+    runs before backward() / autograd.grad() return, so every caller sees the gradients ordered on `cur` (and a
+    CUDA-graph capture records the wait, joining the side stream back into the capture)."""
+    task = torch._C._current_graph_task_id()
+    pend = _PENDING.get(task)
+    if pend is None:
+        pend = _PENDING[task] = set()
+
+        def _join():
+            for c, s in _PENDING.pop(task, ()):
+                c.wait_stream(s)
+        torch.autograd.Variable._execution_engine.queue_callback(_join)
+    pend.add((cur, side))
 
 
 def fprop(ap, wp, N, H, W, Ca, Cb, taps, nsrc=1, wtaps=9, out=None, OH=None, OW=None, os_=1, op=0, oq=0,
@@ -299,9 +336,10 @@ def conv_forward(x, weight, kind, need_dx):
     return y, xp, wtp
 
 
-def conv_backward(xp, wtp, gp, geom, kind, need_dx, need_dw, dev, addend=None, addmask=None):
+def conv_backward(xp, wtp, gp, geom, kind, need_dx, need_dw, dev, addend=None, addmask=None, weight=None):
     """Weight gradient (side stream) and data gradient of one convolution from the planes of dY -> (dx, dw).
-    addend / addmask (s1 / p1 only): the data gradient becomes dgrad + (mask bit ? addend : 0), in its epilogue."""
+    addend / addmask (s1 / p1 only): the data gradient becomes dgrad + (mask bit ? addend : 0), in its epilogue.
+    weight: the convolution's weight, which decides whether the wait for dw can be deferred (_fork_wgrad.join)."""
     N, Ci, H, W, Co = geom
     dx = dw = None
     if kind == "stem":
@@ -320,7 +358,7 @@ def conv_backward(xp, wtp, gp, geom, kind, need_dx, need_dw, dev, addend=None, a
             skip = {} if addend is None else {"addend": addend, "addmask": addmask}
             dx = fprop(gp, wtp, N, H, W, Co, Ci, dtaps, 1, T, **skip).permute(0, 3, 1, 2)
         if need_dw:
-            fork.join(dwr)
+            fork.join(dw, weight, xp, gp)
     else:
         assert addend is None, "the skip-connection gradient is folded into stride-1 data gradients only"
         Ho, Wo = H // 2, W // 2
@@ -340,7 +378,7 @@ def conv_backward(xp, wtp, gp, geom, kind, need_dx, need_dw, dev, addend=None, a
                 fprop(gp, wtp, N, Ho, Wo, Co, Ci, TAPS_1X1, 1, 1, out=dxn, OH=H, OW=W, os_=2, op=0, oq=0)
             dx = dxn.permute(0, 3, 1, 2)
         if need_dw:
-            fork.join(dwr)
+            fork.join(dw, weight, xp, gp)
     return dx, dw
 
 
@@ -348,7 +386,7 @@ class _ConvTcFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, kind):
         N, Ci, H, W = x.shape
-        ctx.kind, ctx.geom = kind, (N, Ci, H, W, weight.shape[0])
+        ctx.kind, ctx.geom, ctx.weight = kind, (N, Ci, H, W, weight.shape[0]), weakref.ref(weight)
         y, xp, wtp = conv_forward(x, weight, kind, ctx.needs_input_grad[0])
         ctx.save_for_backward(xp, wtp)
         return y.permute(0, 3, 1, 2)                                    # logical NCHW, channels_last memory
@@ -362,7 +400,7 @@ class _ConvTcFn(torch.autograd.Function):
         if gp is None:
             gp = split3(dy)
         dx, dw = conv_backward(xp, wtp, gp, ctx.geom, ctx.kind, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
-                               dy.device)
+                               dy.device, weight=ctx.weight())
         return dx, dw, None
 
 
