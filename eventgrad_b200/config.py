@@ -76,8 +76,10 @@ class TrainConfig:
     topology: str = "ring"           # gossip graph (parallel/topology.py): ring | exp (offsets 1,2,4,...) | "o1,o2,..."
                                      # | onepeer-exp (time-varying: one peer r + 2^((k-1) mod ceil(log2 R)) per step)
                                      # (circulant offsets, at most 4); decent/event only beyond the ring
-    compress: str = "none"           # none | int8: decent/event on the ring send the int8 code of theta - prev (one fp32
-                                     # scale per 256 elements) with error feedback instead of fp32 theta
+    compress: str = "none"           # none | int8 | sign: decent/event on the ring send the int8 (sign: 1-bit scaled sign)
+                                     # code of theta - prev (one fp32 scale per 256 elements) instead of fp32 theta
+    choco_gamma: float = 0.0         # int8/sign: 0 < gamma <= 1 mixes by CHOCO-SGD's consensus step on the public copies,
+                                     # theta += gamma * (W prev - prev), which keeps the ranks' average; 0 = off
     gradient_tracking: bool = False  # decent on the ring: also gossip y, which tracks the average gradient, and step
                                      # along y instead of the local gradient (DSGT / DIGing; fused single-slot step)
     local_steps: int = 1             # decent: gossip at every H-th step only (step k iff H divides k); the H - 1 steps
@@ -181,29 +183,36 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError(f"topology {self.topology!r} does not support file_write: the reference's log format "
                                  "has exactly one left and one right receive column")
-        if self.compress not in ("none", "int8"):
-            raise ValueError(f"compress must be none|int8, got {self.compress!r}")
-        if self.compress == "int8":
+        if self.compress not in ("none", "int8", "sign"):
+            raise ValueError(f"compress must be none|int8|sign, got {self.compress!r}")
+        g = self.choco_gamma
+        if isinstance(g, bool) or not isinstance(g, (int, float)) or not 0.0 <= g <= 1.0:   # NaN fails the range
+            raise ValueError(f"--choco-gamma must be a number in [0, 1] (0: off), got {g!r}; aggressive codecs want a "
+                             "small gamma (with --compress sign, 1 diverges on 2 ranks and 0.2 converges on 2 to 8)")
+        if g > 0.0 and self.compress == "none":
+            raise ValueError("--choco-gamma needs --compress int8 or sign: it mixes the compressed public copies")
+        if self.compress != "none":
             # the int8 step exists as the iter-sync fused ring step (csrc/gossip_q8.cu) and in the torch.distributed
             # backends.  Explicit offsets other than "1" are never the ring; exp and onepeer-exp are the ring at small
             # world sizes, so for_world() checks them once the world size is known
             s = str(self.topology).strip().lower()
             if not (self.ring_topology or s in ("exp", "onepeer-exp")):
-                raise ValueError(f"--compress int8 runs on the ring only, got topology {self.topology!r}")
+                raise ValueError(f"--compress {self.compress} runs on the ring only, got topology {self.topology!r}")
             if self.algo not in ("decent", "event"):
-                raise ValueError(f"--compress int8 needs algo decent or event, got {self.algo!r}"
+                raise ValueError(f"--compress {self.compress} needs algo decent or event, got {self.algo!r}"
                                  + (" (spevent is its own compressor)" if self.algo == "spevent" else ""))
             if self.sync_mode != "iter":
-                raise ValueError("--compress int8 needs --sync-mode iter: a delta applied to a torn or stale inbox is "
-                                 "not idempotent")
+                raise ValueError(f"--compress {self.compress} needs --sync-mode iter: a delta applied to a torn or "
+                                 "stale inbox is not idempotent")
             if self.backend == "refport":
-                raise ValueError("--compress int8 is not supported by --backend refport")
+                raise ValueError(f"--compress {self.compress} is not supported by --backend refport")
             for name in ("overlap_push", "double_buffer", "ce_push"):
                 if getattr(self, name):
-                    raise ValueError(f"--compress int8 does not support {name} (fused single-kernel step only)")
+                    raise ValueError(f"--compress {self.compress} does not support {name} (fused single-kernel step "
+                                     "only)")
             if self.file_write:
-                raise ValueError("--compress int8 does not support file_write: the reference's log format records "
-                                 "the received fp32 tensors")
+                raise ValueError(f"--compress {self.compress} does not support file_write: the reference's log "
+                                 "format records the received fp32 tensors")
         if self.gradient_tracking:
             # the tracking step exists as the iter-sync fused single-slot ring step (csrc/gossip_gt.cu), in the
             # torch.distributed backends and in the simulator; sum_r y_r = sum_r g_r holds only if every y a rank mixes
@@ -221,7 +230,7 @@ class TrainConfig:
                 if getattr(self, name):
                     raise ValueError(f"--gradient-tracking does not support {name} (fused single-slot step only)")
             if self.compress != "none":
-                raise ValueError("--gradient-tracking does not support --compress int8")
+                raise ValueError(f"--gradient-tracking does not support --compress {self.compress}")
             if self.file_write:
                 raise ValueError("--gradient-tracking does not support file_write: the reference's log format has no "
                                  "column for y")
@@ -240,7 +249,7 @@ class TrainConfig:
             if self.gradient_tracking:
                 raise ValueError(f"{h} does not support --gradient-tracking")
             if self.compress != "none":
-                raise ValueError(f"{h} does not support --compress int8")
+                raise ValueError(f"{h} does not support --compress {self.compress}")
             if self.backend == "refport":
                 raise ValueError(f"{h} is not supported by --backend refport")
             for name in ("overlap_push", "double_buffer", "ce_push"):
@@ -270,7 +279,7 @@ class TrainConfig:
                 if getattr(self, name):
                     raise ValueError(f"--exact-diffusion does not support {name} (fused single-slot step only)")
             if self.compress != "none":
-                raise ValueError("--exact-diffusion does not support --compress int8")
+                raise ValueError(f"--exact-diffusion does not support --compress {self.compress}")
             if self.gradient_tracking:
                 raise ValueError("--exact-diffusion does not support --gradient-tracking (both remove the same bias)")
             if self.local_steps > 1:
@@ -299,7 +308,7 @@ class TrainConfig:
             if self.exact_diffusion:
                 raise ValueError(f"{h} does not support --exact-diffusion")
             if self.compress != "none":
-                raise ValueError(f"{h} does not support --compress int8")
+                raise ValueError(f"{h} does not support --compress {self.compress}")
             if self.local_steps > 1:
                 raise ValueError(f"{h} does not support --local-steps {self.local_steps}")
             if self.backend == "refport":
@@ -322,7 +331,7 @@ class TrainConfig:
                 raise ValueError(f"{h} needs --sync-mode iter: an async mix of a torn or stale inbox would enter the "
                                  "momentum buffer")
             if self.compress != "none":
-                raise ValueError(f"{h} does not support --compress int8")
+                raise ValueError(f"{h} does not support --compress {self.compress}")
             if self.gradient_tracking:
                 raise ValueError(f"{h} does not support --gradient-tracking")
             if self.exact_diffusion:
@@ -368,7 +377,7 @@ class TrainConfig:
             if self.exact_diffusion:
                 raise ValueError(f"{h} does not support --exact-diffusion")
             if self.compress != "none":
-                raise ValueError(f"{h} does not support --compress int8")
+                raise ValueError(f"{h} does not support --compress {self.compress}")
             if self.quasi_global_momentum:
                 raise ValueError(f"{h} does not support --quasi-global-momentum: the sync overwrites theta_k before the "
                                  "step kernel reads it back")
@@ -414,8 +423,9 @@ class TrainConfig:
             ring = world == 1
         else:
             ring = parse_topology(self.topology, world) == (1,)
-        if not ring and self.compress == "int8":
-            raise ValueError(f"--compress int8 runs on the ring only; topology {self.topology!r} is not the ring for "
+        if not ring and self.compress != "none":
+            raise ValueError(f"--compress {self.compress} runs on the ring only; topology {self.topology!r} is not "
+                             "the ring for "
                              f"{world} ranks")
         return dataclasses.replace(self, topology="ring") if ring else self
 
@@ -516,9 +526,14 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
                    help="gossip graph: ring (default), exp (offsets 1,2,4,... up to R/2), explicit circulant offsets, or "
                         "onepeer-exp (time-varying: at step k push to r + 2^((k-1) mod ceil(log2 R)) only, "
                         "mix (theta + received) / 2)")
-    p.add_argument("--compress", default=None, choices=["none", "int8"],
+    p.add_argument("--compress", default=None, choices=["none", "int8", "sign"],
                    help="decent/event on the ring: send the int8 code of theta - (what the neighbours hold) with one "
-                        "fp32 scale per 256 elements, about a quarter of the fp32 bytes (default none)")
+                        "fp32 scale per 256 elements, about a quarter of the fp32 bytes, or its 1-bit scaled sign, "
+                        "about 1/28 (sign; pair it with --choco-gamma) (default none)")
+    p.add_argument("--choco-gamma", type=float, default=None, metavar="GAMMA",
+                   help="--compress int8/sign: mix by CHOCO-SGD's consensus step theta += GAMMA * (W prev - prev) on "
+                        "the public copies, which keeps the ranks' average; 0 < GAMMA <= 1, small for the sign codec "
+                        "(default 0: the error-feedback mix)")
     p.add_argument("--gradient-tracking", action="store_true", default=None,
                    help="decent on the ring: also gossip y, a running estimate of the average gradient, and step along "
                         "it (DSGT): removes the bias of constant-lr D-PSGD under heterogeneous data")

@@ -164,6 +164,16 @@ struct GraphSlots {
 // dequantized delta to `prev`, and its receivers add the same delta to their replica of it; the mix reads the
 // replicas: theta <- ((theta + rep_l) + rep_r) / 3.  The codec (parallel/trigger.py q8_encode) is
 // s = max|d| / 127, q = s == 0 ? 0 : clamp(rint(d / s), -127, 127), deq = q * s, all IEEE round-to-nearest.
+// codec = 1 (--compress sign) replaces it by a 1-bit scaled sign on the same (tile, warp) block of 256 elements
+// (parallel/trigger.py sign_encode): each lane sums its 8 values of |d| left to right, the warp adds a + shfl_xor(a, o)
+// for o = 16, 8, 4, 2, 1, s = a / 256 (true division); bit e of the lane's byte is d_e < 0 and deq_e = bit ? -s : s.
+// Lane j of block b writes byte 32 b + j (= base >> 3) of the code inbox and the scale goes where int8's does, so the
+// sign path uses 1/8 of the code section.
+// gamma > 0 (--choco-gamma, CHOCO-SGD) replaces the mix by the consensus step on the public copies, after this step's
+// push has updated prev and the receive side the replicas (parallel/trigger.py choco_mix_):
+//   t = ((prev + rep_l) + rep_r) / 3,  theta <- theta + gamma * (t - prev)
+// which keeps the sum of theta over the ranks whatever the codec.  gamma = 0: the mix above.  The push, the flags,
+// prev and the replica updates are the same for both mixes.
 struct Q8Slots {
   const int8_t* q_from_l;   // local [n_tiles * EG_TILE] codes last pushed by my LEFT neighbour
   const int8_t* q_from_r;
@@ -176,6 +186,8 @@ struct Q8Slots {
   float* prev;              // what my neighbours hold of my theta (dequantized public copy)
   float* rep_l;             // my copy of my LEFT neighbour's prev
   float* rep_r;
+  int codec;                // 0: int8, 1: scaled sign (appended last, so no existing offset moves)
+  float gamma;              // 0: the mix ((theta + rep_l) + rep_r) / 3; (0, 1]: the CHOCO consensus step
 };
 
 // Gradient tracking for decent on the ring (csrc/gossip_gt.cu, --gradient-tracking): a separate block passed to the
@@ -217,8 +229,8 @@ cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_
 int gossip_graph_max_grid(int device);
 cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g, int grid, cudaStream_t s);
 // int8-compressed ring step (csrc/gossip_q8.cu): the fused single-kernel step with the pushes, replicas and flags of
-// `q`; requires phase 0, sync, do_push and do_mix, no sparse block, and every pointer of `q` set.  The iter-sync flag of
-// (tile, warp) carries 2*step + fired (PROTOCOL.md 1.7)
+// `q`; requires phase 0, sync, do_push and do_mix, no sparse block, every pointer of `q` set, codec 0 or 1 and gamma 0
+// or in (0, 1].  The iter-sync flag of (tile, warp) carries 2*step + fired (PROTOCOL.md 1.7, 1.15)
 int gossip_q8_max_grid(int device);
 cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int grid, cudaStream_t s);
 // gradient-tracking ring step (csrc/gossip_gt.cu): the fused single-kernel decent step that also gossips y and steps

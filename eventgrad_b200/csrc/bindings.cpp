@@ -84,7 +84,7 @@ static const std::unordered_map<std::string, Setter<GraphSlots>> kGraph = {
 static const std::unordered_map<std::string, Setter<Q8Slots>> kQ8 = {
     PTRF(Q8Slots, q_from_l), PTRF(Q8Slots, q_from_r), PTRF(Q8Slots, s_from_l), PTRF(Q8Slots, s_from_r),
     PTRF(Q8Slots, q_to_l), PTRF(Q8Slots, q_to_r), PTRF(Q8Slots, s_to_l), PTRF(Q8Slots, s_to_r),
-    PTRF(Q8Slots, prev), PTRF(Q8Slots, rep_l), PTRF(Q8Slots, rep_r),
+    PTRF(Q8Slots, prev), PTRF(Q8Slots, rep_l), PTRF(Q8Slots, rep_r), NUMF(Q8Slots, codec), NUMF(Q8Slots, gamma),
 };
 
 static const std::unordered_map<std::string, Setter<TrackSlots>> kTrack = {

@@ -43,7 +43,9 @@
 // of its 256 elements as int8 codes plus one fp32 scale, stores them into the neighbours' code / scale inboxes of the
 // Q8Slots block, and adds the dequantized delta to `prev`.  The (tile, warp) flag carries 2*step + fired, so the
 // receiver learns from the flag whether to add the neighbour's delta to its replica before the mix
-// ((theta + rep_l) + rep_r) / 3.  Under the drift trigger GossipParams.sent is `prev`.
+// ((theta + rep_l) + rep_r) / 3.  Under the drift trigger GossipParams.sent is `prev`.  Template parameters pick the
+// codec (kSign: a 1-bit scaled sign per element, one byte per lane) and the mix (kChoco: CHOCO's
+// theta + gamma * (((prev + rep_l) + rep_r) / 3 - prev)); Q8Slots.codec / gamma select the instance.
 // csrc/gossip_gt.cu defines EG_GT and includes it a fifth time for gradient tracking (`gossip_step_kernel_gt`, decent
 // on the ring, iter-sync fused step only): next to theta_k, the same thread pushes y_{k-1} of its slice into the
 // neighbours' y inboxes of the TrackSlots block before the unchanged (tile, warp) flag, and the mix forms
@@ -326,8 +328,39 @@ __device__ __forceinline__ void ld_u32x2_cg(const void* p, uint32_t& lo, uint32_
 // One block = the 256 elements of this warp's slice of the tile (base >> 8 is its (tile, warp) index).  Encode
 // d = theta - prev with one scale per block, push the 8 codes of this lane to both neighbours (one 8-byte store each),
 // lane 0 pushes the scale, and prev += deq.  Bit for bit parallel/trigger.py q8_encode / q8_decode.
-__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
+// kSign: the 1-bit scaled-sign codec (sign_encode / sign_decode), one byte per lane and neighbour at base >> 3.  Only
+// this thread's first `nvalid` elements belong to the tensor: the padding after it decodes to 0 and stays 0 in prev.
+template <bool kSign = false>
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/,
+                                          int nvalid = EG_VEC) {
   F8 pv = ld_f8(p.q.prev + base);
+  if (kSign) {
+    F8 d;
+    float a = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      d.v[e] = __fsub_rn(th.v[e], pv.v[e]);
+      a = __fadd_rn(a, fabsf(d.v[e]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a = __fadd_rn(a, __shfl_xor_sync(0xffffffffu, a, o));
+    const float s = __fdiv_rn(a, 256.f);
+    uint32_t bits = 0u;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const bool neg = d.v[e] < 0.f;
+      bits |= (neg ? 1u : 0u) << e;
+      if (e < nvalid) pv.v[e] = __fadd_rn(pv.v[e], neg ? -s : s);
+    }
+    p.q.q_to_l[base >> 3] = (int8_t)bits;
+    p.q.q_to_r[base >> 3] = (int8_t)bits;
+    if ((threadIdx.x & 31) == 0) {
+      p.q.s_to_l[base >> 8] = s;
+      p.q.s_to_r[base >> 8] = s;
+    }
+    st_f8(p.q.prev + base, pv);
+    return;
+  }
   F8 d;
   float a = 0.f;
 #pragma unroll
@@ -358,11 +391,20 @@ __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, cons
   st_f8(p.q.prev + base, pv);
 }
 // Receive side of one neighbour: when it fired this block, add its dequantized delta to my replica of its prev (the
-// same fp32 add it applied to prev) and store the replica back; return theta + replica.
+// same fp32 add it applied to prev) and store the replica back; return theta + replica.  kSign: the sign codec's byte,
+// added to the first `nvalid` elements only (the rest is the tensor's padding).
+template <bool kSign = false>
 __device__ __forceinline__ F8 q8_recv_add(float* rep, const int8_t* qin, const float* sin, size_t base, F8 th,
-                                          bool fired) {
+                                          bool fired, int nvalid = EG_VEC) {
   F8 r = ld_f8(rep + base);
-  if (fired) {
+  if (fired && kSign) {
+    const uint32_t bits = (uint32_t)__ldcg(reinterpret_cast<const unsigned char*>(qin) + (base >> 3));
+    const float s = __ldcg(sin + (base >> 8));
+#pragma unroll
+    for (int e = 0; e < 8; ++e)
+      if (e < nvalid) r.v[e] = __fadd_rn(r.v[e], ((bits >> e) & 1u) ? -s : s);
+    st_f8(rep + base, r);
+  } else if (fired) {
     uint32_t lo, hi;
     ld_u32x2_cg(qin + base, lo, hi);
     const float s = __ldcg(sin + (base >> 8));
@@ -522,8 +564,9 @@ __device__ __forceinline__ void ed_push_stage(const StepParams& p, const TileInf
 #endif
 
 // mix + SGD + norm-on-write for one tile. `th` already holds theta_k for this thread's 8 floats.  `mix`: p.do_mix of
-// a gossip step, false on a local step of --local-steps (plain SGD); the q8 and tracking builds always mix
-template <bool kMom, bool kQG>
+// a gossip step, false on a local step of --local-steps (plain SGD); the q8 and tracking builds always mix.  kSign and
+// kChoco exist in the q8 build only: the codec of the received deltas and the CHOCO mix (Q8Slots in api.h)
+template <bool kMom, bool kQG, bool kSign = false, bool kChoco = false>
 __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileInfo& ti, size_t base, F8 th,
                                          int lane, int warp, int step, int slot, bool mix) {
 #ifdef EG_GRAPH
@@ -563,11 +606,32 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
   float ssl = 0.f, ssr = 0.f;
   F8 m;
   const F8 g = load_grad(p, ti, base, threadIdx.x);
-  if (kMom) m = ld_f8(p.mom + base);
-  th = q8_recv_add(p.q.rep_l, p.q.q_from_l, p.q.s_from_l, base, th, (slot & 1) != 0);
-  th = q8_recv_add(p.q.rep_r, p.q.q_from_r, p.q.s_from_r, base, th, (slot & 2) != 0);
+  if (kMom && !kChoco) m = ld_f8(p.mom + base);
+  if (kChoco) {
+    // CHOCO: t = ((prev + rep_l) + rep_r) / 3, theta <- theta + gamma * (t - prev).  prev (stored by this thread's push
+    // of this slice earlier in the step, or unchanged when it did not fire) is read twice, and theta (not passed by the
+    // caller) and the momentum only once the replicas are summed: staged like the int8 mix, this spills
+    const int nv = ti.valid - (int)threadIdx.x * EG_VEC;
+    F8 acc = ld_f8(p.q.prev + base);
+    acc = q8_recv_add<kSign>(p.q.rep_l, p.q.q_from_l, p.q.s_from_l, base, acc, (slot & 1) != 0, nv);
+    acc = q8_recv_add<kSign>(p.q.rep_r, p.q.q_from_r, p.q.s_from_r, base, acc, (slot & 2) != 0, nv);
+    {
+      const F8 pv = ld_f8(p.q.prev + base);
 #pragma unroll
-  for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(th.v[e], 3.0f);
+      for (int e = 0; e < 8; ++e) acc.v[e] = __fsub_rn(__fdiv_rn(acc.v[e], 3.0f), pv.v[e]);
+    }
+    th = ld_f8(p.theta + base);
+    const float gamma = p.q.gamma;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) th.v[e] = __fadd_rn(th.v[e], __fmul_rn(gamma, acc.v[e]));
+    if (kMom) m = ld_f8(p.mom + base);
+  } else {
+    const int nv = kSign ? ti.valid - (int)threadIdx.x * EG_VEC : EG_VEC;
+    th = q8_recv_add<kSign>(p.q.rep_l, p.q.q_from_l, p.q.s_from_l, base, th, (slot & 1) != 0, nv);
+    th = q8_recv_add<kSign>(p.q.rep_r, p.q.q_from_r, p.q.s_from_r, base, th, (slot & 2) != 0, nv);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(th.v[e], 3.0f);
+  }
 #elif defined(EG_GT)
   // staged so the gradient registers die before theta and its inboxes are loaded (the caller passes no theta): (1) g,
   // g_prev -> g - g_prev, g_prev <- g; y, yL, yR -> y_k, stored; (2) theta and its inboxes, mix; (3) sgd_elem on y_k
@@ -792,6 +856,8 @@ __device__ __forceinline__ void push_phase(const StepParams& p, int step) {
 
 #if EG_QG
 template <bool kMom, bool kQG>   // kQG: quasi-global momentum, an instance of its own (see DESIGN §4)
+#elif defined(EG_Q8)
+template <bool kMom, bool kSign, bool kChoco>   // kSign: the 1-bit sign codec; kChoco: the CHOCO mix (Q8Slots)
 #else
 template <bool kMom>
 #endif
@@ -916,6 +982,9 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
           const size_t base = (size_t)t * EG_TILE + (size_t)tid * EG_VEC;
 #ifdef EG_DBUF
           push_tile_slot(p, base, ld_f8(p.theta + base), step);
+#elif defined(EG_Q8)
+          push_tile<kSign>(p, base, ld_f8(p.theta + base), slot,
+                           kSign ? tile_info(p, s_ti, j, t).valid - tid * EG_VEC : EG_VEC);
 #elif defined(EG_ED)
           ed_push_stage<kMom>(p, tile_info(p, s_ti, j, t), base, step);
 #else
@@ -952,8 +1021,10 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
         // the fired bits lane 0 observed, to the whole warp
         const int sides = __shfl_sync(0xffffffffu, (int)((fl & 1u) | ((fr & 1u) << 1)), 0);
         const size_t base = (size_t)t2 * EG_TILE + (size_t)tid * EG_VEC;
-        mix_tile<kMom, kQG>(p, t2, tile_info(p, s_ti, j - D, t2), base, ld_f8(p.theta + base), lane, warp, step,
-                            sides, p.do_mix != 0);
+        // the CHOCO mix loads theta itself, after the replicas
+        mix_tile<kMom, kQG, kSign, kChoco>(p, t2, tile_info(p, s_ti, j - D, t2), base,
+                                           kChoco ? F8{} : ld_f8(p.theta + base), lane, warp, step, sides,
+                                           p.do_mix != 0);
 #else
         if (lane == 0) {
 #ifdef EG_GRAPH
@@ -1126,17 +1197,38 @@ cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g,
 }
 
 #elif defined(EG_Q8)   // only the step kernel + its launcher exist in this translation unit
-int gossip_q8_max_grid(int device) {
-  int sms = 0, a = 0, b = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_q8<true>, EG_THREADS, 0);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_q8<false>, EG_THREADS, 0);
+template <bool kMom, bool kSign, bool kChoco>
+static void q8_occupancy(int& a) {
+  int b = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_q8<kMom, kSign, kChoco>, EG_THREADS, 0);
   if (b < a) a = b;
+}
+
+int gossip_q8_max_grid(int device) {   // the minimum over all eight instances
+  int sms = 0, a = 1 << 30;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  q8_occupancy<true, false, false>(a);
+  q8_occupancy<false, false, false>(a);
+  q8_occupancy<true, true, false>(a);
+  q8_occupancy<false, true, false>(a);
+  q8_occupancy<true, false, true>(a);
+  q8_occupancy<false, false, true>(a);
+  q8_occupancy<true, true, true>(a);
+  q8_occupancy<false, true, true>(a);
   if (a < 1) a = 1;
   return sms * a;
 }
 
-// int8-compressed ring step (decent/event): iter-sync fused step only.
+template <bool kSign, bool kChoco>
+static void q8_launch(const Q8StepParams& k, bool mom, int grid, cudaStream_t s) {
+  if (mom)
+    gossip_step_kernel_q8<true, kSign, kChoco><<<grid, EG_THREADS, 0, s>>>(k);
+  else
+    gossip_step_kernel_q8<false, kSign, kChoco><<<grid, EG_THREADS, 0, s>>>(k);
+}
+
+// Compressed ring step (decent/event): iter-sync fused step only.  codec 0 int8 / 1 sign; gamma 0 (the EF mix) or in
+// (0, 1] (CHOCO)
 cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int grid, cudaStream_t s) {
   const bool ptrs = q.q_from_l && q.q_from_r && q.s_from_l && q.s_from_r && q.q_to_l && q.q_to_r && q.s_to_l &&
                     q.s_to_r && q.prev && q.rep_l && q.rep_r && p.flag_from_l && p.flag_from_r && p.flag_to_l &&
@@ -1144,14 +1236,17 @@ cudaError_t launch_gossip_step_q8(const GossipParams& p, const Q8Slots& q, int g
   if (p.phase != 0 || !p.sync || p.sparse != nullptr || !p.do_push || !p.do_mix || !ptrs || p.local_steps > 1 ||
       p.global_avg_period != 0 || p.quasi_global != 0)
     return cudaErrorInvalidValue;
+  if (q.codec != 0 && q.codec != 1) return cudaErrorInvalidValue;
+  if (!(q.gamma == 0.f || (q.gamma > 0.f && q.gamma <= 1.f))) return cudaErrorInvalidValue;   // NaN fails both
   Q8StepParams k;
   static_cast<GossipCore&>(k) = p;   // no global_avg_period, no quasi_global (refused above)
   k.q = q;
   eg_count_launch(EG_FAM_GOSSIP, 1);
-  if (p.mu != 0.f && p.mom != nullptr)
-    gossip_step_kernel_q8<true><<<grid, EG_THREADS, 0, s>>>(k);
+  const bool mom = p.mu != 0.f && p.mom != nullptr, sign = q.codec == 1, choco = q.gamma > 0.f;
+  if (sign)
+    choco ? q8_launch<true, true>(k, mom, grid, s) : q8_launch<true, false>(k, mom, grid, s);
   else
-    gossip_step_kernel_q8<false><<<grid, EG_THREADS, 0, s>>>(k);
+    choco ? q8_launch<false, true>(k, mom, grid, s) : q8_launch<false, false>(k, mom, grid, s);
   return cudaGetLastError();
 }
 

@@ -13,9 +13,9 @@ import torch
 
 from ..parallel.arena import TensorTable
 from ..parallel.topology import Graph
-from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, consensus_stats, drift_norms, mix2_, mix3_,
-                                mixk_, q8_decode, q8_encode, q8_msg_bytes, qg_sgd_, rank_mean, sgd_, slowmo_sync_,
-                                topk_select, trigger_step)
+from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, choco_mix_, codec_of, consensus_stats,
+                                drift_norms, mix2_, mix3_, mixk_, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
+                                trigger_step)
 from .lr_schedule import lr_at
 
 
@@ -27,7 +27,7 @@ class RingSimulator:
                  offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1,
                  exact_diffusion: bool = False, global_avg_period: int = 0, quasi_global: bool = False,
                  slowmo_period: int = 0, slowmo_beta: float = 0.5, slowmo_lr: float = 1.0,
-                 consensus_every: int = 0):
+                 consensus_every: int = 0, choco_gamma: float = 0.0):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -35,7 +35,11 @@ class RingSimulator:
         receivers hold (event: zero at start, theta_k of every fired tensor at its push; spevent: prev).
         `compress="int8"` (decent/event on the ring): a fired tensor sends the int8 code of theta - prev (q8_encode)
         instead of theta; sender and receivers add the same dequantized delta to prev and to their replica of it, the
-        mix reads the replicas, and under drift `sent` is prev.
+        mix reads the replicas, and under drift `sent` is prev.  `compress="sign"`: the same with the 1-bit scaled-sign
+        codec (sign_encode / sign_decode).
+        `choco_gamma=gamma` in (0, 1] (compress int8 or sign; CHOCO-SGD): the mix becomes choco_mix_, theta <- theta +
+        gamma * (((prev + rep_l) + rep_r) / 3 - prev) with prev and the replicas after this step's deltas; pushes, prev,
+        replicas, events and bytes are unchanged.  0: the mix above.
         `gradient_tracking=True` (decent on the ring, DSGT): every rank also keeps y (tracking the average gradient),
         the previous gradient g_prev and y inboxes, all zero at start; at step k it pushes theta_k and y_{k-1}, then
         y_k = mix3_(y, yL, yR) + (g_k - g_prev), g_prev <- g_k, and the SGD step reads y_k instead of g_k.  At R = 1 the
@@ -71,7 +75,14 @@ class RingSimulator:
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
-        self.q8 = compress == "int8"
+        self.q8 = compress in ("int8", "sign")
+        self.compress = compress
+        g = choco_gamma
+        if isinstance(g, bool) or not isinstance(g, (int, float)) or not 0.0 <= g <= 1.0:
+            raise ValueError(f"choco_gamma must be a number in [0, 1], got {g!r}")
+        if g and not self.q8:
+            raise ValueError("choco_gamma: compress int8 or sign only")
+        self.choco_gamma = float(g)
         self.graphs = [Graph.build(r, world, offsets) for r in range(world)]
         self.offsets = self.graphs[0].offsets
         self.n_slots = self.graphs[0].n_slots
@@ -80,7 +91,7 @@ class RingSimulator:
         if not self.graphs[0].is_ring and algo not in ("decent", "event"):
             raise ValueError(f"topology {offsets!r}: only decent and event gossip beyond the ring")
         if self.q8 and (algo not in ("decent", "event") or not self.graphs[0].is_ring):
-            raise ValueError("compress int8: decent or event on the ring only")
+            raise ValueError(f"compress {compress}: decent or event on the ring only")
         if gradient_tracking and (algo != "decent" or not self.graphs[0].is_ring or self.q8):
             raise ValueError("gradient tracking: decent on the ring, without compression, only")
         self.gt = bool(gradient_tracking) and world > 1
@@ -293,12 +304,13 @@ class RingSimulator:
                     self._flat(self.rep_l[Rn], i)[ix] = v    # and my right neighbour's left
                     self.bytes[r] += 2 * 2 * self.k[i] * 4
                 elif self.q8:
+                    enc, dec, msg = codec_of(self.compress)
                     pv = self._padded(self.prev[r], i)
-                    deq = q8_decode(*q8_encode(self._padded(snap[r], i) - pv))
+                    deq = dec(*enc(self._padded(snap[r], i) - pv), t.numels[i])
                     pv.add_(deq)
                     self._padded(self.rep_r[L], i).add_(deq)    # I am my left neighbour's right
                     self._padded(self.rep_l[Rn], i).add_(deq)   # and my right neighbour's left
-                    self.bytes[r] += 2 * q8_msg_bytes(t.numels[i])
+                    self.bytes[r] += 2 * msg(t.numels[i])
                 else:
                     outs = self.graphs[r].out_slots()
                     if self.period:                            # one-peer graph: only this round's out-slot
@@ -316,7 +328,9 @@ class RingSimulator:
                 self.bytes[r] += 2 * t.n_elems * 4
         # ---- phase 2: mix with whatever the inboxes hold, then SGD -----------------------
         for r in range(R):
-            if self.algo == "spevent" or self.q8:
+            if self.choco_gamma:
+                choco_mix_(self.theta[r], self.prev[r], self.rep_l[r], self.rep_r[r], self.choco_gamma)
+            elif self.algo == "spevent" or self.q8:
                 mix3_(self.theta[r], self.rep_l[r], self.rep_r[r])
             elif self.period:
                 mix2_(self.theta[r], self.inbox[r][self.graphs[r].active(rnd)])

@@ -67,6 +67,18 @@ def check_compress_state(sd: Dict, compress: str, algo: str) -> None:
                          "resume with the same --compress")
 
 
+def check_choco_state(sd: Dict, gamma: float, algo: str) -> None:
+    """Refuse to resume decent / event state saved under another --choco-gamma: the public copies and replicas were
+    built by a different mix, and the run would silently change its fixed point.  Checkpoints without a `choco_gamma`
+    key were written with the feature off (0)."""
+    if algo not in ("decent", "event"):
+        return
+    saved = float(sd.get("choco_gamma", 0.0))
+    if saved != float(gamma):
+        raise ValueError(f"checkpoint was written with --choco-gamma {saved:g}, this run uses --choco-gamma "
+                         f"{float(gamma):g}; resume with the same --choco-gamma")
+
+
 def check_tracking_state(sd: Dict, tracking: bool, algo: str) -> None:
     """Refuse to resume decent state saved under the other --gradient-tracking setting: tracking state is y, the
     previous gradient and the y inboxes, which a plain run neither saves nor restores.  Checkpoints without a

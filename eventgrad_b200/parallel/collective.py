@@ -11,7 +11,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
   spevent fired tensors travel as (top-k values, indices) records; receiver scatters into
           persistent neighbour replicas      (/root/reference/dcifar10/spevent/spevent.cpp:342-542)
   --compress int8 (decent / event, ring): fired tensors travel as int8 codes of theta - prev plus block scales;
-          both ends add the dequantized delta to prev / their replica of it, and the mix reads the replicas
+          both ends add the dequantized delta to prev / their replica of it, and the mix reads the replicas;
+          --compress sign sends 1-bit scaled signs packed 8 to a byte, and --choco-gamma mixes by choco_mix_
   --gradient-tracking (decent, ring): theta and y travel in one batched exchange; y_k = (y + yL + yR)/3 + g_k - g_prev,
           and SGD steps along y_k
   --local-steps H (decent): only every H-th step runs the exchange and mix; the others are the SGD update alone
@@ -38,10 +39,10 @@ import torch
 import torch.distributed as dist
 
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
-                   check_local_steps_state, check_qg_state, check_slowmo_state, check_topology_state,
+                   check_choco_state, check_local_steps_state, check_qg_state, check_slowmo_state, check_topology_state,
                    check_tracking_state, check_trigger_state, slowmo_state)
-from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, consensus_stats, drift_norms, mix2_, mix3_, mixk_,
-                      q8_decode, q8_encode, q8_msg_bytes, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
+from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, choco_mix_, codec_of, consensus_stats, drift_norms, mix2_,
+                      mix3_, mixk_, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
                       trigger_step)
 
 
@@ -63,7 +64,9 @@ class CollectiveBackend(CommBackend):
         # --compress int8 (decent/event, ring): fired tensors travel as int8 codes of theta - prev plus one scale per
         # block; prev and the neighbour replicas start from theta_0 (identical on all ranks), the mix reads the replicas
         self.compress = getattr(cfg, "compress", "none")
-        self.q8 = gossip and self.compress == "int8"
+        self.q8 = gossip and self.compress in ("int8", "sign")
+        # --choco-gamma (int8 / sign): the CHOCO consensus step on the public copies replaces the mix of the replicas
+        self.choco_gamma = float(getattr(cfg, "choco_gamma", 0.0)) if self.q8 else 0.0
         if self.q8:
             self.prev = arena.theta.clone()
             self.rep_l = arena.theta.clone()
@@ -367,27 +370,31 @@ class CollectiveBackend(CommBackend):
         return buf[t.offsets[i]: t.offsets[i] + t.tile_count[i] * t.tile]
 
     def _step_q8(self, mine, masks) -> None:
-        """int8 ring step: my fired tensors' codes of theta - prev and their block scales go to both neighbours (decent:
-        every tensor; event: after the fire-mask exchange, `masks` = (left's, right's)); each side adds the dequantized
-        delta to prev / to its replica of the sender's prev, then theta <- ((theta + rep_l) + rep_r) / 3 and SGD."""
+        """Compressed ring step: my fired tensors' codes of theta - prev (int8: one byte per element; sign: one bit,
+        packed 8 to a byte) and their block scales go to both neighbours (decent: every tensor; event: after the
+        fire-mask exchange, `masks` = (left's, right's)); each side adds the dequantized delta to prev / to its replica of
+        the sender's prev, then theta <- ((theta + rep_l) + rep_r) / 3 (--choco-gamma: choco_mix_) and SGD."""
         a, t = self.arena, self.arena.table
+        enc, dec, msg = codec_of(self.compress)
+        per = 8 if self.compress == "sign" else 1          # arena elements per code byte
+        cdt = torch.uint8 if self.compress == "sign" else torch.int8
         lm, rm = masks if masks is not None else (mine, mine)
         qs, ss = [], []
         for i in range(t.n_tensors):
             if mine[i]:
                 pv = self._padded(self.prev, i)
-                q, s = q8_encode(self._padded(a.theta, i) - pv)
-                pv.add_(q8_decode(q, s))
+                q, s = enc(self._padded(a.theta, i) - pv)
+                pv.add_(dec(q, s, t.numels[i]))
                 qs.append(q)
                 ss.append(s)
-                self.bytes += 2 * q8_msg_bytes(t.numels[i])
-        pq = torch.cat(qs) if qs else torch.empty(0, dtype=torch.int8, device=a.theta.device)
+                self.bytes += 2 * msg(t.numels[i])
+        pq = torch.cat(qs) if qs else torch.empty(0, dtype=cdt, device=a.theta.device)
         ps = torch.cat(ss) if ss else a.theta.new_empty(0)
         blocks = [t.tile_count[i] * t.tile for i in range(t.n_tensors)]
         nl = sum(blocks[i] for i in range(t.n_tensors) if lm[i])
         nr = sum(blocks[i] for i in range(t.n_tensors) if rm[i])
-        ql, qr = torch.empty(nl, dtype=torch.int8, device=a.theta.device), torch.empty(nr, dtype=torch.int8,
-                                                                                       device=a.theta.device)
+        ql = torch.empty(nl // per, dtype=cdt, device=a.theta.device)
+        qr = torch.empty(nr // per, dtype=cdt, device=a.theta.device)
         sl, sr = a.theta.new_empty(nl // Q8_BLOCK), a.theta.new_empty(nr // Q8_BLOCK)
         self._exchange([pq, ps], [pq, ps], [ql, sl], [qr, sr])
         for mask, qb, sb, rep in ((lm, ql, sl, self.rep_l), (rm, qr, sr, self.rep_r)):
@@ -395,9 +402,13 @@ class CollectiveBackend(CommBackend):
             for i in range(t.n_tensors):
                 if mask[i]:
                     n = blocks[i]
-                    self._padded(rep, i).add_(q8_decode(qb[off:off + n], sb[off // Q8_BLOCK:(off + n) // Q8_BLOCK]))
+                    self._padded(rep, i).add_(dec(qb[off // per:(off + n) // per],
+                                                  sb[off // Q8_BLOCK:(off + n) // Q8_BLOCK], t.numels[i]))
                     off += n
-        mix3_(a.theta, self.rep_l, self.rep_r)
+        if self.choco_gamma:
+            choco_mix_(a.theta, self.prev, self.rep_l, self.rep_r, self.choco_gamma)
+        else:
+            mix3_(a.theta, self.rep_l, self.rep_r)
         self._opt()
 
     def _step_event(self) -> None:
@@ -544,7 +555,9 @@ class CollectiveBackend(CommBackend):
         if self.qg:
             sd["quasi_global_momentum"] = True      # the arena's momentum holds m_hat
         if self.cfg.algo in ("decent", "event"):
-            sd["compress"] = self.compress          # int8: prev / rep_l / rep_r are saved above
+            sd["compress"] = self.compress          # int8 / sign: prev / rep_l / rep_r are saved above
+            if self.choco_gamma:
+                sd["choco_gamma"] = self.choco_gamma
         if self.cfg.algo in ("event", "spevent"):
             sd["trigger"] = self.tcfg.metric
             if self.drift and self.cfg.algo == "event" and not self.q8:
@@ -564,6 +577,7 @@ class CollectiveBackend(CommBackend):
         check_topology_state(sd, self.ring, self.cfg.algo)
         check_trigger_state(sd, self.tcfg.metric, self.cfg.algo)
         check_compress_state(sd, self.compress, self.cfg.algo)
+        check_choco_state(sd, self.choco_gamma, self.cfg.algo)
         check_tracking_state(sd, self.gt, self.cfg.algo)
         check_local_steps_state(sd, self.local_steps, self.cfg.algo)
         check_global_avg_state(sd, self.global_avg_period, self.cfg.algo)

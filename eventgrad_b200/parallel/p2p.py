@@ -9,7 +9,8 @@ Per training step, after backward():
   event    ONE launch: as decent, but a tensor is pushed only if its device-resident trigger fired;
            the same kernel accumulates the norms and runs the trigger FSM for the next step
            (--compress int8, ring: csrc/gossip_q8.cu pushes the int8 code of theta - prev + block scales, the receivers
-           add the delta to their replicas of prev, and the mix reads the replicas)
+           add the delta to their replicas of prev, and the mix reads the replicas; --compress sign sends a 1-bit scaled
+           sign instead, and --choco-gamma mixes by CHOCO's theta += gamma * (((prev + rep_l) + rep_r) / 3 - prev))
            (--gradient-tracking, decent on the ring: csrc/gossip_gt.cu also pushes y_{k-1} before the same flag, forms
            y_k = (y + yL + yR)/3 + g_k - g_prev and steps along y_k)
            (--exact-diffusion, decent on the ring: csrc/gossip_ed.cu runs SGD in the push stage, pushes
@@ -37,10 +38,10 @@ import torch
 
 from .arena import TILE, ParamArena, TensorTable
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
-                   check_local_steps_state, check_slowmo_state, slowmo_state, check_qg_state, check_topology_state, check_tracking_state,
+                   check_choco_state, check_local_steps_state, check_slowmo_state, slowmo_state, check_qg_state, check_topology_state, check_tracking_state,
                    check_trigger_state)
 from .topology import Graph
-from .trigger import q8_msg_bytes
+from .trigger import codec_of
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
 
 ONE_SHOT_MAX_BYTES = 512 * 1024        # above this the all-reduce switches to two-shot
@@ -70,8 +71,8 @@ def _wants_dbuf(cfg) -> bool:
 
 
 def _wants_q8(cfg) -> bool:
-    """--compress int8: decent/event on the ring run the int8 step of csrc/gossip_q8.cu."""
-    return getattr(cfg, "compress", "none") == "int8" and cfg.algo in ("decent", "event")
+    """--compress int8 / sign: decent/event on the ring run the compressed step of csrc/gossip_q8.cu."""
+    return getattr(cfg, "compress", "none") in ("int8", "sign") and cfg.algo in ("decent", "event")
 
 
 def _wants_gt(cfg, world: int) -> bool:
@@ -222,11 +223,14 @@ class P2PBackend(CommBackend):
         # split step: everything that depends only on theta_k (pushes / top-k records) is launched on a
         # side stream at the start of the step and overlaps forward+backward
         self.overlap = bool(getattr(cfg, "overlap_push", False)) and self.do_comm
-        # --compress int8: the iter-sync fused ring step of csrc/gossip_q8.cu
+        # --compress int8 / sign: the iter-sync fused ring step of csrc/gossip_q8.cu; --choco-gamma selects its CHOCO mix
         self.q8 = _wants_q8(cfg)
+        self.compress = cfg.compress if self.q8 else "none"
+        self.choco_gamma = float(getattr(cfg, "choco_gamma", 0.0)) if self.q8 else 0.0
         if self.q8 and (self.graph is not None or self.overlap or getattr(cfg, "ce_push", False) or self.want_logs
                         or not self.sync):
-            raise ValueError("p2p backend: --compress int8 runs decent/event on the ring's fused iter-sync step only")
+            raise ValueError(f"p2p backend: --compress {self.compress} runs decent/event on the ring's fused iter-sync "
+                             "step only")
         # --gradient-tracking: the iter-sync fused single-slot ring step of csrc/gossip_gt.cu
         self.gt = _wants_gt(cfg, ring.world) and self.do_comm
         if self.gt and (self.graph is not None or self.overlap or getattr(cfg, "ce_push", False) or self.want_logs
@@ -305,7 +309,7 @@ class P2PBackend(CommBackend):
             self.K = sum(self.k)
             self.d_k, self.d_rec_off = i32(self.k), i32(rec_off)
         elif self.q8:
-            msg = [q8_msg_bytes(n) for n in t.numels]     # int8 codes of the real elements + the blocks' scales
+            msg = [codec_of(self.compress)[2](n) for n in t.numels]   # codes of the real elements + the blocks' scales
         else:
             msg = [n * 4 for n in t.numels]
         self.msg_bytes = msg
@@ -484,6 +488,7 @@ class P2PBackend(CommBackend):
                     "q_to_l": win.addr("q_from_r", L), "q_to_r": win.addr("q_from_l", R),
                     "s_to_l": win.addr("qs_from_r", L), "s_to_r": win.addr("qs_from_l", R),
                     "prev": P(self.prev), "rep_l": P(self.rep_l), "rep_r": P(self.rep_r),
+                    "codec": 1 if self.compress == "sign" else 0, "gamma": self.choco_gamma,
                 })
                 self.qs = qs
             elif dense and self.graph is None:
@@ -921,7 +926,9 @@ class P2PBackend(CommBackend):
             sd["inbox_l"] = self.win.view("inbox_l", torch.float32).cpu().clone()
             sd["inbox_r"] = self.win.view("inbox_r", torch.float32).cpu().clone()
         if self.cfg.algo in ("decent", "event"):
-            sd["compress"] = "int8" if self.q8 else "none"
+            sd["compress"] = self.compress
+            if self.choco_gamma:
+                sd["choco_gamma"] = self.choco_gamma
         if self.cfg.algo == "decent":
             sd["gradient_tracking"] = self.gt
             sd["local_steps"] = self.local_steps
@@ -947,7 +954,8 @@ class P2PBackend(CommBackend):
     def load_state_dict(self, sd):
         check_topology_state(sd, self.ring, self.cfg.algo)
         check_trigger_state(sd, self.metric, self.cfg.algo)
-        check_compress_state(sd, "int8" if self.q8 else "none", self.cfg.algo)
+        check_compress_state(sd, self.compress, self.cfg.algo)
+        check_choco_state(sd, self.choco_gamma, self.cfg.algo)
         check_tracking_state(sd, self.gt, self.cfg.algo)
         check_local_steps_state(sd, self.local_steps, self.cfg.algo)
         check_exact_diffusion_state(sd, self.ed, self.cfg.algo)

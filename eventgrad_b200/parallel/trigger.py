@@ -228,7 +228,7 @@ def consensus_values(D, A, world: int):
 
 
 Q8_BLOCK = 256          # elements per int8 scale: one warp's slice of a 2048-float tile (never straddles tensors)
-COMPRESS = ("none", "int8")
+COMPRESS = ("none", "int8", "sign")
 
 
 def q8_msg_bytes(numel: int) -> int:
@@ -257,6 +257,77 @@ def q8_encode(d: torch.Tensor):
 def q8_decode(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
     """deq = (float)q * s per block (one rounded multiply): the delta both ends add to prev / their replica."""
     return (q.reshape(-1, Q8_BLOCK).to(torch.float32) * s.reshape(-1, 1)).reshape(-1)
+
+
+SIGN_LANES = 32         # a block is one warp: lane j holds elements 8j .. 8j + 7 and sends byte j of the block
+
+
+def sign_msg_bytes(numel: int) -> int:
+    """Logical bytes of one tensor's sign message: one bit per real element (rounded up to bytes) + one fp32 scale per
+    block holding any."""
+    return -(-numel // 8) + 4 * (-(-numel // Q8_BLOCK))
+
+
+@torch.no_grad()
+def sign_encode(d: torch.Tensor):
+    """1-bit scaled-sign code of a padded flat arena d (length a multiple of Q8_BLOCK), one scale per block, bit for bit
+    the sign path of the q8 step kernel (csrc/gossip.cu, EG_Q8):
+        each lane sums its 8 values of |d| left to right; the warp adds a + shfl_xor(a, o) for o = 16, 8, 4, 2, 1 (every
+        stage is commutative, so all lanes end with the same value); s = a / 256, a true division;
+        bit e of lane j's byte is d_{8j+e} < 0 (+0, -0 and NaN give 0)
+    Returns (bytes uint8 [n / 8], s [n / Q8_BLOCK]) in d's dtype (float32 on the wire; float64 for convergence
+    studies).  Byte 32 b + j is lane j of block b."""
+    b = d.reshape(-1, SIGN_LANES, 8)
+    ab = b.abs()
+    a = ab[:, :, 0].clone()
+    for e in range(1, 8):
+        a = a + ab[:, :, e]
+    lane = torch.arange(SIGN_LANES, device=d.device)
+    o = SIGN_LANES // 2
+    while o:
+        a = a + a[:, lane ^ o]
+        o //= 2
+    s = a[:, 0] / torch.full_like(a[:, 0], float(Q8_BLOCK))
+    weights = torch.tensor([1 << e for e in range(8)], dtype=torch.int32, device=d.device)
+    bits = ((b < 0).to(torch.int32) * weights).sum(dim=2).to(torch.uint8)
+    return bits.reshape(-1), s
+
+
+@torch.no_grad()
+def sign_decode(bits: torch.Tensor, s: torch.Tensor, numel=None) -> torch.Tensor:
+    """deq_e = bit_e ? -s : s per block, in s's dtype: the delta both ends add to prev / their replica (one rounded
+    add each).  `numel`: the decoded span is one tensor's whole tiles, and the elements from `numel` on are its zero
+    padding, which decodes to 0 (as in the kernel, which adds nothing there), so padding stays 0."""
+    shifts = torch.arange(8, dtype=torch.int32, device=bits.device)
+    neg = ((bits.to(torch.int32).reshape(-1, 1) >> shifts) & 1).bool().reshape(-1, Q8_BLOCK)
+    sb = s.reshape(-1, 1).expand(-1, Q8_BLOCK)
+    deq = torch.where(neg, -sb, sb).reshape(-1)
+    if numel is not None:
+        deq[numel:] = 0
+    return deq
+
+
+def codec_of(compress: str):
+    """(encode(d), decode(code, scales, numel), msg_bytes(numel)) of a --compress codec other than none; decode takes the
+    tensor's real element count (int8's padding codes are 0 already)."""
+    if compress == "int8":
+        return q8_encode, lambda q, s, numel=None: q8_decode(q, s), q8_msg_bytes
+    if compress == "sign":
+        return sign_encode, sign_decode, sign_msg_bytes
+    raise ValueError(f"no codec for compress {compress!r}")
+
+
+@torch.no_grad()
+def choco_mix_(theta: torch.Tensor, prev: torch.Tensor, rep_l: torch.Tensor, rep_r: torch.Tensor,
+               gamma: float) -> torch.Tensor:
+    """CHOCO-SGD's consensus step (Koloskova, Stich and Jaggi 2019) on the ring, op for op as the q8 step kernel's
+    CHOCO mix: t = ((prev + rep_l) + rep_r) / 3 ; theta <- theta + gamma * (t - prev).  `prev` is this rank's public
+    copy after this step's push, rep_l / rep_r its replicas of the neighbours' after their deltas arrived.  gamma is
+    rounded to theta's dtype once and the division takes a tensor divisor, so every operation is one IEEE rounding.
+    Summed over the ranks, t - prev vanishes in exact arithmetic, so the average of theta is kept whatever the codec."""
+    g = torch.tensor(gamma, dtype=theta.dtype, device=theta.device)
+    t = prev.add(rep_l).add_(rep_r).div_(torch.tensor(3.0, dtype=theta.dtype, device=theta.device))
+    return theta.add_(t.sub_(prev).mul_(g))
 
 
 @torch.no_grad()

@@ -5,8 +5,9 @@ One file per rank: arena (theta + momentum, with its layout), the backend's comm
 inboxes / sparse replicas, event counters, pass_num; on a gossip graph every slot's inbox, the offsets and, for
 onepeer-exp, the topology name, checked on resume by parallel/base.py; event/spevent: the trigger name, and under
 --trigger drift event's `sent` buffer, also checked on resume; decent/event: the `compress` setting, and under
---compress int8 `prev` and the neighbour replicas `rep_l` / `rep_r` instead of the inboxes, checked on resume by
-check_compress_state; decent: the `gradient_tracking` setting, and under --gradient-tracking y, the previous gradient
+--compress int8 / sign `prev` and the neighbour replicas `rep_l` / `rep_r` instead of the inboxes, checked on resume by
+check_compress_state, and `choco_gamma` when --choco-gamma is on (check_choco_state); decent: the
+`gradient_tracking` setting, and under --gradient-tracking y, the previous gradient
 `g_prev` and the y inboxes `y_in_l` / `y_in_r`, checked on resume by check_tracking_state; decent: the `local_steps`
 period, checked on resume by check_local_steps_state; decent: the `exact_diffusion` setting, and under
 --exact-diffusion `psi`, checked on resume by check_exact_diffusion_state; decent with --global-avg-period P > 0: the
