@@ -105,6 +105,20 @@ KINDS = [  # kind, N, H, W, Cin, Cout, k, stride, pad
     ("p2", 2, 8, 8, 8, 16, 1, 2, 0),
     ("p1", 2, 4, 4, 8, 16, 1, 1, 0),
     ("stem", 2, 8, 8, 3, 16, 3, 1, 1),
+    # grids off the square power-of-two ones (see test_conv_tc_geometry.py): 1x1 images, strips, columns, 3 tiles
+    # per image, stride-2 convs on 2x2 / 4x4 / 24x64 inputs
+    ("s1", 3, 1, 1, 8, 16, 3, 1, 1),
+    ("s1", 2, 1, 64, 8, 16, 3, 1, 1),
+    ("s1", 2, 128, 1, 8, 8, 3, 1, 1),
+    ("s1", 2, 12, 32, 8, 16, 3, 1, 1),
+    ("s2", 5, 2, 2, 8, 16, 3, 2, 1),
+    ("s2", 2, 4, 4, 8, 16, 3, 2, 1),
+    ("s2", 3, 24, 64, 8, 16, 3, 2, 1),
+    ("p2", 7, 2, 2, 8, 16, 1, 2, 0),
+    ("p2", 2, 24, 64, 8, 8, 1, 2, 0),
+    ("p1", 3, 6, 64, 8, 16, 1, 1, 0),
+    ("stem", 3, 1, 1, 3, 16, 3, 1, 1),
+    ("stem", 2, 24, 16, 3, 16, 3, 1, 1),
 ]
 
 
