@@ -97,6 +97,8 @@ class TrainConfig:
     slowmo_lr: float = 1.0           # SlowMo slow learning rate, alpha > 0
     consensus_every: int = 0         # gossip algorithms: every N-th step measure the consensus distance
                                      # sqrt(sum_r ||theta_r - theta_bar||^2 / R) per tensor (read-only); 0 = off
+    gossip_rounds: int = 1           # decent on the ring / a static graph: Q >= 2 runs Q - 1 mix-only gossip rounds
+                                     # before the step's own mix, theta_{k+1} = SGD(W^Q theta_k); Q times the bytes
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -401,6 +403,45 @@ class TrainConfig:
                                  "promises no cross-rank waits in the step loop")
             if self.backend == "refport":
                 raise ValueError(f"{h} is not supported by --backend refport")
+        Q = self.gossip_rounds
+        if isinstance(Q, bool) or not isinstance(Q, int) or Q < 1:
+            raise ValueError(f"--gossip-rounds must be an integer >= 1, got {Q!r}")
+        if Q > 1:
+            # the mix-only rounds exist for decent in front of the fused single-kernel ring, double-buffered ring and
+            # static-graph steps (csrc/gossip_rounds.cu), the torch.distributed backends and the simulator
+            h = f"--gossip-rounds {Q}"
+            if self.algo != "decent":
+                raise ValueError(f"{h} needs algo decent, got {self.algo!r}"
+                                 + ("" if self.algo == "cent" else ": the trigger decides what a step sends, and a "
+                                    "mix-only round would send every tensor"))
+            if str(self.topology).strip().lower() == "onepeer-exp":
+                raise ValueError(f"{h} does not support topology onepeer-exp: its single active slot per step has no "
+                                 "rule for extra rounds")
+            if self.compress != "none":
+                raise ValueError(f"{h} does not support --compress {self.compress}: a mix-only round would have to "
+                                 "encode and replicate its own deltas")
+            if self.gradient_tracking:
+                raise ValueError(f"{h} does not support --gradient-tracking: y would need rounds of its own")
+            if self.exact_diffusion:
+                raise ValueError(f"{h} does not support --exact-diffusion: its step gossips phi, not theta")
+            if self.local_steps > 1:
+                raise ValueError(f"{h} does not support --local-steps {self.local_steps}")
+            if self.global_avg_period:
+                raise ValueError(f"{h} does not support --global-avg-period: an averaging step has no mix to repeat")
+            if self.slowmo_period:
+                raise ValueError(f"{h} does not support --slowmo-period: a sync step has no mix to repeat")
+            if self.quasi_global_momentum:
+                raise ValueError(f"{h} does not support --quasi-global-momentum: its theta_k is overwritten by the "
+                                 "rounds before the step kernel reads it")
+            if self.backend == "refport":
+                raise ValueError(f"{h} is not supported by --backend refport")
+            for name in ("overlap_push", "ce_push"):
+                if getattr(self, name):
+                    raise ValueError(f"{h} does not support {name}: the rounds overwrite theta, which the forward "
+                                     "reads, so they cannot run under backward")
+            if self.file_write:
+                raise ValueError(f"{h} does not support file_write: the reference's log format records one exchange "
+                                 "per step")
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
@@ -453,7 +494,7 @@ class TrainConfig:
                                       and not bool(c.double_buffer) and c.ring_topology and c.compress == "none"
                                       and not c.gradient_tracking and c.local_steps == 1
                                       and not c.exact_diffusion and not c.global_avg_period
-                                      and not c.slowmo_period)
+                                      and not c.slowmo_period and c.gossip_rounds == 1)
         return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
@@ -564,6 +605,10 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
                    help="decent/event/spevent: after every N-th step measure how far the ranks' parameters are from "
                         "their average, per tensor, without changing training; rank 0 prints the relative distance "
                         "per epoch and --log-dir gets consensus.csv and consensus_tensors.csv (default 0: off)")
+    p.add_argument("--gossip-rounds", type=int, default=None, metavar="Q",
+                   help="decent on the ring or a static graph: mix Q times per step, theta <- W^Q theta, before the "
+                        "optimizer step (Q - 1 mix-only rounds, then the step's own); sends Q times the bytes "
+                        "(default 1)")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

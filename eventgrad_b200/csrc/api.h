@@ -243,6 +243,32 @@ cudaError_t launch_gossip_step_gt(const GossipParams& p, const TrackSlots& y, in
 // off, local_steps <= 1, the ring's inbox / push / flag / ack pointers and `psi`
 int gossip_ed_max_grid(int device);
 cudaError_t launch_gossip_step_ed(const GossipParams& p, const EdSlots& e, int grid, cudaStream_t s);
+// Mix-only gossip rounds (csrc/gossip_rounds.cu, --gossip-rounds Q >= 2, decent on the ring or a static circulant
+// graph): `rounds` = Q - 1 launches of one round each, enqueued after backward and before the step kernel.  Round q of
+// step k = *pass_num + 1 pushes theta into every out-slot's round inbox, flags and acks with h = rounds * (k - 1) + q,
+// and mixes theta <- (((theta + in_0) + in_1) + ...) / (n_slots + 1) in place.  Its own parameter block and window
+// sections (slot s of this rank receives from Graph.slots()[s]; out-slot j pushes into slot j of Graph.out_slots()[j]),
+// so no step kernel's parameters change.  2-rank ring: push[0] is null and inbox[0] == inbox[1] (one copy on the wire)
+struct RoundParams {
+  float* theta;
+  const int* pass_num;                  // completed steps (the gossip pass counter the step kernel advances)
+  unsigned int* ticket;                 // [1] last-CTA election of this kernel only
+  int* status;                          // sticky error word
+  unsigned long long timeout_ns;
+  int n_tiles;
+  int group_iters;                      // per-warp pipeline depth in tiles, as the step kernel's
+  int rounds;                           // Q - 1 >= 1
+  int n_slots;                          // 2 (ring) or 2|O|: even, 2..EG_MAX_SLOTS
+  const float* inbox[EG_MAX_SLOTS];     // local: round inbox of slot s
+  float* push[EG_MAX_SLOTS];            // peer-mapped: slot j's round inbox of my j-th out peer (null: not sent)
+  uint32_t* flag_from[EG_MAX_SLOTS];    // local [n_tiles * 8] (tile, warp), written by the sender of slot s
+  uint32_t* flag_to[EG_MAX_SLOTS];      // peer-mapped: flag_from[j] of my j-th out peer
+  uint32_t* ack_from[EG_MAX_SLOTS];     // local: my j-th out peer finished reading my round h push
+  uint32_t* ack_to[EG_MAX_SLOTS];       // peer-mapped: ack_from[s] of the sender of slot s
+};
+int gossip_rounds_max_grid(int device);  // co-resident CTAs (persistent grid upper bound)
+// the p.rounds launches of one step, q = 1 .. rounds, on stream s
+cudaError_t launch_gossip_rounds(const RoundParams& p, int grid, cudaStream_t s);
 // (re)compute tile_ss (+ shadow) from theta and evaluate the trigger for step pass_num+1.
 cudaError_t launch_gossip_init(const GossipParams& p, int grid, int run_fsm, cudaStream_t s);
 // Trigger FSM alone with externally supplied norms (unit tests against the oracle).

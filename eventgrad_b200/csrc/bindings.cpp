@@ -96,6 +96,13 @@ static const std::unordered_map<std::string, Setter<EdSlots>> kEd = {
     PTRF(EdSlots, psi),
 };
 
+static const std::unordered_map<std::string, Setter<RoundParams>> kRounds = {
+    PTRF(RoundParams, theta), PTRF(RoundParams, pass_num), PTRF(RoundParams, ticket), PTRF(RoundParams, status),
+    NUMF(RoundParams, timeout_ns), NUMF(RoundParams, n_tiles), NUMF(RoundParams, group_iters),
+    NUMF(RoundParams, rounds), NUMF(RoundParams, n_slots), ARRF(RoundParams, inbox), ARRF(RoundParams, push),
+    ARRF(RoundParams, flag_from), ARRF(RoundParams, flag_to), ARRF(RoundParams, ack_from), ARRF(RoundParams, ack_to),
+};
+
 static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce = {
     PTRF(AllReduceParams, peer_bufs), PTRF(AllReduceParams, local), PTRF(AllReduceParams, theta),
     PTRF(AllReduceParams, mom), PTRF(AllReduceParams, shadow), PTRF(AllReduceParams, peer_flags),
@@ -210,6 +217,7 @@ PYBIND11_MODULE(_C, m) {
   bind_params<Q8Slots>(m, "Q8Slots", kQ8);
   bind_params<TrackSlots>(m, "TrackSlots", kTrack);
   bind_params<EdSlots>(m, "EdSlots", kEd);
+  bind_params<RoundParams>(m, "RoundParams", kRounds);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
   bind_params<SlowMoParams>(m, "SlowMoParams", kSlowMo);
   bind_params<ConsensusParams>(m, "ConsensusParams", kConsensus);
@@ -245,6 +253,10 @@ PYBIND11_MODULE(_C, m) {
   m.def("gossip_ed_max_grid", &gossip_ed_max_grid);
   m.def("gossip_step_ed", [](const GossipParams& p, const EdSlots& e, int grid, uintptr_t s) {
     check(launch_gossip_step_ed(p, e, grid, S(s)), "gossip_step_ed");
+  });
+  m.def("gossip_rounds_max_grid", &gossip_rounds_max_grid);
+  m.def("gossip_rounds", [](const RoundParams& p, int grid, uintptr_t s) {
+    check(launch_gossip_rounds(p, grid, S(s)), "gossip_rounds");
   });
   m.def("gossip_init", [](const GossipParams& p, int grid, int run_fsm, uintptr_t s) {
     check(launch_gossip_init(p, grid, run_fsm, S(s)), "gossip_init");

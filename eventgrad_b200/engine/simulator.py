@@ -27,7 +27,7 @@ class RingSimulator:
                  offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1,
                  exact_diffusion: bool = False, global_avg_period: int = 0, quasi_global: bool = False,
                  slowmo_period: int = 0, slowmo_beta: float = 0.5, slowmo_lr: float = 1.0,
-                 consensus_every: int = 0, choco_gamma: float = 0.0):
+                 consensus_every: int = 0, choco_gamma: float = 0.0, gossip_rounds: int = 1):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -71,7 +71,12 @@ class RingSimulator:
         `consensus_every=N` (decent, event, spevent): after step k with N dividing k, append (k, D, A) of
         consensus_stats(theta, table) to `self.consensus` -- D_i = sum_r ||theta_r,i - theta_bar_i||^2 and
         A_i = ||theta_bar_i||^2 in float64, theta_bar = rank_mean(theta).  Read-only: training is unchanged.  At R = 1
-        every measurement is zero.  0: off."""
+        every measurement is zero.  0: off.
+        `gossip_rounds=Q` (decent on the ring or a static circulant graph, Q >= 2; multi-consensus D-PSGD): a gossip step
+        first runs Q - 1 mix-only rounds -- every rank pushes its current theta into every slot it feeds, then mixes
+        its inboxes into theta with the step's own mix (mix3_ on the ring, mixk_ on a static graph) -- and then the
+        unchanged step on the result, so theta_{k+1} = sgd(W^Q theta_k, g_k).  Bytes are Q times the step's.  At R = 1
+        nothing extra runs.  1: off."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -139,6 +144,15 @@ class RingSimulator:
         if consensus_every and algo == "cent":
             raise ValueError("consensus distance: cent keeps theta identical on every rank")
         self.consensus_every = int(consensus_every)
+        Q = gossip_rounds
+        if isinstance(Q, bool) or int(Q) != Q or Q < 1:
+            raise ValueError(f"gossip_rounds must be an integer >= 1, got {Q!r}")
+        if Q > 1 and (algo != "decent" or self.period or self.q8 or gradient_tracking or exact_diffusion
+                      or local_steps > 1 or global_avg_period or quasi_global or tau):
+            raise ValueError("gossip rounds: decent on the ring or a static graph, without compression, gradient "
+                             "tracking, exact diffusion, local steps, global averaging, quasi-global momentum or "
+                             "slowmo, only")
+        self.gossip_rounds = int(Q)
         self.consensus: List[Tuple[int, torch.Tensor, torch.Tensor]] = []
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
@@ -274,6 +288,8 @@ class RingSimulator:
             return self._step_global_avg(grads)
         if self.ed:
             return self._step_ed(grads)
+        for _ in range(self.gossip_rounds - 1 if R > 1 else 0):
+            self._mix_round()
         rnd = self.round_of(self.pass_num)
         # ---- phase 1: every rank decides and "Puts" (uses pre-mix theta_k) --------------
         if self.algo == "decent":
@@ -346,6 +362,21 @@ class RingSimulator:
                 continue
             self._sgd(r, grads[r])
 
+    def _mix_round(self) -> None:
+        """One mix-only round of --gossip-rounds: every rank pushes its whole theta into every slot it feeds, then every
+        rank mixes its inboxes into theta exactly as the step does.  No optimizer, no trigger, no events."""
+        R, t = self.R, self.table
+        snap = [th.clone() for th in self.theta]
+        for r in range(R):
+            for p, j in self.graphs[r].out_slots():
+                self.inbox[p][j].copy_(snap[r])
+            self.bytes[r] += self.fanout * t.n_elems * 4
+        for r in range(R):
+            if self.n_slots == 2:
+                mix3_(self.theta[r], self.inbox[r][0], self.inbox[r][1])
+            else:
+                mixk_(self.theta[r], self.inbox[r])
+
     def _step_ed(self, grads) -> None:
         """Exact diffusion: p = sgd(theta_k, g_k), phi = p + (theta_k - psi), psi <- p; phi goes to both neighbours (the
         ring's inboxes, decent's bytes); theta_{k+1} = (phi + ((phi + L) + R) / 3) / 2."""
@@ -394,14 +425,14 @@ class RingSimulator:
 
     def dense_messages(self) -> int:
         """Denominator of 'messages saved': fanout * sz * passes * R (BASELINE.md; 2 on the ring, 2|O| on a static
-        graph, 1 on the one-peer graph)."""
-        return self.fanout * self.table.n_tensors * self.pass_num * self.R
+        graph, 1 on the one-peer graph), times gossip_rounds."""
+        return self.gossip_rounds * self.fanout * self.table.n_tensors * self.pass_num * self.R
 
     def mixing_matrix(self, step: Optional[int] = None) -> torch.Tensor:
         """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD.  It depends on the 1-based step
         (default: the next one) on the one-peer graph, whose slot is that of the step's round, and under local_steps,
         where a step that does not communicate has W = I.  A global-averaging step has W = 11^T / R, and so does the
-        average of a SlowMo sync step (before its outer update)."""
+        average of a SlowMo sync step (before its outer update).  With gossip_rounds Q a gossip step has W^Q."""
         k = self.pass_num + 1 if step is None else step
         if self.global_avg_step(k) or self.slowmo_step(k):
             return torch.full((self.R, self.R), 1.0 / self.R, dtype=torch.float64)
@@ -409,4 +440,5 @@ class RingSimulator:
             return torch.eye(self.R, dtype=torch.float64)
         if self.period:
             return torch.tensor([g.mixing_row(self.round_of(k)) for g in self.graphs], dtype=torch.float64)
-        return torch.tensor([g.mixing_row() for g in self.graphs], dtype=torch.float64)
+        W = torch.tensor([g.mixing_row() for g in self.graphs], dtype=torch.float64)
+        return torch.linalg.matrix_power(W, self.gossip_rounds)

@@ -380,6 +380,7 @@ class Trainer:
         if gossip and env.rank == 0 and not cfg.quiet:
             print(f"Total number of events - {res['events_total']}", flush=True)
         dense = self.ring.fanout * self.arena.table.n_tensors * self.backend.pass_num * env.world
+        dense *= cfg.gossip_rounds if env.world > 1 else 1      # --gossip-rounds: every round sends every tensor
         res["dense_messages"] = dense
         res["messages_saved"] = (1.0 - res["events_total"] / dense) if (gossip and dense) else 0.0
         if evaluate and env.rank == 0:

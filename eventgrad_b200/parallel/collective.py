@@ -24,6 +24,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
   --consensus-every N (decent/event/spevent): after every N-th step all_gathers theta and records consensus_stats
   --quasi-global-momentum (decent/event/spevent): theta_k is snapshotted before the exchange and every SGD update is
           qg_sgd_, whose momentum follows theta_k - theta_{k+1}
+  --gossip-rounds Q (decent, ring / static graph): Q - 1 exchanges of theta, each followed by the step's own mix, then
+          the unchanged decent step
 
 torch.distributed has no one-sided RMA, so the "window" is emulated with an iteration-
 synchronous exchange: first the fire masks, then a payload holding only the fired tensors.
@@ -119,6 +121,8 @@ class CollectiveBackend(CommBackend):
         # counted in bytes_sent
         self.consensus_every = int(getattr(cfg, "consensus_every", 0)) if gossip else 0
         self.consensus_rows = []
+        # --gossip-rounds Q (decent, R >= 2): Q - 1 mix-only rounds before the decent step's exchange
+        self.gossip_rounds = int(getattr(cfg, "gossip_rounds", 1)) if cfg.algo == "decent" and ring.world > 1 else 1
         self.theta_k = None
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
@@ -250,16 +254,22 @@ class CollectiveBackend(CommBackend):
             return self._step_tracking()
         if self.ed:
             return self._step_ed()
+        for _ in range(self.gossip_rounds):            # --gossip-rounds Q: Q - 1 mix-only rounds, then the step's mix
+            self._mix_round()
+        self._opt()
+
+    def _mix_round(self) -> None:
+        """Exchange theta with every neighbour slot and mix it in (mix3_ on the ring, mixk_ on a graph): the decent
+        step without its optimizer, and one round of --gossip-rounds."""
+        a = self.arena
         if hasattr(self, "inbox"):
             self._exchange_slots(a.theta, self.inbox)
             self.bytes += self.ring.fanout * a.table.n_elems * 4
             self._mix_slots()
-            self._opt()
             return
         self._exchange([a.theta], [a.theta], [self.inbox_l], [self.inbox_r])
         self.bytes += 2 * a.table.n_elems * 4
         mix3_(a.theta, self.inbox_l, self.inbox_r)
-        self._opt()
 
     def _step_global_avg(self) -> None:
         """Global-averaging step, the simulator's ops: theta <- rank_mean(every rank's theta), then SGD on the own

@@ -22,6 +22,9 @@ Per training step, after backward():
            csrc/allreduce.cu gated on "tau divides the step" -- the two-shot average plus the outer update of x and u --
            then the step kernel: the gossip step (local_steps 1, which takes the plain SGD step at a sync step) or the
            serial step (local_steps tau, local SGD))
+           (--gossip-rounds Q, decent on the ring / a static graph: Q - 1 mix-only round launches of
+           csrc/gossip_rounds.cu before the step kernel, each pushing theta into its own round inboxes and mixing it in
+           place with the step's mix)
            (--consensus-every N, decent/event/spevent: one more launch per step after the step kernel, the
            consensus kernel of csrc/allreduce.cu gated on "N divides the step that just completed"; it only reads theta
            and writes per-tensor sums into a device ring that drain_consensus() reads at epoch boundaries)
@@ -107,6 +110,24 @@ def _add_consensus(lay: Layout, table: TensorTable, cfg, world: int) -> Layout:
     return lay
 
 
+def _wants_rounds(cfg, world: int) -> bool:
+    """--gossip-rounds Q >= 2 on decent with peers: the round kernel runs, and the window gets its sections.  At R = 1
+    nothing extra runs."""
+    return int(getattr(cfg, "gossip_rounds", 1)) > 1 and cfg.algo == "decent" and world > 1
+
+
+def _add_rounds(lay: Layout, table: TensorTable, cfg, world: int, n_slots: int) -> Layout:
+    """The round kernel's sections, appended last and only with Q > 1, so every other window keeps its layout: one
+    inbox, one (tile, warp) flag block and one ack word per slot (csrc/gossip_rounds.cu)."""
+    if _wants_rounds(cfg, world):
+        for k in range(n_slots):
+            lay.add(f"round_inbox_{k}", table.n_padded * 4)
+        for k in range(n_slots):
+            lay.add(f"round_flag_{k}", (table.n_tiles * 8 + 64) * 4)
+            lay.add(f"round_ack_{k}", 256)
+    return lay
+
+
 def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None) -> Layout:
     lay = Layout()
     n = table.n_padded * 4
@@ -121,7 +142,7 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None)
             lay.add(f"flag_from_{k}", nflag)
             lay.add(f"ack_from_{k}", 256)
         lay.add("ar_flags", 3 * max_grid * world * 4)
-        return _add_consensus(lay, table, cfg, world)
+        return _add_rounds(_add_consensus(lay, table, cfg, world), table, cfg, world, graph.n_slots)
     if _wants_q8(cfg):
         # int8 codes (one byte per arena element) and one fp32 scale per (tile, warp) block from each neighbour
         lay.add("q_from_l", table.n_padded)
@@ -152,7 +173,7 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None)
     lay.add("pushed_from_l", 256)
     lay.add("pushed_from_r", 256)
     lay.add("ar_flags", 3 * max_grid * world * 4)
-    return _add_consensus(lay, table, cfg, world)
+    return _add_rounds(_add_consensus(lay, table, cfg, world), table, cfg, world, 2)
 
 
 def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
@@ -173,6 +194,8 @@ def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
         max_grid = min(max_grid, C.gossip_gt_max_grid(env.device.index or 0))
     if _wants_ed(cfg, env.world):
         max_grid = min(max_grid, C.gossip_ed_max_grid(env.device.index or 0))
+    if _wants_rounds(cfg, env.world):
+        max_grid = min(max_grid, C.gossip_rounds_max_grid(env.device.index or 0))
     if _wants_consensus(cfg, env.world):
         # the query loads the consensus kernel now: enqueued behind spinning step kernels, a lazy load at its first
         # launch could wait for them to finish
@@ -276,6 +299,17 @@ class P2PBackend(CommBackend):
             raise ValueError("p2p backend: --slowmo-period runs decent on the fused single-kernel ring / static graph "
                              "step with --local-steps 1 or tau only")
         self.slowmo_x = self.slowmo_u = None
+        # --gossip-rounds Q (decent, R >= 2): Q - 1 launches of the round kernel before the unchanged ring,
+        # double-buffered ring or static-graph step kernel
+        self.gossip_rounds = int(getattr(cfg, "gossip_rounds", 1))
+        self.rounds = _wants_rounds(cfg, ring.world) and self.do_comm
+        if self.gossip_rounds > 1 and (cfg.algo != "decent" or self.overlap or self.q8 or self.gt or self.ed
+                                       or self.local_steps > 1 or self.global_avg_period or self.slowmo_period
+                                       or self.qg or getattr(cfg, "ce_push", False) or self.want_logs or not self.sync
+                                       or getattr(self.graph, "period", 0)):
+            raise ValueError("p2p backend: --gossip-rounds runs decent on the fused single-kernel ring, "
+                             "double-buffered ring or static graph step only")
+        self.round_ticket = None
         # --consensus-every N: the gated consensus kernel after the step kernel (R >= 2); its rows wait in a device
         # ring of `cons_cap` rows until drain_consensus().  At R = 1 account_step() records the zero rows itself
         self.consensus_every = int(getattr(cfg, "consensus_every", 0)) if self.gossip else 0
@@ -371,6 +405,8 @@ class P2PBackend(CommBackend):
         if self.drift:
             self.sent = self.prev if (self.sparse or self.q8) else zf(t.n_padded)
         self.ar_ctr = zi(1)
+        if self.rounds:
+            self.round_ticket = zi(1)
         if self.cons:
             self.cons_ring = torch.zeros(self.cons_cap * t.n_tensors * 2, dtype=torch.float64, device=dev)
             self.cons_step, self.cons_ctr = zi(self.cons_cap), zi(1)
@@ -387,6 +423,7 @@ class P2PBackend(CommBackend):
         self.host_bytes = 0
         self._connected = False
         self.gp = self.ap = self.ap_avg = self.ap_pga = self.sm = self.sp = self.gs = self.qs = self.ts = self.es = None
+        self.rp = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
@@ -551,6 +588,26 @@ class P2PBackend(CommBackend):
             C.sparse_params_to_device(sp, self.d_sp.data_ptr())
             if self.do_comm:
                 self.gp.update({"sparse": self.d_sp.data_ptr()})
+        if self.rounds:
+            # the ring's slots and the graph's share one wiring: slot s receives from ring.slots()[s], out-slot j writes
+            # slot j of its peer, and the receiver acks slot s into its sender's round ack word of the same index.
+            # 2-rank ring: one copy on the wire, into the peer's slot 1, read for both slots (as the ring step does)
+            g, n = self.ring, self.ring.n_slots
+            outs, ins = g.out_slots(), g.slots()
+            dedup = self.graph is None and self.ring.world == 2
+            rp = C.RoundParams()
+            rp.update({
+                "theta": P(a.theta), "pass_num": P(self.d_pass), "ticket": P(self.round_ticket),
+                "status": P(self.status), "timeout_ns": int(self.timeout_ns), "n_tiles": t.n_tiles,
+                "group_iters": int(self.group_iters), "rounds": self.gossip_rounds - 1, "n_slots": n,
+                "inbox": [win.addr("round_inbox_1" if dedup else f"round_inbox_{s}") for s in range(n)],
+                "push": [0 if (dedup and j == 0) else win.addr(f"round_inbox_{k}", p) for j, (p, k) in enumerate(outs)],
+                "flag_from": [win.addr(f"round_flag_{s}") for s in range(n)],
+                "flag_to": [win.addr(f"round_flag_{k}", p) for p, k in outs],
+                "ack_from": [win.addr(f"round_ack_{j}") for j in range(n)],
+                "ack_to": [win.addr(f"round_ack_{s}", ins[s]) for s in range(n)],
+            })
+            self.rp = rp
         # ---- all-reduce parameter blocks (cent step; final averaging for every algorithm) ----
         W = self.ring.world
         self.d_peer_grad = torch.tensor([win.addr("grad", r) for r in range(W)], dtype=torch.int64, device=self.dev)
@@ -799,6 +856,9 @@ class P2PBackend(CommBackend):
             if self.sm is not None:
                 # the sync comes first: the step kernel of a sync step runs SGD on theta <- x
                 C.slowmo_sync(self.sm, self.grid, s)
+            if self.rp is not None:
+                # theta <- W^(Q-1) theta, then the step kernel's own push, mix and optimizer step
+                C.gossip_rounds(self.rp, self.grid, s)
             if self.sparse and self.do_comm:
                 if not self.overlap:
                     C.sparse_select_push(self.sp, self.grid, s)        # 3 launches: hist, candidates, compaction
@@ -842,8 +902,9 @@ class P2PBackend(CommBackend):
             # --global-avg-period P: an averaging step counts one all-reduce of theta (cent's convention)
             self.host_bytes += self.table.n_elems * 4 if self.ring.world > 1 else 0
         elif self.cfg.algo == "decent" and self.do_comm and self.pass_num % self.local_steps == 0:
-            # --local-steps H: only every H-th step sends
-            self.host_bytes += getattr(self.ring, "fanout", 2) * self.table.n_elems * 4
+            # --local-steps H: only every H-th step sends; --gossip-rounds Q: every step sends Q times
+            q = self.gossip_rounds if self.rounds else 1
+            self.host_bytes += q * getattr(self.ring, "fanout", 2) * self.table.n_elems * 4
 
     def step(self) -> None:
         if self.overlap:        # no compute to hide behind when called stand-alone: run both halves in order
@@ -1009,7 +1070,9 @@ class P2PBackend(CommBackend):
             for k in range(self.graph.n_slots):
                 self.win.view(f"flag_from_{k}", torch.int32).fill_(step)
                 self.win.view(f"ack_from_{k}", torch.int32).fill_(step)
+            self._reset_rounds(step)
             return
+        self._reset_rounds(step)
         for name in ("flag_from_l", "flag_from_r", "ack_from_l", "ack_from_r", "pushed_from_l", "pushed_from_r"):
             self.win.view(name, torch.int32).fill_(step)
         if self.q8:
@@ -1019,6 +1082,15 @@ class P2PBackend(CommBackend):
         if self.sparse:
             for name in ("done_from_l", "done_from_r"):
                 self.win.view(name, torch.int32).fill_(step)
+
+    def _reset_rounds(self, step: int) -> None:
+        """--gossip-rounds: the round flags and acks restart at (Q - 1) * step, the counter of the last round of step
+        `step`, so the next step's first round waits for fresh flags and for no ack.  The round inboxes are not restored:
+        every round rewrites them before they are read."""
+        if self.rounds:
+            for k in range(self.ring.n_slots):
+                self.win.view(f"round_flag_{k}", torch.int32).fill_((self.gossip_rounds - 1) * step)
+                self.win.view(f"round_ack_{k}", torch.int32).fill_((self.gossip_rounds - 1) * step)
 
     def close(self) -> None:
         try:
