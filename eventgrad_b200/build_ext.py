@@ -20,7 +20,7 @@ CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
                            "--expt-relaxed-constexpr", "-Xptxas", "-v"]
-CU_SOURCES = ["gossip.cu", "gossip_dbuf.cu", "gossip_graph.cu", "gossip_q8.cu", "gossip_gt.cu", "gossip_ed.cu", "gossip_rounds.cu", "ce_push.cu", "allreduce.cu", "allreduce_nvls.cu", "sparse.cu", "augment.cu", "ipc.cu", "bn_act.cu", "bn_nchw.cu", "linear_tc_tma.cu", "conv_tc.cu"]
+CU_SOURCES = ["gossip.cu", "gossip_dbuf.cu", "gossip_graph.cu", "gossip_q8.cu", "gossip_gt.cu", "gossip_ed.cu", "gossip_rounds.cu", "gossip_match.cu", "ce_push.cu", "allreduce.cu", "allreduce_nvls.cu", "sparse.cu", "augment.cu", "ipc.cu", "bn_act.cu", "bn_nchw.cu", "linear_tc_tma.cu", "conv_tc.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 HEADERS = ["api.h", "common.cuh", "bn_common.cuh", "host_loader.h", "tc_common.cuh"]
 
@@ -83,7 +83,7 @@ def _build_locked(force: bool, verbose: bool) -> str:
         obj = os.path.join(BUILD, src + ".o")
         objs.append(obj)
         twin = {"gossip_dbuf.cu": "gossip.cu", "gossip_graph.cu": "gossip.cu", "gossip_q8.cu": "gossip.cu",
-                "gossip_gt.cu": "gossip.cu", "gossip_ed.cu": "gossip.cu",
+                "gossip_gt.cu": "gossip.cu", "gossip_ed.cu": "gossip.cu", "gossip_match.cu": "gossip.cu",
                 "allreduce_nvls.cu": "allreduce.cu"}.get(src)   # second compile of the same source
         deps = [sp] + hdrs + ([os.path.join(CSRC, twin)] if twin else [])
         if force or _stale(obj, deps):

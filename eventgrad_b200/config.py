@@ -75,7 +75,9 @@ class TrainConfig:
                                      # EGB_PEER_TIMEOUT_S overrides
     topology: str = "ring"           # gossip graph (parallel/topology.py): ring | exp (offsets 1,2,4,...) | "o1,o2,..."
                                      # | onepeer-exp (time-varying: one peer r + 2^((k-1) mod ceil(log2 R)) per step)
+                                     # | random-match (a seeded random perfect matching per step, pairwise averaging)
                                      # (circulant offsets, at most 4); decent/event only beyond the ring
+    topology_seed: int = 0           # random-match: seed in [0, 2^31) of the per-step matchings (same on every rank)
     compress: str = "none"           # none | int8 | sign: decent/event on the ring send the int8 (sign: 1-bit scaled sign)
                                      # code of theta - prev (one fp32 scale per 256 elements) instead of fp32 theta
     choco_gamma: float = 0.0         # int8/sign: 0 < gamma <= 1 mixes by CHOCO-SGD's consensus step on the public copies,
@@ -442,9 +444,54 @@ class TrainConfig:
             if self.file_write:
                 raise ValueError(f"{h} does not support file_write: the reference's log format records one exchange "
                                  "per step")
+        from .parallel.topology import check_match_seed, is_match
+        check_match_seed(self.topology_seed)
+        if is_match(self.topology):
+            self._validate_random_match()
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
+
+    def _validate_random_match(self) -> None:
+        """--topology random-match exists for decent in iter-sync mode: the fused single-inbox step (csrc/gossip_match.cu),
+        the torch.distributed backends and the simulator.  Each rejection says why."""
+        h = "--topology random-match"
+        if self.algo in ("event", "spevent"):
+            raise ValueError(f"{h} needs algo decent, got {self.algo!r}: a single inbox holds whichever peer wrote last, "
+                             "so a tensor that did not fire would mix with another rank's stale copy")
+        if self.algo != "decent":
+            raise ValueError(f"{h} needs algo decent, got {self.algo!r}: cent averages every gradient, it has no graph")
+        if self.sync_mode != "iter":
+            raise ValueError(f"{h} needs --sync-mode iter: a single inbox holds whichever peer wrote last, so an async "
+                             "mix could read another rank's stale copy")
+        if self.local_steps > 1:
+            raise ValueError(f"{h} does not support --local-steps {self.local_steps}")
+        if self.global_avg_period:
+            raise ValueError(f"{h} does not support --global-avg-period")
+        if self.slowmo_period:
+            raise ValueError(f"{h} does not support --slowmo-period")
+        if self.gossip_rounds > 1:
+            raise ValueError(f"{h} does not support --gossip-rounds {self.gossip_rounds}: a round would need a "
+                             "matching of its own")
+        if self.compress != "none":
+            raise ValueError(f"{h} does not support --compress {self.compress}: the replicas of a compressed peer "
+                             "assume a fixed neighbour")
+        if self.choco_gamma:
+            raise ValueError(f"{h} does not support --choco-gamma")
+        if self.gradient_tracking:
+            raise ValueError(f"{h} does not support --gradient-tracking")
+        if self.exact_diffusion:
+            raise ValueError(f"{h} does not support --exact-diffusion")
+        if self.quasi_global_momentum:
+            raise ValueError(f"{h} does not support --quasi-global-momentum")
+        if self.backend == "refport":
+            raise ValueError(f"{h} is not supported by --backend refport (ring only)")
+        for name in ("overlap_push", "double_buffer", "ce_push"):
+            if getattr(self, name):
+                raise ValueError(f"{h} does not support {name} (fused single-kernel step only)")
+        if self.file_write:
+            raise ValueError(f"{h} does not support file_write: the reference's log format has exactly one left and "
+                             "one right receive column")
 
     @property
     def ring_topology(self) -> bool:
@@ -459,8 +506,8 @@ class TrainConfig:
         offsets out of range for `world`."""
         if self.ring_topology:
             return self
-        from .parallel.topology import is_onepeer, parse_topology
-        if is_onepeer(self.topology):       # time-varying: the ring only when there is no peer at all
+        from .parallel.topology import is_match, is_onepeer, parse_topology
+        if is_onepeer(self.topology) or is_match(self.topology):   # time-varying: the ring only with no peer at all
             ring = world == 1
         else:
             ring = parse_topology(self.topology, world) == (1,)
@@ -563,10 +610,13 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
     p.add_argument("--double-buffer", action=argparse.BooleanOptionalAction, default=None)
     p.add_argument("--peer-timeout-s", type=float, default=None)
     p.add_argument("--ce-push", action="store_true", default=None)
-    p.add_argument("--topology", default=None, metavar="ring|exp|onepeer-exp|O1,O2,...",
-                   help="gossip graph: ring (default), exp (offsets 1,2,4,... up to R/2), explicit circulant offsets, or "
+    p.add_argument("--topology", default=None, metavar="ring|exp|onepeer-exp|random-match|O1,O2,...",
+                   help="gossip graph: ring (default), exp (offsets 1,2,4,... up to R/2), explicit circulant offsets, "
                         "onepeer-exp (time-varying: at step k push to r + 2^((k-1) mod ceil(log2 R)) only, "
-                        "mix (theta + received) / 2)")
+                        "mix (theta + received) / 2), or random-match (decent: a random perfect matching per step, "
+                        "seeded by --topology-seed; each rank averages with its partner, one idle rank at odd R)")
+    p.add_argument("--topology-seed", type=int, default=None, metavar="S",
+                   help="random-match: seed in [0, 2^31) of the per-step matchings, the same on every rank (default 0)")
     p.add_argument("--compress", default=None, choices=["none", "int8", "sign"],
                    help="decent/event on the ring: send the int8 code of theta - (what the neighbours hold) with one "
                         "fp32 scale per 256 elements, about a quarter of the fp32 bytes, or its 1-bit scaled sign, "

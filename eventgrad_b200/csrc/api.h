@@ -11,6 +11,7 @@
 #define EG_TILE 2048     // fp32 elements per tile == parallel/arena.py:TILE
 #define EG_THREADS 256
 #define EG_MAX_SLOTS 8   // inbox slots of a circulant gossip graph: 2 per offset, <= 4 offsets (parallel/topology.py)
+#define EG_MATCH_MAX_WORLD 1024   // random-match: ranks of the matching (its shuffle is kept in shared memory)
 
 namespace egb {
 
@@ -158,6 +159,28 @@ struct GraphSlots {
   uint32_t* ack_to[EG_MAX_SLOTS];       // peer-mapped: ack_from[s] of the sender of slot s
 };
 
+// Random pairwise matchings (csrc/gossip_match.cu, --topology random-match, decent): a separate block passed to the match
+// kernel next to GossipParams, whose ring pointers it leaves unused.  At step k = *pass_num + 1 thread 0 of every CTA
+// derives the partner p from (seed, world, k) (parallel/topology.py match_pairs: splitmix64 from (seed << 32) ^ k,
+// Fisher-Yates, pairs (pi[0], pi[1]), ...).  A matched rank waits for peers[p].done >= k - 1 (p has finished step k - 1,
+// so its single inbox is free), pushes theta_k into peers[p].inbox with one (tile, warp) flag = k in peers[p].flags,
+// waits for its own flag_from = k and mixes theta <- (theta + inbox) / 2; an idle rank (odd world) takes the plain SGD
+// step.  The last CTA stores *done = k on every rank (PROTOCOL.md 1.17).
+struct MatchPeer {
+  float* inbox;             // peer-mapped: that rank's single inbox [n_padded]
+  uint32_t* flags;          // peer-mapped: that rank's (tile, warp) flag block [n_tiles * 8]
+  const uint32_t* done;     // peer-mapped: the last step that rank has finished
+};
+struct MatchSlots {
+  int world;                // 2 .. EG_MATCH_MAX_WORLD
+  int rank;
+  int seed;                 // [0, 2^31)
+  const MatchPeer* peers;   // device array [world], built once by the backend
+  const float* inbox;       // local: what this step's partner pushed
+  uint32_t* flag_from;      // local [n_tiles * 8]: written by this step's partner
+  uint32_t* done;           // local: the last step this rank has finished (read by every partner)
+};
+
 // int8 error-feedback compression of the ring's pushes (csrc/gossip_q8.cu, --compress int8): a separate block passed
 // to the q8 kernel next to GossipParams, which keeps its ring flag / ack pointers.  Per fired tile each warp sends the
 // int8 code of theta - prev for its 256 elements (one 8-byte store per lane and neighbour) and one fp32 scale, adds the
@@ -228,6 +251,11 @@ cudaError_t launch_gossip_step_dbuf(const GossipParams& p, int grid, cudaStream_
 // [1, EG_MAX_SLOTS] (one-peer)
 int gossip_graph_max_grid(int device);
 cudaError_t launch_gossip_step_graph(const GossipParams& p, const GraphSlots& g, int grid, cudaStream_t s);
+// random-match step (csrc/gossip_match.cu): the fused single-kernel decent step over the single inbox of `m`; requires
+// phase 0, sync, do_push, do_mix and send_ack, no sparse block, no `sent`, the trigger off, local_steps <= 1, no global
+// averaging or quasi-global momentum, and every pointer of `m`
+int gossip_match_max_grid(int device);
+cudaError_t launch_gossip_step_match(const GossipParams& p, const MatchSlots& m, int grid, cudaStream_t s);
 // int8-compressed ring step (csrc/gossip_q8.cu): the fused single-kernel step with the pushes, replicas and flags of
 // `q`; requires phase 0, sync, do_push and do_mix, no sparse block, every pointer of `q` set, codec 0 or 1 and gamma 0
 // or in (0, 1].  The iter-sync flag of (tile, warp) carries 2*step + fired (PROTOCOL.md 1.7, 1.15)

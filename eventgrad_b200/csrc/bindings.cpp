@@ -96,6 +96,11 @@ static const std::unordered_map<std::string, Setter<EdSlots>> kEd = {
     PTRF(EdSlots, psi),
 };
 
+static const std::unordered_map<std::string, Setter<MatchSlots>> kMatch = {
+    NUMF(MatchSlots, world), NUMF(MatchSlots, rank), NUMF(MatchSlots, seed), PTRF(MatchSlots, peers),
+    PTRF(MatchSlots, inbox), PTRF(MatchSlots, flag_from), PTRF(MatchSlots, done),
+};
+
 static const std::unordered_map<std::string, Setter<RoundParams>> kRounds = {
     PTRF(RoundParams, theta), PTRF(RoundParams, pass_num), PTRF(RoundParams, ticket), PTRF(RoundParams, status),
     NUMF(RoundParams, timeout_ns), NUMF(RoundParams, n_tiles), NUMF(RoundParams, group_iters),
@@ -218,6 +223,8 @@ PYBIND11_MODULE(_C, m) {
   bind_params<TrackSlots>(m, "TrackSlots", kTrack);
   bind_params<EdSlots>(m, "EdSlots", kEd);
   bind_params<RoundParams>(m, "RoundParams", kRounds);
+  bind_params<MatchSlots>(m, "MatchSlots", kMatch);
+  m.attr("MATCH_PEER_BYTES") = (int)sizeof(MatchPeer);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
   bind_params<SlowMoParams>(m, "SlowMoParams", kSlowMo);
   bind_params<ConsensusParams>(m, "ConsensusParams", kConsensus);
@@ -253,6 +260,10 @@ PYBIND11_MODULE(_C, m) {
   m.def("gossip_ed_max_grid", &gossip_ed_max_grid);
   m.def("gossip_step_ed", [](const GossipParams& p, const EdSlots& e, int grid, uintptr_t s) {
     check(launch_gossip_step_ed(p, e, grid, S(s)), "gossip_step_ed");
+  });
+  m.def("gossip_match_max_grid", &gossip_match_max_grid);
+  m.def("gossip_step_match", [](const GossipParams& p, const MatchSlots& ms, int grid, uintptr_t s) {
+    check(launch_gossip_step_match(p, ms, grid, S(s)), "gossip_step_match");
   });
   m.def("gossip_rounds_max_grid", &gossip_rounds_max_grid);
   m.def("gossip_rounds", [](const RoundParams& p, int grid, uintptr_t s) {

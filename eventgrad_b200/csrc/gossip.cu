@@ -66,6 +66,12 @@
 // with P dividing k, the gated all-reduce enqueued before this kernel (csrc/allreduce.cu, gate_period = P) has already
 // replaced theta by the rank mean, and this kernel takes the same single-pass plain SGD step as a local step.  The
 // other steps gossip; their WAR guard waits for the ack of the last step that gossiped (PROTOCOL.md 1.11).
+// csrc/gossip_match.cu defines EG_MATCH and includes it a seventh time for random pairwise matchings
+// (`gossip_step_kernel_match`, decent, iter-sync fused step only; --topology random-match): thread 0 of every CTA derives
+// this step's partner from (seed, world, k) into shared memory (match_partner), the WAR guard waits for the partner's
+// `done` word to reach k - 1, each warp pushes its slice into the partner's single inbox and publishes the (tile, warp)
+// flag k there, waits for its own flag k and mixes (theta + inbox) / 2 as the one-peer graph does; the last CTA stores
+// `done` = k.  An idle rank (odd world) takes the single-pass plain SGD step and still stores `done` (PROTOCOL.md 1.17).
 // The int8, tracking and exact-diffusion builds derive their parameter block from GossipCore, which has no
 // global_avg_period, so their slots keep their offsets; the launchers of every build but the ring and graph refuse P.
 #include "api.h"
@@ -93,6 +99,11 @@ struct EdStepParams : GossipCore {        // kernel parameter of the exact-diffu
   EdSlots ed;
 };
 using StepParams = EdStepParams;
+#elif defined(EG_MATCH)
+struct MatchStepParams : GossipParams {   // kernel parameter of the match build: the ring block + the matching
+  MatchSlots m;
+};
+using StepParams = MatchStepParams;
 #else
 using StepParams = GossipParams;
 #endif
@@ -113,6 +124,9 @@ using StepParams = GossipParams;
 #elif defined(EG_ED)
 #define EG_SYM(name) name##_ed
 #define EG_SLOT_OFF(p, step) ((size_t)0)
+#elif defined(EG_MATCH)
+#define EG_SYM(name) name##_match
+#define EG_SLOT_OFF(p, step) ((size_t)0)
 #else
 #define EG_SYM(name) name
 #define EG_SLOT_OFF(p, step) ((size_t)0)
@@ -128,14 +142,14 @@ using StepParams = GossipParams;
 #endif
 // Periodic gossip (GossipParams.local_steps = H > 1) exists in the ring and graph builds only; the other builds gossip
 // at every step and their launchers reject H > 1
-#if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT) || defined(EG_ED)
+#if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT) || defined(EG_ED) || defined(EG_MATCH)
 #define EG_LOCAL_STEPS 0
 #else
 #define EG_LOCAL_STEPS 1
 #endif
 // Quasi-global momentum (GossipParams.quasi_global) exists in the ring, double-buffered and graph builds; the int8,
 // tracking and exact-diffusion builds take GossipCore, which has no such field, and their launchers reject it
-#if defined(EG_Q8) || defined(EG_GT) || defined(EG_ED)
+#if defined(EG_Q8) || defined(EG_GT) || defined(EG_ED) || defined(EG_MATCH)
 #define EG_QG 0
 #else
 #define EG_QG 1
@@ -447,6 +461,34 @@ __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, cons
   st_f8(p.push_l + base, phi);
   if (p.push_r != nullptr) st_f8(p.push_r + base, phi);
 }
+#elif defined(EG_MATCH)
+// theta_k of this thread's 8 elements into the single inbox of this step's partner `slot` (>= 0: the caller never pushes
+// on an idle step)
+__device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int slot) {
+  st_f8(p.m.peers[slot].inbox + base, th);
+}
+// Partner of this rank at 1-based step `step`, or -1 when it is idle (thread 0 only): splitmix64 from
+// (seed << 32) ^ step, Fisher-Yates over `pi` from the identity, pairs (pi[0], pi[1]), (pi[2], pi[3]), ...  Bit for bit
+// parallel/topology.py match_perm / match_partner
+__device__ __noinline__ int match_partner(int seed, int R, int rank, int step, short* pi) {
+  for (int i = 0; i < R; ++i) pi[i] = (short)i;
+  uint64_t x = ((uint64_t)(uint32_t)seed << 32) ^ (uint64_t)(uint32_t)step;
+  for (int i = R - 1; i >= 1; --i) {
+    x += 0x9E3779B97F4A7C15ull;
+    uint64_t z = x;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    z ^= z >> 31;
+    const int j = (int)(z % (uint64_t)(i + 1));
+    const short v = pi[i];
+    pi[i] = pi[j];
+    pi[j] = v;
+  }
+  int pos = 0;
+  while (pi[pos] != rank) ++pos;
+  if ((R & 1) && pos == R - 1) return -1;
+  return pi[pos ^ 1];
+}
 #else
 __device__ __forceinline__ void push_tile(const StepParams& p, size_t base, const F8& th, int /*slot*/) {
   // push_r == nullptr: 2-rank ring, the one neighbour is both left and right and reads the single copy twice
@@ -598,6 +640,19 @@ __device__ __forceinline__ void mix_tile(const StepParams& p, int t, const TileI
     const float k = (float)(p.g.n_slots + 1);
 #pragma unroll
     for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(th.v[e], k);
+  }
+#elif defined(EG_MATCH)
+  // one-peer mix with this step's partner: theta <- (theta + inbox) / 2, loaded after the gradient and momentum as the
+  // graph build stages its slots.  mix is false on an idle step
+  constexpr bool logrecv = false;
+  float ssl = 0.f, ssr = 0.f;
+  F8 m;
+  const F8 g = load_grad(p, ti, base, threadIdx.x);
+  if (kMom) m = ld_f8(p.mom + base);
+  if (mix) {
+    const F8 A = ld_f8_cg(p.m.inbox + base);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) th.v[e] = __fdiv_rn(__fadd_rn(th.v[e], A.v[e]), 2.f);
   }
 #elif defined(EG_Q8)
   // `slot` carries the sides whose neighbour fired this block (bit 0 left, bit 1 right), read from the flags.  The
@@ -804,6 +859,13 @@ __device__ __forceinline__ void grid_tail(const StepParams& p, int step, int slo
       for (int s = 0; s < EG_MAX_SLOTS; ++s)
         if (slot_on(p, s, slot)) st_release_sys(p.g.ack_to[s], (uint32_t)step);
     }
+#elif defined(EG_MATCH)
+    if (p.sync && p.send_ack) {
+      // every CTA of this rank has finished reading its inbox for `step` (idle ranks too): the partners of later steps
+      // may write it
+      fence_sys();
+      st_release_sys(p.m.done, (uint32_t)step);
+    }
 #elif !defined(EG_DBUF)
     if (p.sync && p.send_ack && comm) {
       // every CTA of this rank has finished reading its inboxes for `step`
@@ -871,12 +933,22 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
   // --local-steps H: step k gossips iff H divides k, as round k / H; every other step is the serial SGD step.
   // --global-avg-period P: a step with P dividing k is the serial SGD step on the averaged theta.  A uniform branch on
   // the device pass counter, which iter-sync keeps equal on every rank (PROTOCOL.md 1.9, 1.11)
+#ifdef EG_MATCH
+  // this step's partner, -1 when idle (uniform per grid): an idle step is the single-pass plain SGD step
+  __shared__ int s_partner;
+  __shared__ short s_pi[EG_MATCH_MAX_WORLD];
+  if (tid == 0) s_partner = match_partner(p.m.seed, p.m.world, p.m.rank, step, s_pi);
+  __syncthreads();
+  const int slot = s_partner;
+  const bool comm = slot >= 0;
+#else
   const bool comm = gossip_step_comm(p, step);
 #if EG_LOCAL_STEPS
   const int H = max(p.local_steps, 1);
   const int slot = EG_ACTIVE_SLOT(p, step / H);
 #else
   const int slot = EG_ACTIVE_SLOT(p, step);
+#endif
 #endif
   const int n_tiles = p.tab.n_tiles;
   const bool push = p.do_push != 0 && p.phase != 2 && comm;
@@ -887,7 +959,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 
 #if defined(EG_DBUF) || defined(EG_Q8) || defined(EG_GT) || defined(EG_ED)
   if (p.phase != 0 || !(p.sync && push)) return;   // the launcher rejects these; never reached
-#elif defined(EG_GRAPH)
+#elif defined(EG_GRAPH) || defined(EG_MATCH)
   if (p.phase != 0) return;                        // fused step only (the launcher rejects the rest)
 #else
   if (p.phase == 1) {
@@ -897,7 +969,7 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #endif
   __shared__ TileInfo s_ti[EG_TI_CACHE];
   fill_tile_cache(p, s_ti);
-#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT) && !defined(EG_ED)
+#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT) && !defined(EG_ED) && !defined(EG_MATCH)
   // spevent: receive side first -- scatter the records that arrived for this step into the replicas
   // (inbox_l / inbox_r point at them), grid barrier, then the dense mix below reads them tile by tile
   if (p.sparse != nullptr) sparse_apply_prologue(*p.sparse, p.sparse->bar);
@@ -946,6 +1018,15 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
       for (int k = 0; k < EG_MAX_SLOTS; ++k)
         if (slot_on(p, k, slot)) ok = wait_ge(p.g.ack_from[k], (uint32_t)prev, p.status, p.timeout_ns) && ok;
       s_ok = ok;
+    }
+    __syncthreads();
+    if (!s_ok) return;
+#elif defined(EG_MATCH)
+    __shared__ int s_ok;
+    if (tid == 0) {
+      // WAR guard: my partner has finished step k - 1, so nothing reads its inbox any more (it is written by one sender
+      // per step, and only once its owner is done with the previous one)
+      s_ok = wait_ge(p.m.peers[slot].done, (uint32_t)(step - 1), p.status, p.timeout_ns);
     }
     __syncthreads();
     if (!s_ok) return;
@@ -998,6 +1079,8 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
 #pragma unroll
           for (int k = 0; k < EG_MAX_SLOTS; ++k)   // (k: out-slot; j is the tile loop's index)
             if (slot_on(p, k, slot)) st_release_sys(p.g.flag_to[k] + (size_t)t * EG_WARPS + warp, (uint32_t)step);
+#elif defined(EG_MATCH)
+          st_release_sys(p.m.peers[slot].flags + (size_t)t * EG_WARPS + warp, (uint32_t)step);
 #elif defined(EG_Q8)
           // 2*step + fired: the receivers learn from the flag whether this block carries a delta
           const uint32_t v = 2u * (uint32_t)step + (fired ? 1u : 0u);
@@ -1032,6 +1115,8 @@ __global__ void __launch_bounds__(EG_THREADS, 4) EG_SYM(gossip_step_kernel)(cons
           for (int s = 0; s < EG_MAX_SLOTS; ++s)
             if (slot_on(p, s, slot))
               wait_ge(p.g.flag_from[s] + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
+#elif defined(EG_MATCH)
+          wait_ge(p.m.flag_from + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
 #else
           wait_ge(p.flag_from_l + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
           wait_ge(p.flag_from_r + (size_t)t2 * EG_WARPS + warp, (uint32_t)step, p.status, p.timeout_ns);
@@ -1063,7 +1148,7 @@ static inline bool qg_rejected(const GossipParams& p) {
   return p.quasi_global != 0 && (p.mu == 0.f || p.mom == nullptr || !p.sync || p.global_avg_period != 0);
 }
 
-#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT) && !defined(EG_ED)
+#if !defined(EG_DBUF) && !defined(EG_GRAPH) && !defined(EG_Q8) && !defined(EG_GT) && !defined(EG_ED) && !defined(EG_MATCH)
 // (Re)compute tile partials (+ bf16 shadow) from theta (drift trigger: from theta - sent); optionally evaluate the trigger for the
 // first step.  Used once at start-up and after theta is modified outside the step kernel
 // (checkpoint restore).
@@ -1307,6 +1392,35 @@ cudaError_t launch_gossip_step_ed(const GossipParams& p, const EdSlots& e, int g
     gossip_step_kernel_ed<true><<<grid, EG_THREADS, 0, s>>>(k);
   else
     gossip_step_kernel_ed<false><<<grid, EG_THREADS, 0, s>>>(k);
+  return cudaGetLastError();
+}
+
+#elif defined(EG_MATCH)   // only the step kernel + its launcher exist in this translation unit
+int gossip_match_max_grid(int device) {
+  int sms = 0, a = 0, b = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, gossip_step_kernel_match<true>, EG_THREADS, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, gossip_step_kernel_match<false>, EG_THREADS, 0);
+  if (b < a) a = b;
+  if (a < 1) a = 1;
+  return sms * a;
+}
+
+// Random-match step (decent): iter-sync fused step only, every tensor pushed to the step's partner.
+cudaError_t launch_gossip_step_match(const GossipParams& p, const MatchSlots& m, int grid, cudaStream_t s) {
+  const bool ok = m.world >= 2 && m.world <= EG_MATCH_MAX_WORLD && m.rank >= 0 && m.rank < m.world && m.seed >= 0 &&
+                  m.peers && m.inbox && m.flag_from && m.done;
+  if (p.phase != 0 || !p.sync || p.sparse != nullptr || p.sent != nullptr || p.fsm.enabled || !p.do_push ||
+      !p.do_mix || !p.send_ack || !ok || p.local_steps > 1 || p.global_avg_period != 0 || p.quasi_global != 0)
+    return cudaErrorInvalidValue;
+  MatchStepParams k;
+  static_cast<GossipParams&>(k) = p;
+  k.m = m;
+  eg_count_launch(EG_FAM_GOSSIP, 1);
+  if (p.mu != 0.f && p.mom != nullptr)
+    gossip_step_kernel_match<true><<<grid, EG_THREADS, 0, s>>>(k);
+  else
+    gossip_step_kernel_match<false><<<grid, EG_THREADS, 0, s>>>(k);
   return cudaGetLastError();
 }
 

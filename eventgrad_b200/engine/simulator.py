@@ -12,7 +12,7 @@ from typing import List, Optional, Sequence, Tuple
 import torch
 
 from ..parallel.arena import TensorTable
-from ..parallel.topology import Graph
+from ..parallel.topology import Graph, is_match, match_pairs
 from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, choco_mix_, codec_of, consensus_stats,
                                 drift_norms, mix2_, mix3_, mixk_, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
                                 trigger_step)
@@ -27,7 +27,8 @@ class RingSimulator:
                  offsets=(1,), compress: str = "none", gradient_tracking: bool = False, local_steps: int = 1,
                  exact_diffusion: bool = False, global_avg_period: int = 0, quasi_global: bool = False,
                  slowmo_period: int = 0, slowmo_beta: float = 0.5, slowmo_lr: float = 1.0,
-                 consensus_every: int = 0, choco_gamma: float = 0.0, gossip_rounds: int = 1):
+                 consensus_every: int = 0, choco_gamma: float = 0.0, gossip_rounds: int = 1,
+                 topology_seed: int = 0):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -76,7 +77,13 @@ class RingSimulator:
         first runs Q - 1 mix-only rounds -- every rank pushes its current theta into every slot it feeds, then mixes
         its inboxes into theta with the step's own mix (mix3_ on the ring, mixk_ on a static graph) -- and then the
         unchanged step on the result, so theta_{k+1} = sgd(W^Q theta_k, g_k).  Bytes are Q times the step's.  At R = 1
-        nothing extra runs.  1: off."""
+        nothing extra runs.  1: off.
+        `offsets="random-match"` with `topology_seed=S` (decent; randomized pairwise gossip): at step k the ranks are
+        paired by match_pairs(S, R, k) (parallel/topology.py); every matched rank pushes its whole theta_k into its
+        partner's single inbox and mixes theta <- (theta + inbox) / 2 (mix2_), then takes its SGD step; the idle rank of
+        an odd R takes its SGD step only.  A matched rank counts n_elems * 4 bytes per step, an idle rank none.  No
+        compression, tracking, exact diffusion, local steps, global averaging, quasi-global momentum, slowmo or extra
+        gossip rounds.  At R = 1 the name is the ring."""
         assert algo in ("cent", "decent", "event", "spevent")
         if compress not in COMPRESS:
             raise ValueError(f"compress must be one of {COMPRESS}, got {compress!r}")
@@ -88,7 +95,9 @@ class RingSimulator:
         if g and not self.q8:
             raise ValueError("choco_gamma: compress int8 or sign only")
         self.choco_gamma = float(g)
-        self.graphs = [Graph.build(r, world, offsets) for r in range(world)]
+        self.graphs = [Graph.build(r, world, offsets, seed=topology_seed) for r in range(world)]
+        self.match = is_match(self.graphs[0])         # random pairwise matchings: one inbox, partner from the seed
+        self.topology_seed = int(topology_seed)
         self.offsets = self.graphs[0].offsets
         self.n_slots = self.graphs[0].n_slots
         self.period = self.graphs[0].period          # 0: static graph; tau: one-peer graph, one active slot per step
@@ -153,6 +162,10 @@ class RingSimulator:
                              "tracking, exact diffusion, local steps, global averaging, quasi-global momentum or "
                              "slowmo, only")
         self.gossip_rounds = int(Q)
+        if self.match and (algo != "decent" or self.q8 or gradient_tracking or exact_diffusion or local_steps > 1
+                           or global_avg_period or quasi_global or tau or Q > 1):
+            raise ValueError("random-match: decent without compression, gradient tracking, exact diffusion, local "
+                             "steps, global averaging, quasi-global momentum, slowmo or gossip rounds, only")
         self.consensus: List[Tuple[int, torch.Tensor, torch.Tensor]] = []
         self.R, self.table, self.algo = world, table, algo
         self.tcfg = tcfg or TriggerConfig()
@@ -288,6 +301,8 @@ class RingSimulator:
             return self._step_global_avg(grads)
         if self.ed:
             return self._step_ed(grads)
+        if self.match:
+            return self._step_match(grads)
         for _ in range(self.gossip_rounds - 1 if R > 1 else 0):
             self._mix_round()
         rnd = self.round_of(self.pass_num)
@@ -377,6 +392,29 @@ class RingSimulator:
             else:
                 mixk_(self.theta[r], self.inbox[r])
 
+    def partners(self, step: int) -> List[Optional[int]]:
+        """random-match: the partner of every rank at 1-based step `step` (None: idle)."""
+        out: List[Optional[int]] = [None] * self.R
+        for a, b in match_pairs(self.topology_seed, self.R, step):
+            out[a], out[b] = b, a
+        return out
+
+    def _step_match(self, grads) -> None:
+        """random-match step: matched ranks swap theta_k through their single inbox and mix (theta + inbox) / 2, then
+        every rank takes its SGD step."""
+        R, t = self.R, self.table
+        part = self.partners(self.pass_num)
+        self.fire_history.append([torch.ones(t.n_tensors, dtype=torch.bool) for _ in range(R)])
+        snap = [th.clone() for th in self.theta]
+        for r in range(R):
+            if part[r] is not None:
+                self.inbox[part[r]][0].copy_(snap[r])
+                self.bytes[r] += t.n_elems * 4
+        for r in range(R):
+            if part[r] is not None:
+                mix2_(self.theta[r], self.inbox[r][0])
+            self._sgd(r, grads[r])
+
     def _step_ed(self, grads) -> None:
         """Exact diffusion: p = sgd(theta_k, g_k), phi = p + (theta_k - psi), psi <- p; phi goes to both neighbours (the
         ring's inboxes, decent's bytes); theta_{k+1} = (phi + ((phi + L) + R) / 3) / 2."""
@@ -432,13 +470,14 @@ class RingSimulator:
         """W [R, R] (float64) of the graph: theta' = W theta for decent without SGD.  It depends on the 1-based step
         (default: the next one) on the one-peer graph, whose slot is that of the step's round, and under local_steps,
         where a step that does not communicate has W = I.  A global-averaging step has W = 11^T / R, and so does the
-        average of a SlowMo sync step (before its outer update).  With gossip_rounds Q a gossip step has W^Q."""
+        average of a SlowMo sync step (before its outer update).  With gossip_rounds Q a gossip step has W^Q.  On
+        random-match, W_k pairs the matched ranks with weights 1/2 and leaves the idle rank's row e_r."""
         k = self.pass_num + 1 if step is None else step
         if self.global_avg_step(k) or self.slowmo_step(k):
             return torch.full((self.R, self.R), 1.0 / self.R, dtype=torch.float64)
         if not self.communicates(k):
             return torch.eye(self.R, dtype=torch.float64)
-        if self.period:
+        if self.match or self.period:     # random-match: round_of(k) == k (it refuses local steps)
             return torch.tensor([g.mixing_row(self.round_of(k)) for g in self.graphs], dtype=torch.float64)
         W = torch.tensor([g.mixing_row() for g in self.graphs], dtype=torch.float64)
         return torch.linalg.matrix_power(W, self.gossip_rounds)

@@ -43,7 +43,7 @@ class Trainer:
                  test_source=None):
         cfg = cfg.validate().resolved(env.device.type, env.world)
         self.cfg, self.env = cfg, env
-        graph = Graph.build(env.rank, env.world, cfg.topology)    # ValueError: offsets out of range for this world
+        graph = Graph.build(env.rank, env.world, cfg.topology, seed=cfg.topology_seed)    # ValueError: offsets out of range for this world
         self.ring = Ring(env.rank, env.world) if graph.is_ring else graph
         dev = env.device
         self.device = dev

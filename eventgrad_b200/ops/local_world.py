@@ -47,7 +47,7 @@ class LocalWorld:
             arena = ParamArena(model, self.device, theta=theta, grad=grad)
             if table_mode:
                 arena.enable_table_mode(shadow=False)
-            g = Graph.build(r, world, topology)
+            g = Graph.build(r, world, topology, seed=cfg.topology_seed)
             be = P2PBackend(cfg, arena, Ring(r, world) if g.is_ring else g, env, symm=symm, grid_cap=grid_cap,
                             defer_connect=True, **backend_kw)
             self.models.append(model)

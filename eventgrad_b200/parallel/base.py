@@ -15,6 +15,8 @@ from typing import Dict, List, Optional
 
 import torch
 
+from .topology import is_match
+
 
 @dataclass
 class StepLog:
@@ -32,15 +34,18 @@ class StepLog:
 def check_topology_state(sd: Dict, ring, algo: str) -> None:
     """Refuse to resume gossip state saved under a different graph: the inbox slots would mean other peers.  Ring
     checkpoints carry no `topology_offsets` key (their format predates graphs); static graphs carry no `topology` key,
-    time-varying ones store their name (onepeer-exp), whose offsets can equal a static graph's."""
+    time-varying ones store their name (onepeer-exp), whose offsets can equal a static graph's.  random-match also stores
+    its `topology_seed`: under another seed the run would continue with another sequence of matchings."""
     if algo not in ("decent", "event"):
         return
-    saved = (str(sd.get("topology", "circulant")), tuple(sd.get("topology_offsets", (1,))))
-    now = (getattr(ring, "kind", "circulant"), tuple(getattr(ring, "offsets", (1,))))
+    saved = (str(sd.get("topology", "circulant")), tuple(sd.get("topology_offsets", (1,))), sd.get("topology_seed"))
+    now = (getattr(ring, "kind", "circulant"), tuple(getattr(ring, "offsets", (1,))),
+           ring.seed if is_match(ring) else None)
     if saved != now:
-        raise ValueError(f"checkpoint was written with topology {saved[0]} offsets {saved[1]}, this run uses "
-                         f"{now[0]} offsets {now[1]}; "
-                         "resume with the same --topology")
+        seed = lambda s: "" if s is None else f" seed {s}"
+        raise ValueError(f"checkpoint was written with topology {saved[0]} offsets {saved[1]}{seed(saved[2])}, this run "
+                         f"uses {now[0]} offsets {now[1]}{seed(now[2])}; "
+                         "resume with the same --topology" + (" and --topology-seed" if saved[2] is not None else ""))
 
 
 def check_trigger_state(sd: Dict, metric: str, algo: str) -> None:

@@ -24,6 +24,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
   --consensus-every N (decent/event/spevent): after every N-th step all_gathers theta and records consensus_stats
   --quasi-global-momentum (decent/event/spevent): theta_k is snapshotted before the exchange and every SGD update is
           qg_sgd_, whose momentum follows theta_k - theta_{k+1}
+  --topology random-match (decent): at step k each matched rank swaps theta with its partner of match_pairs(seed, R, k)
+          (one batch_isend_irecv) and mixes add_ then div_(2); the idle rank of an odd R takes its SGD step only
   --gossip-rounds Q (decent, ring / static graph): Q - 1 exchanges of theta, each followed by the step's own mix, then
           the unchanged decent step
 
@@ -43,6 +45,7 @@ import torch.distributed as dist
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
                    check_choco_state, check_local_steps_state, check_qg_state, check_slowmo_state, check_topology_state,
                    check_tracking_state, check_trigger_state, slowmo_state)
+from .topology import is_match
 from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, choco_mix_, codec_of, consensus_stats, drift_norms, mix2_,
                       mix3_, mixk_, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
                       trigger_step)
@@ -262,6 +265,8 @@ class CollectiveBackend(CommBackend):
         """Exchange theta with every neighbour slot and mix it in (mix3_ on the ring, mixk_ on a graph): the decent
         step without its optimizer, and one round of --gossip-rounds."""
         a = self.arena
+        if is_match(self.ring):
+            return self._match_round()
         if hasattr(self, "inbox"):
             self._exchange_slots(a.theta, self.inbox)
             self.bytes += self.ring.fanout * a.table.n_elems * 4
@@ -270,6 +275,20 @@ class CollectiveBackend(CommBackend):
         self._exchange([a.theta], [a.theta], [self.inbox_l], [self.inbox_r])
         self.bytes += 2 * a.table.n_elems * 4
         mix3_(a.theta, self.inbox_l, self.inbox_r)
+
+    def _match_round(self) -> None:
+        """random-match: swap theta with this step's partner and mix (theta + received) / 2 -- add_ then div_(2), the
+        kernel's __fadd_rn / __fdiv_rn.  Both partners form the same sum, so they hold bitwise-equal theta after it.
+        An idle rank (odd R) exchanges nothing."""
+        a = self.arena
+        p = self.ring.partner(self.pass_num)
+        if p is None:
+            return
+        ops = [dist.P2POp(dist.isend, a.theta, p, self.group), dist.P2POp(dist.irecv, self.inbox[0], p, self.group)]
+        for w in dist.batch_isend_irecv(ops):
+            w.wait()
+        self.bytes += a.table.n_elems * 4
+        mix2_(a.theta, self.inbox[0])
 
     def _step_global_avg(self) -> None:
         """Global-averaging step, the simulator's ops: theta <- rank_mean(every rank's theta), then SGD on the own
@@ -576,6 +595,8 @@ class CollectiveBackend(CommBackend):
             sd["topology_offsets"] = list(self.ring.offsets)
             if self.ring.period:
                 sd["topology"] = self.ring.kind
+            if is_match(self.ring):
+                sd["topology"], sd["topology_seed"] = self.ring.kind, int(self.ring.seed)
             for s, ib in enumerate(self.inbox):
                 sd[f"inbox_{s}"] = ib.cpu().clone()
         return sd

@@ -25,6 +25,9 @@ Per training step, after backward():
            (--gossip-rounds Q, decent on the ring / a static graph: Q - 1 mix-only round launches of
            csrc/gossip_rounds.cu before the step kernel, each pushing theta into its own round inboxes and mixing it in
            place with the step's mix)
+           (--topology random-match, decent: csrc/gossip_match.cu derives this step's partner from the seed, waits for
+           the partner's `done` word of the previous step, pushes theta into its single inbox -> flags -> (t+in)/2 ->
+           SGD, and publishes `done`; an idle rank of an odd world takes the plain SGD step)
            (--consensus-every N, decent/event/spevent: one more launch per step after the step kernel, the
            consensus kernel of csrc/allreduce.cu gated on "N divides the step that just completed"; it only reads theta
            and writes per-tensor sums into a device ring that drain_consensus() reads at epoch boundaries)
@@ -43,7 +46,7 @@ from .arena import TILE, ParamArena, TensorTable
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
                    check_choco_state, check_local_steps_state, check_slowmo_state, slowmo_state, check_qg_state, check_topology_state, check_tracking_state,
                    check_trigger_state)
-from .topology import Graph
+from .topology import Graph, is_match
 from .trigger import codec_of
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
 
@@ -91,8 +94,8 @@ def _wants_ed(cfg, world: int) -> bool:
 
 
 def _graph_of(cfg, rank: int, world: int):
-    """The circulant graph of a non-ring topology, or None when the topology resolves to the ring."""
-    g = Graph.build(rank, world, getattr(cfg, "topology", "ring"))
+    """The circulant graph (or random matching) of a non-ring topology, or None when the topology resolves to the ring."""
+    g = Graph.build(rank, world, getattr(cfg, "topology", "ring"), seed=getattr(cfg, "topology_seed", 0))
     return None if g.is_ring else g
 
 
@@ -134,6 +137,14 @@ def build_layout(table: TensorTable, cfg, world: int, max_grid: int, graph=None)
     lay.add("theta", n)
     lay.add("grad", n)
     nflag = (table.n_tiles * 8 + 64) * 4      # one flag per (tile, warp)
+    if is_match(graph):
+        # random matchings: ONE inbox, one (tile, warp) flag block and one `done` word, whoever the sender
+        # (csrc/gossip_match.cu)
+        lay.add("match_inbox", n)
+        lay.add("match_flag", nflag)
+        lay.add("match_done", 256)
+        lay.add("ar_flags", 3 * max_grid * world * 4)
+        return _add_consensus(lay, table, cfg, world)
     if graph is not None:
         # circulant graph: one inbox, one flag block and one ack word per slot (csrc/gossip_graph.cu)
         for k in range(graph.n_slots):
@@ -186,7 +197,9 @@ def preallocate_arena_buffers(model, cfg, env, group=None, bootstrap=None):
     graph = _graph_of(cfg, env.rank, env.world) if cfg.algo in ("decent", "event") else None
     if _wants_dbuf(cfg):
         max_grid = min(max_grid, C.gossip_dbuf_max_grid(env.device.index or 0))
-    if graph is not None:
+    if is_match(graph):
+        max_grid = min(max_grid, C.gossip_match_max_grid(env.device.index or 0))
+    elif graph is not None:
         max_grid = min(max_grid, C.gossip_graph_max_grid(env.device.index or 0))
     if _wants_q8(cfg):
         max_grid = min(max_grid, C.gossip_q8_max_grid(env.device.index or 0))
@@ -240,6 +253,13 @@ class P2PBackend(CommBackend):
         self.do_comm = self.comm_enabled and self.gossip
         # circulant graph beyond the ring (parallel/topology.py): the fused single-kernel step of csrc/gossip_graph.cu
         self.graph = None if getattr(ring, "is_ring", True) else ring
+        # --topology random-match: the single-inbox step of csrc/gossip_match.cu (decent, iter-sync, fused step only)
+        self.match = ring if is_match(ring) else None
+        if self.match is not None:
+            self.graph = None
+            if (cfg.algo != "decent" or not self.sync or getattr(cfg, "overlap_push", False)
+                    or getattr(cfg, "ce_push", False) or self.want_logs):
+                raise ValueError("p2p backend: random-match runs decent on the fused iter-sync step only")
         if self.graph is not None and (cfg.algo not in ("decent", "event") or getattr(cfg, "overlap_push", False)
                                        or getattr(cfg, "ce_push", False) or self.want_logs):
             raise ValueError("p2p backend: a non-ring topology runs decent/event on the fused step only")
@@ -310,6 +330,10 @@ class P2PBackend(CommBackend):
             raise ValueError("p2p backend: --gossip-rounds runs decent on the fused single-kernel ring, "
                              "double-buffered ring or static graph step only")
         self.round_ticket = None
+        if self.match is not None and (self.q8 or self.gt or self.ed or self.local_steps > 1 or self.global_avg_period
+                                       or self.slowmo_period or self.qg or self.gossip_rounds > 1):
+            raise ValueError("p2p backend: random-match runs plain decent only (no compression, tracking, exact "
+                             "diffusion, local steps, global averaging, slowmo, quasi-global momentum or gossip rounds)")
         # --consensus-every N: the gated consensus kernel after the step kernel (R >= 2); its rows wait in a device
         # ring of `cons_cap` rows until drain_consensus().  At R = 1 account_step() records the zero rows itself
         self.consensus_every = int(getattr(cfg, "consensus_every", 0)) if self.gossip else 0
@@ -424,10 +448,13 @@ class P2PBackend(CommBackend):
         self._connected = False
         self.gp = self.ap = self.ap_avg = self.ap_pga = self.sm = self.sp = self.gs = self.qs = self.ts = self.es = None
         self.rp = None
+        self.ms = self.d_match_peers = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
             self.boot.publish("window_ptr", self.win.ptr)
             self.boot.publish("grid", self.grid)
+            if self.match is not None:
+                self.boot.publish("topology_seed", self.match.seed)
         if not defer_connect:
             self.connect()
 
@@ -441,8 +468,16 @@ class P2PBackend(CommBackend):
         else:
             grids = boot.all_gather_object(self.grid)
         self.grid = int(min(grids))          # identical persistent grid on every rank
+        if self.match is not None:
+            # every rank derives the matchings from the seed: a rank with another seed would wait for a partner that
+            # never pushes, and end in a timeout.  Refuse it here instead
+            seeds = boot.collect("topology_seed") if hasattr(boot, "collect") else \
+                boot.all_gather_object(self.match.seed)
+            if len(set(int(x) for x in seeds)) != 1:
+                raise ValueError(f"p2p backend: random-match needs the same --topology-seed on every rank, got "
+                                 f"{list(seeds)}")
         boot.connect(win)
-        L, R = (ring.left, ring.right) if self.graph is None else (None, None)
+        L, R = (ring.left, ring.right) if (self.graph is None and self.match is None) else (None, None)
         C, t, cfg = self.C, self.table, self.cfg
         a = self.arena
         P = lambda x: 0 if x is None else x.data_ptr()
@@ -489,7 +524,20 @@ class P2PBackend(CommBackend):
             if self.slowmo_local:
                 # local-SGD base: every step the step kernel runs is the serial step -- no push, mix, flag or ack
                 gp.update({"do_mix": 0, "do_push": 0, "send_ack": 0, "local_steps": 1})
-            if self.graph is None:
+            if self.match is not None:
+                # one inbox, one flag block and one `done` word per rank; every rank's three addresses in a device
+                # array (MatchPeer: inbox, flags, done), indexed by this step's partner
+                W = ring.world
+                self.d_match_peers = torch.tensor(
+                    [[win.addr("match_inbox", q), win.addr("match_flag", q), win.addr("match_done", q)] for q in range(W)],
+                    dtype=torch.int64, device=self.dev)
+                assert self.d_match_peers.numel() * 8 == W * C.MATCH_PEER_BYTES
+                ms = C.MatchSlots()
+                ms.update({"world": W, "rank": ring.rank, "seed": int(self.match.seed),
+                           "peers": P(self.d_match_peers), "inbox": win.addr("match_inbox"),
+                           "flag_from": win.addr("match_flag"), "done": win.addr("match_done")})
+                self.ms = ms
+            elif self.graph is None:
                 gp.update({
                     "flag_from_l": win.addr("flag_from_l"), "flag_from_r": win.addr("flag_from_r"),
                     "flag_to_l": win.addr("flag_from_r", L), "flag_to_r": win.addr("flag_from_l", R),
@@ -528,7 +576,7 @@ class P2PBackend(CommBackend):
                     "codec": 1 if self.compress == "sign" else 0, "gamma": self.choco_gamma,
                 })
                 self.qs = qs
-            elif dense and self.graph is None:
+            elif dense and self.graph is None and self.match is None:
                 gp.update({"inbox_l": win.addr("inbox_l"), "inbox_r": win.addr("inbox_r"),
                            "push_l": win.addr("inbox_r", L), "push_r": win.addr("inbox_l", R)})
                 # 2-rank ring: left == right.  Push theta ONCE (into the peer's inbox_r) and let the peer read that
@@ -869,6 +917,8 @@ class P2PBackend(CommBackend):
                 C.gossip_step_gt(self.gp, self.ts, self.grid, s)
             elif self.ed:
                 C.gossip_step_ed(self.gp, self.es, self.grid, s)
+            elif self.match is not None and self.do_comm:
+                C.gossip_step_match(self.gp, self.ms, self.grid, s)
             elif self.overlap:
                 C.gossip_step_phase(self.gp, 2, self.grid, s)
             elif self.dbuf:
@@ -901,6 +951,10 @@ class P2PBackend(CommBackend):
         elif self.global_avg_period and self.do_comm and self.pass_num % self.global_avg_period == 0:
             # --global-avg-period P: an averaging step counts one all-reduce of theta (cent's convention)
             self.host_bytes += self.table.n_elems * 4 if self.ring.world > 1 else 0
+        elif self.match is not None and self.do_comm:
+            # random-match: one copy to this step's partner, nothing on an idle step
+            if self.match.partner(self.pass_num) is not None:
+                self.host_bytes += self.table.n_elems * 4
         elif self.cfg.algo == "decent" and self.do_comm and self.pass_num % self.local_steps == 0:
             # --local-steps H: only every H-th step sends; --gossip-rounds Q: every step sends Q times
             q = self.gossip_rounds if self.rounds else 1
@@ -983,6 +1037,10 @@ class P2PBackend(CommBackend):
                 sd["topology"] = self.graph.kind
             for k in range(self.graph.n_slots):
                 sd[f"inbox_{k}"] = self.win.view(f"inbox_{k}", torch.float32).cpu().clone()
+        elif self.match is not None:
+            # the matching is a function of (seed, R, step): the name and the seed, and no inbox (every step's partner
+            # rewrites it before it is read)
+            sd["topology"], sd["topology_seed"], sd["topology_offsets"] = self.match.kind, int(self.match.seed), []
         elif self.cfg.algo in ("decent", "event") and not self.q8:
             sd["inbox_l"] = self.win.view("inbox_l", torch.float32).cpu().clone()
             sd["inbox_r"] = self.win.view("inbox_r", torch.float32).cpu().clone()
@@ -1066,6 +1124,12 @@ class P2PBackend(CommBackend):
         torch.cuda.synchronize(self.dev)
 
     def _reset_handshake(self, step: int) -> None:
+        if self.match is not None:
+            # flags and `done` restart at the resumed step s: step s + 1 waits for fresh flags and for partners that have
+            # finished step s, which every rank has
+            self.win.view("match_flag", torch.int32).fill_(step)
+            self.win.view("match_done", torch.int32).fill_(step)
+            return
         if self.graph is not None:
             for k in range(self.graph.n_slots):
                 self.win.view(f"flag_from_{k}", torch.int32).fill_(step)

@@ -26,20 +26,83 @@ R is a power of two, W_tau ... W_1 = 11^T / R: exact consensus every tau steps. 
 ring.  Rank r has tau slots: slot m receives from r - o_m and out-slot m feeds slot m of r + o_m.  In event mode slot m
 keeps the last value that arrived from r - o_m, which can be from step k - tau or earlier; the trigger state is per
 tensor, not per peer.
+
+`RandomMatch` ("random-match") is randomized pairwise gossip (Boyd et al. 2006): at every step the ranks are split into
+pairs by a random perfect matching, and each rank averages with its partner,
+    theta' = (theta + theta_partner) / 2          (one rounded add, one true division, as onepeer-exp)
+For odd R one rank is idle at each step (its own SGD step only).  The matching is a pure function of (seed, R, k),
+`match_pairs` below, so every rank computes it itself; csrc/gossip.cu (EG_MATCH) holds the identical device copy.  W_k
+is symmetric, doubly stochastic and idempotent, and lambda_2(E[W]) = (R - 2) / (2 (R - 1)) for even R, 1/2 for odd R.
+A rank sends ONE copy per step (none when idle).  At R == 1 the name resolves to the ring; at R == 2 the pair is fixed
+and the mix is onepeer-exp's.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import List, Tuple
+from typing import List, Optional, Tuple
 
 MAX_OFFSETS = 4          # degree <= 8 (csrc/api.h EG_MAX_SLOTS)
 MAX_SLOTS = 8            # csrc/api.h EG_MAX_SLOTS: the one-peer graph's period tau <= 8, i.e. R <= 256
 RING = (1,)
 ONEPEER = "onepeer-exp"
+MATCH = "random-match"
+MATCH_MAX_WORLD = 1024   # csrc/api.h EG_MATCH_MAX_WORLD: the device copy of the shuffle keeps pi in shared memory
+_M64 = (1 << 64) - 1
 
 
 def is_onepeer(spec) -> bool:
     return isinstance(spec, str) and spec.strip().lower() == ONEPEER
+
+
+def is_match(spec) -> bool:
+    """The random-match topology, by name or by topology object."""
+    if isinstance(spec, str):
+        return spec.strip().lower() == MATCH
+    return getattr(spec, "kind", None) == MATCH
+
+
+def check_match_seed(seed) -> None:
+    """--topology-seed: an int in [0, 2^31) (not a bool)."""
+    if isinstance(seed, bool) or not isinstance(seed, int) or not 0 <= seed < (1 << 31):
+        raise ValueError(f"--topology-seed must be an integer in [0, 2^31), got {seed!r}")
+
+
+def _splitmix64(x: int) -> Tuple[int, int]:
+    """One step of splitmix64: (new state, output)."""
+    x = (x + 0x9E3779B97F4A7C15) & _M64
+    z = x
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return x, z ^ (z >> 31)
+
+
+def match_perm(seed: int, world: int, step: int) -> List[int]:
+    """The shuffled rank order pi of 1-based step `step`: x_0 = (seed << 32) ^ step, then Fisher-Yates from the
+    identity, for i = R-1 down to 1 swap pi[i] and pi[next() mod (i + 1)]."""
+    if step < 1:
+        raise ValueError(f"steps are 1-based, got {step}")
+    x = ((seed << 32) ^ step) & _M64
+    pi = list(range(world))
+    for i in range(world - 1, 0, -1):
+        x, z = _splitmix64(x)
+        j = z % (i + 1)
+        pi[i], pi[j] = pi[j], pi[i]
+    return pi
+
+
+def match_pairs(seed: int, world: int, step: int) -> List[Tuple[int, int]]:
+    """The pairs (pi[0], pi[1]), (pi[2], pi[3]), ... of step `step`; for odd R, pi[R-1] is idle."""
+    pi = match_perm(seed, world, step)
+    return [(pi[i], pi[i + 1]) for i in range(0, world - 1, 2)]
+
+
+def match_partner(seed: int, world: int, step: int, rank: int) -> Optional[int]:
+    """The partner of `rank` at step `step`, or None when it is idle."""
+    pi = match_perm(seed, world, step)
+    pos = pi.index(rank)
+    if pos == world - 1 and world % 2 == 1:
+        return None
+    return pi[pos ^ 1]
 
 
 @dataclass(frozen=True)
@@ -118,10 +181,10 @@ def parse_topology(spec, world: int) -> Tuple[int, ...]:
         return RING
     if world < 1:
         raise ValueError(f"world must be >= 1, got {world}")
-    if s == ONEPEER:
+    if s in (ONEPEER, MATCH):
         if world == 1:
             return RING
-        raise ValueError(f"{ONEPEER} is time-varying: it has no static offsets (use Graph.build / OnePeerExp)")
+        raise ValueError(f"{s} is time-varying: it has no static offsets (use Graph.build)")
     half = world // 2
     if s == "exp":
         offs, o = [], 1
@@ -149,12 +212,12 @@ def parse_topology(spec, world: int) -> Tuple[int, ...]:
 def check_topology_name(spec) -> None:
     """World-independent syntax check of a topology name (TrainConfig.validate)."""
     s = str(spec).strip().lower()
-    if s in ("ring", "exp", ONEPEER):
+    if s in ("ring", "exp", ONEPEER, MATCH):
         return
     try:
         offs = [int(x) for x in s.split(",")]
     except ValueError:
-        raise ValueError(f"topology must be ring, exp, {ONEPEER} or comma-separated offsets like '1,3', "
+        raise ValueError(f"topology must be ring, exp, {ONEPEER}, {MATCH} or comma-separated offsets like '1,3', "
                          f"got {spec!r}") from None
     if not offs or len(offs) > MAX_OFFSETS or offs != sorted(set(offs)) or offs[0] < 1:
         raise ValueError(f"topology {spec!r}: 1 to {MAX_OFFSETS} distinct ascending offsets >= 1")
@@ -173,10 +236,13 @@ class Graph:
         object.__setattr__(self, "offsets", parse_topology(tuple(self.offsets), self.world))
 
     @staticmethod
-    def build(rank: int, world: int, spec="ring"):
-        """The graph of `spec` for this rank: a `Graph`, or a `OnePeerExp` for onepeer-exp at world >= 2."""
+    def build(rank: int, world: int, spec="ring", seed: int = 0):
+        """The graph of `spec` for this rank: a `Graph`, a `OnePeerExp` for onepeer-exp at world >= 2, or a
+        `RandomMatch` with matching seed `seed` for random-match at world >= 2."""
         if is_onepeer(spec) and world >= 2:
             return OnePeerExp(rank, world)
+        if is_match(spec) and world >= 2:
+            return RandomMatch(rank, world, seed)
         return Graph(rank, world, parse_topology(spec, world))
 
     period = 0               # static graph (OnePeerExp: tau)
@@ -316,4 +382,54 @@ class OnePeerExp:
         row = [0.0] * self.world
         row[self.rank] += 0.5
         row[self.in_peer(step)] += 0.5
+        return row
+
+
+@dataclass(frozen=True)
+class RandomMatch:
+    """Random pairwise matchings of one rank (see the module docstring): at step k (1-based) this rank averages with
+    match_partner(seed, R, k, rank), or is idle.  One inbox, whoever the sender; no static slots."""
+    rank: int
+    world: int
+    seed: int = 0
+
+    kind = MATCH
+    is_ring = False
+    period = 0               # not the one-peer graph's slot cycle: the partner comes from the matching
+    offsets = ()             # no circulant offsets (checkpoints store the name and the seed)
+
+    def __post_init__(self):
+        if not (0 <= self.rank < self.world):
+            raise ValueError(f"rank {self.rank} outside world {self.world}")
+        if self.world < 2:
+            raise ValueError(f"{MATCH} needs at least 2 ranks, got {self.world} (R = 1 resolves to the ring)")
+        if self.world > MATCH_MAX_WORLD:
+            raise ValueError(f"{MATCH}: at most {MATCH_MAX_WORLD} ranks, got {self.world}")
+        check_match_seed(self.seed)
+
+    @property
+    def serial(self) -> bool:
+        return False
+
+    @property
+    def n_slots(self) -> int:
+        return 1
+
+    @property
+    def fanout(self) -> int:
+        """Messages one tensor costs per step on a matched rank: one copy to the partner (an idle rank sends none)."""
+        return 1
+
+    def partner(self, step: int) -> Optional[int]:
+        return match_partner(self.seed, self.world, step, self.rank)
+
+    def mixing_row(self, step: int) -> List[float]:
+        """Row of W_step: 1/2 on me and 1/2 on my partner, or 1 on me when idle."""
+        row = [0.0] * self.world
+        p = self.partner(step)
+        if p is None:
+            row[self.rank] = 1.0
+        else:
+            row[self.rank] += 0.5
+            row[p] += 0.5
         return row

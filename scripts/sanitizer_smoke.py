@@ -26,7 +26,8 @@ def exchange(algo, **kw):
     w = LocalWorld(cfg, 2, lambda: build_model("cnn2"), grid_cap=4, timeout_ns=20_000_000_000)
     t = w.arenas[0].table
     sim = RingSimulator(2, w.arenas[0].theta.cpu(), t, algo, TriggerConfig.from_train(cfg), lr=cfg.lr,
-                        momentum=cfg.momentum, topk_percent=10.0, serial_skip=False, gossip_rounds=cfg.gossip_rounds)
+                        momentum=cfg.momentum, topk_percent=10.0, serial_skip=False, gossip_rounds=cfg.gossip_rounds,
+                        offsets=cfg.for_world(2).topology, topology_seed=cfg.topology_seed)
     mask = torch.zeros(t.n_padded, device="cuda")
     for o, n in zip(t.offsets, t.numels):
         mask[o:o + n] = 1
@@ -53,6 +54,7 @@ def main():
         exchange(algo)
     exchange("decent", overlap_push=True)
     exchange("decent", overlap_push=False, gossip_rounds=2)       # the mix-only round kernel ahead of the step
+    exchange("decent", topology="random-match", topology_seed=3)  # the single-inbox random-match step
     # fused BN (+res)(+relu), both paths
     from eventgrad_b200.ops.bn_act import FusedBNAct, _workspace
     for fused in (0, 1):
