@@ -101,6 +101,8 @@ class TrainConfig:
                                      # sqrt(sum_r ||theta_r - theta_bar||^2 / R) per tensor (read-only); 0 = off
     gossip_rounds: int = 1           # decent on the ring / a static graph: Q >= 2 runs Q - 1 mix-only gossip rounds
                                      # before the step's own mix, theta_{k+1} = SGD(W^Q theta_k); Q times the bytes
+    gossip_accel: str = "none"       # none | chebyshev: the Q rounds of --gossip-rounds apply the degree-Q Chebyshev
+                                     # polynomial P_Q(W) of the graph's spectrum instead of W^Q, at the same bytes
     # ---- data --------------------------------------------------------------
     data: str = "synthetic"          # synthetic | path to dataset root
     sampler: str = "random"          # random | sequential
@@ -411,39 +413,12 @@ class TrainConfig:
         if Q > 1:
             # the mix-only rounds exist for decent in front of the fused single-kernel ring, double-buffered ring and
             # static-graph steps (csrc/gossip_rounds.cu), the torch.distributed backends and the simulator
-            h = f"--gossip-rounds {Q}"
-            if self.algo != "decent":
-                raise ValueError(f"{h} needs algo decent, got {self.algo!r}"
-                                 + ("" if self.algo == "cent" else ": the trigger decides what a step sends, and a "
-                                    "mix-only round would send every tensor"))
-            if str(self.topology).strip().lower() == "onepeer-exp":
-                raise ValueError(f"{h} does not support topology onepeer-exp: its single active slot per step has no "
-                                 "rule for extra rounds")
-            if self.compress != "none":
-                raise ValueError(f"{h} does not support --compress {self.compress}: a mix-only round would have to "
-                                 "encode and replicate its own deltas")
-            if self.gradient_tracking:
-                raise ValueError(f"{h} does not support --gradient-tracking: y would need rounds of its own")
-            if self.exact_diffusion:
-                raise ValueError(f"{h} does not support --exact-diffusion: its step gossips phi, not theta")
-            if self.local_steps > 1:
-                raise ValueError(f"{h} does not support --local-steps {self.local_steps}")
-            if self.global_avg_period:
-                raise ValueError(f"{h} does not support --global-avg-period: an averaging step has no mix to repeat")
-            if self.slowmo_period:
-                raise ValueError(f"{h} does not support --slowmo-period: a sync step has no mix to repeat")
-            if self.quasi_global_momentum:
-                raise ValueError(f"{h} does not support --quasi-global-momentum: its theta_k is overwritten by the "
-                                 "rounds before the step kernel reads it")
-            if self.backend == "refport":
-                raise ValueError(f"{h} is not supported by --backend refport")
-            for name in ("overlap_push", "ce_push"):
-                if getattr(self, name):
-                    raise ValueError(f"{h} does not support {name}: the rounds overwrite theta, which the forward "
-                                     "reads, so they cannot run under backward")
-            if self.file_write:
-                raise ValueError(f"{h} does not support file_write: the reference's log format records one exchange "
-                                 "per step")
+            self._validate_rounds(f"--gossip-rounds {Q}")
+        from .parallel.topology import ACCELS
+        if self.gossip_accel not in ACCELS:
+            raise ValueError(f"--gossip-accel must be one of {'|'.join(ACCELS)}, got {self.gossip_accel!r}")
+        if self.gossip_accel != "none":
+            self._validate_gossip_accel()
         from .parallel.topology import check_match_seed, is_match
         check_match_seed(self.topology_seed)
         if is_match(self.topology):
@@ -451,6 +426,60 @@ class TrainConfig:
         if self.partition not in ("iid", "label"):
             raise ValueError(f"partition must be iid|label, got {self.partition!r}")
         return self
+
+    def _validate_rounds(self, h: str) -> None:
+        """The combinations the round kernel ahead of the step does not support, each with its reason; `h` names the
+        flag in the message."""
+        if self.algo != "decent":
+            raise ValueError(f"{h} needs algo decent, got {self.algo!r}"
+                             + ("" if self.algo == "cent" else ": the trigger decides what a step sends, and a "
+                                "mix-only round would send every tensor"))
+        if str(self.topology).strip().lower() == "onepeer-exp":
+            raise ValueError(f"{h} does not support topology onepeer-exp: its single active slot per step has no "
+                             "rule for extra rounds")
+        if self.compress != "none":
+            raise ValueError(f"{h} does not support --compress {self.compress}: a mix-only round would have to "
+                             "encode and replicate its own deltas")
+        if self.gradient_tracking:
+            raise ValueError(f"{h} does not support --gradient-tracking: y would need rounds of its own")
+        if self.exact_diffusion:
+            raise ValueError(f"{h} does not support --exact-diffusion: its step gossips phi, not theta")
+        if self.local_steps > 1:
+            raise ValueError(f"{h} does not support --local-steps {self.local_steps}")
+        if self.global_avg_period:
+            raise ValueError(f"{h} does not support --global-avg-period: an averaging step has no mix to repeat")
+        if self.slowmo_period:
+            raise ValueError(f"{h} does not support --slowmo-period: a sync step has no mix to repeat")
+        if self.quasi_global_momentum:
+            raise ValueError(f"{h} does not support --quasi-global-momentum: its theta_k is overwritten by the "
+                             "rounds before the step kernel reads it")
+        if self.backend == "refport":
+            raise ValueError(f"{h} is not supported by --backend refport")
+        for name in ("overlap_push", "ce_push"):
+            if getattr(self, name):
+                raise ValueError(f"{h} does not support {name}: the rounds overwrite theta, which the forward "
+                                 "reads, so they cannot run under backward")
+        if self.file_write:
+            raise ValueError(f"{h} does not support file_write: the reference's log format records one exchange "
+                             "per step")
+
+    def _validate_gossip_accel(self) -> None:
+        """--gossip-accel chebyshev runs the round kernel (csrc/gossip_rounds.cu) for every one of the Q rounds and then
+        the serial step kernel, so it takes every restriction of --gossip-rounds > 1, even at Q = 1, and a few of its
+        own.  Each rejection says why."""
+        h = f"--gossip-accel {self.gossip_accel}"
+        topo = str(self.topology).strip().lower()
+        if topo in ("onepeer-exp", "random-match"):
+            raise ValueError(f"{h} does not support topology {topo}: a time-varying W has no fixed spectrum to fit the "
+                             "polynomial to")
+        if self.sync_mode != "iter":
+            raise ValueError(f"{h} needs --sync-mode iter: every exchange is in the synchronous rounds, there is nothing "
+                             "left to relax")
+        if self.double_buffer:
+            raise ValueError(f"{h} does not support double_buffer: the step after the rounds exchanges nothing, so it "
+                             "has no inbox to double")
+        if self.gossip_rounds == 1:
+            self._validate_rounds(h)            # the rounds path runs at Q = 1 too (Q > 1 was checked already)
 
     def _validate_random_match(self) -> None:
         """--topology random-match exists for decent in iter-sync mode: the fused single-inbox step (csrc/gossip_match.cu),
@@ -541,7 +570,8 @@ class TrainConfig:
                                       and not bool(c.double_buffer) and c.ring_topology and c.compress == "none"
                                       and not c.gradient_tracking and c.local_steps == 1
                                       and not c.exact_diffusion and not c.global_avg_period
-                                      and not c.slowmo_period and c.gossip_rounds == 1)
+                                      and not c.slowmo_period and c.gossip_rounds == 1
+                                      and c.gossip_accel == "none")
         return dataclasses.replace(c, **kw) if kw else c
 
     def replace(self, **kw) -> "TrainConfig":
@@ -659,6 +689,10 @@ def _add_common_flags(p: argparse.ArgumentParser) -> None:
                    help="decent on the ring or a static graph: mix Q times per step, theta <- W^Q theta, before the "
                         "optimizer step (Q - 1 mix-only rounds, then the step's own); sends Q times the bytes "
                         "(default 1)")
+    p.add_argument("--gossip-accel", default=None, choices=["none", "chebyshev"],
+                   help="decent on the ring or a static graph: chebyshev runs the --gossip-rounds Q rounds as the "
+                        "degree-Q Chebyshev polynomial of the graph's spectrum, P_Q(W) theta, instead of W^Q theta, at "
+                        "the same bytes; Q = 1 is the optimally shifted W (default none)")
     p.add_argument("--fresh-replicas", dest="spevent_fresh_replicas", action="store_true", default=None,
                    help="spevent: initialise prev/left/right replicas like the reference (three more random nets)")
     p.add_argument("--no-grad-table", dest="grad_table", action="store_false", default=None)

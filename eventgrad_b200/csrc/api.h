@@ -297,6 +297,17 @@ struct RoundParams {
 int gossip_rounds_max_grid(int device);  // co-resident CTAs (persistent grid upper bound)
 // the p.rounds launches of one step, q = 1 .. rounds, on stream s
 cudaError_t launch_gossip_rounds(const RoundParams& p, int grid, cudaStream_t s);
+// Chebyshev-accelerated rounds (--gossip-accel chebyshev): the same RoundParams with `rounds` = Q (every round is a
+// round launch; the step kernel after them runs as the serial step), plus this block.  Round q keeps x_{q-1}, the theta
+// it loads, forms the round's mix w, and stores
+//   x_q = (x_{q-1} + alpha_q (w - x_{q-1})) + omega_q (x_{q-1} - x_{q-2})      (q = 1: no omega term, prev not read)
+// into theta, and x_{q-1} into prev for q < Q.  coef[2 (q - 1)] = alpha_q, coef[2 (q - 1) + 1] = omega_q, fp32
+// (parallel/topology.py chebyshev_coefficients)
+struct ChebParams {
+  float* prev;                          // local [n_padded]: x_{q-1} of the previous round
+  const float* coef;                    // device [Q][2]: (alpha_q, omega_q)
+};
+cudaError_t launch_gossip_rounds_cheb(const RoundParams& p, const ChebParams& c, int grid, cudaStream_t s);
 // (re)compute tile_ss (+ shadow) from theta and evaluate the trigger for step pass_num+1.
 cudaError_t launch_gossip_init(const GossipParams& p, int grid, int run_fsm, cudaStream_t s);
 // Trigger FSM alone with externally supplied norms (unit tests against the oracle).

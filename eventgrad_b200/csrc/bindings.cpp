@@ -108,6 +108,10 @@ static const std::unordered_map<std::string, Setter<RoundParams>> kRounds = {
     ARRF(RoundParams, flag_from), ARRF(RoundParams, flag_to), ARRF(RoundParams, ack_from), ARRF(RoundParams, ack_to),
 };
 
+static const std::unordered_map<std::string, Setter<ChebParams>> kCheb = {
+    PTRF(ChebParams, prev), PTRF(ChebParams, coef),
+};
+
 static const std::unordered_map<std::string, Setter<AllReduceParams>> kAllReduce = {
     PTRF(AllReduceParams, peer_bufs), PTRF(AllReduceParams, local), PTRF(AllReduceParams, theta),
     PTRF(AllReduceParams, mom), PTRF(AllReduceParams, shadow), PTRF(AllReduceParams, peer_flags),
@@ -223,6 +227,7 @@ PYBIND11_MODULE(_C, m) {
   bind_params<TrackSlots>(m, "TrackSlots", kTrack);
   bind_params<EdSlots>(m, "EdSlots", kEd);
   bind_params<RoundParams>(m, "RoundParams", kRounds);
+  bind_params<ChebParams>(m, "ChebParams", kCheb);
   bind_params<MatchSlots>(m, "MatchSlots", kMatch);
   m.attr("MATCH_PEER_BYTES") = (int)sizeof(MatchPeer);
   bind_params<AllReduceParams>(m, "AllReduceParams", kAllReduce);
@@ -268,6 +273,9 @@ PYBIND11_MODULE(_C, m) {
   m.def("gossip_rounds_max_grid", &gossip_rounds_max_grid);
   m.def("gossip_rounds", [](const RoundParams& p, int grid, uintptr_t s) {
     check(launch_gossip_rounds(p, grid, S(s)), "gossip_rounds");
+  });
+  m.def("gossip_rounds_cheb", [](const RoundParams& p, const ChebParams& c, int grid, uintptr_t s) {
+    check(launch_gossip_rounds_cheb(p, c, grid, S(s)), "gossip_rounds_cheb");
   });
   m.def("gossip_init", [](const GossipParams& p, int grid, int run_fsm, uintptr_t s) {
     check(launch_gossip_init(p, grid, run_fsm, S(s)), "gossip_init");

@@ -12,10 +12,10 @@ from typing import List, Optional, Sequence, Tuple
 import torch
 
 from ..parallel.arena import TensorTable
-from ..parallel.topology import Graph, is_match, match_pairs
-from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, choco_mix_, codec_of, consensus_stats,
-                                drift_norms, mix2_, mix3_, mixk_, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
-                                trigger_step)
+from ..parallel.topology import ACCELS, Graph, chebyshev_coefficients, is_match, match_pairs
+from ..parallel.trigger import (COMPRESS, TriggerConfig, TriggerState, cheb_combine_, choco_mix_, codec_of,
+                                consensus_stats, drift_norms, mix2_, mix3_, mixk_, qg_sgd_, rank_mean, sgd_, slowmo_sync_,
+                                topk_select, trigger_step)
 from .lr_schedule import lr_at
 
 
@@ -28,7 +28,7 @@ class RingSimulator:
                  exact_diffusion: bool = False, global_avg_period: int = 0, quasi_global: bool = False,
                  slowmo_period: int = 0, slowmo_beta: float = 0.5, slowmo_lr: float = 1.0,
                  consensus_every: int = 0, choco_gamma: float = 0.0, gossip_rounds: int = 1,
-                 topology_seed: int = 0):
+                 topology_seed: int = 0, gossip_accel: str = "none"):
         """`lr_table` (engine/lr_schedule.py): per-step learning rates, step s uses lr_table[min(s-1, len-1)];
         None = the constant `lr`.  `offsets`: circulant gossip graph (parallel/topology.py; a name such as "exp" is
         resolved for `world`), or "onepeer-exp" for the time-varying one-peer exponential graph; the default (1,) is
@@ -78,6 +78,12 @@ class RingSimulator:
         its inboxes into theta with the step's own mix (mix3_ on the ring, mixk_ on a static graph) -- and then the
         unchanged step on the result, so theta_{k+1} = sgd(W^Q theta_k, g_k).  Bytes are Q times the step's.  At R = 1
         nothing extra runs.  1: off.
+        `gossip_accel="chebyshev"` (decent on the ring or a static circulant graph, any Q >= 1): the Q rounds are
+        Chebyshev-accelerated -- round q pushes and mixes x_{q-1} into w exactly as a mix-only round, then
+        x_q = cheb_combine_(w, x_{q-1}, x_{q-2}, alpha_q, omega_q) with the fp32 coefficients of
+        parallel/topology.py chebyshev_coefficients (no omega term at q = 1) -- and every rank takes its SGD step on x_Q
+        with no further push or mix: theta_{k+1} = sgd(P_Q(W) theta_k, g_k).  Bytes are those of gossip_rounds=Q.  At
+        R = 1 nothing extra runs.  "none": off.
         `offsets="random-match"` with `topology_seed=S` (decent; randomized pairwise gossip): at step k the ranks are
         paired by match_pairs(S, R, k) (parallel/topology.py); every matched rank pushes its whole theta_k into its
         partner's single inbox and mixes theta <- (theta + inbox) / 2 (mix2_), then takes its SGD step; the idle rank of
@@ -162,6 +168,17 @@ class RingSimulator:
                              "tracking, exact diffusion, local steps, global averaging, quasi-global momentum or "
                              "slowmo, only")
         self.gossip_rounds = int(Q)
+        if gossip_accel not in ACCELS:
+            raise ValueError(f"gossip_accel must be one of {ACCELS}, got {gossip_accel!r}")
+        self.cheb_coef = None
+        if gossip_accel == "chebyshev":
+            if (algo != "decent" or self.period or self.match or self.q8 or gradient_tracking or exact_diffusion
+                    or local_steps > 1 or global_avg_period or quasi_global or tau):
+                raise ValueError("chebyshev gossip: decent on the ring or a static graph, without compression, gradient "
+                                 "tracking, exact diffusion, local steps, global averaging, quasi-global momentum or "
+                                 "slowmo, only")
+            if world > 1:
+                self.cheb_coef = chebyshev_coefficients(self.graphs[0].offsets, world, self.gossip_rounds)
         if self.match and (algo != "decent" or self.q8 or gradient_tracking or exact_diffusion or local_steps > 1
                            or global_avg_period or quasi_global or tau or Q > 1):
             raise ValueError("random-match: decent without compression, gradient tracking, exact diffusion, local "
@@ -303,6 +320,8 @@ class RingSimulator:
             return self._step_ed(grads)
         if self.match:
             return self._step_match(grads)
+        if self.cheb_coef is not None:
+            return self._step_cheb(grads)
         for _ in range(self.gossip_rounds - 1 if R > 1 else 0):
             self._mix_round()
         rnd = self.round_of(self.pass_num)
@@ -392,6 +411,23 @@ class RingSimulator:
             else:
                 mixk_(self.theta[r], self.inbox[r])
 
+    def _step_cheb(self, grads) -> None:
+        """Chebyshev-accelerated rounds: Q rounds of push + the step's mix of x_{q-1} (w), each followed by
+        cheb_combine_ with (alpha_q, omega_q), then every rank's SGD step on x_Q with no further push or mix."""
+        R, t = self.R, self.table
+        self.fire_history.append([torch.ones(t.n_tensors, dtype=torch.bool) for _ in range(R)])
+        x_prev = [None] * R
+        for alpha, omega in self.cheb_coef:
+            x = [th.clone() for th in self.theta]
+            self._mix_round()
+            a = torch.tensor(alpha, dtype=torch.float32)
+            o = torch.tensor(omega, dtype=torch.float32)
+            for r in range(R):
+                cheb_combine_(self.theta[r], x[r], x_prev[r], a, o)
+            x_prev = x
+        for r in range(R):
+            self._sgd(r, grads[r])
+
     def partners(self, step: int) -> List[Optional[int]]:
         """random-match: the partner of every rank at 1-based step `step` (None: idle)."""
         out: List[Optional[int]] = [None] * self.R
@@ -480,4 +516,14 @@ class RingSimulator:
         if self.match or self.period:     # random-match: round_of(k) == k (it refuses local steps)
             return torch.tensor([g.mixing_row(self.round_of(k)) for g in self.graphs], dtype=torch.float64)
         W = torch.tensor([g.mixing_row() for g in self.graphs], dtype=torch.float64)
+        if self.cheb_coef is not None:
+            # x_q = x_{q-1} + alpha_q (W x_{q-1} - x_{q-1}) + omega_q (x_{q-1} - x_{q-2}), from the fp32 coefficients
+            I = torch.eye(self.R, dtype=torch.float64)
+            prev, cur = None, I
+            for alpha, omega in self.cheb_coef:
+                nxt = cur + alpha * (W @ cur - cur)
+                if prev is not None:
+                    nxt = nxt + omega * (cur - prev)
+                prev, cur = cur, nxt
+            return cur
         return torch.linalg.matrix_power(W, self.gossip_rounds)

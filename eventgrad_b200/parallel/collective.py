@@ -28,6 +28,8 @@ plus eager elementwise ops -- i.e. what a straightforward port would look like:
           (one batch_isend_irecv) and mixes add_ then div_(2); the idle rank of an odd R takes its SGD step only
   --gossip-rounds Q (decent, ring / static graph): Q - 1 exchanges of theta, each followed by the step's own mix, then
           the unchanged decent step
+  --gossip-accel chebyshev (decent, ring / static graph): Q exchanges of theta, each followed by the step's own mix and
+          cheb_combine_ with x_{q-1} and x_{q-2}, then the optimizer alone
 
 torch.distributed has no one-sided RMA, so the "window" is emulated with an iteration-
 synchronous exchange: first the fire masks, then a payload holding only the fired tensors.
@@ -45,9 +47,9 @@ import torch.distributed as dist
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
                    check_choco_state, check_local_steps_state, check_qg_state, check_slowmo_state, check_topology_state,
                    check_tracking_state, check_trigger_state, slowmo_state)
-from .topology import is_match
-from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, choco_mix_, codec_of, consensus_stats, drift_norms, mix2_,
-                      mix3_, mixk_, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
+from .topology import chebyshev_coefficients, is_match
+from .trigger import (Q8_BLOCK, TriggerConfig, TriggerState, cheb_combine_, choco_mix_, codec_of, consensus_stats,
+                      drift_norms, mix2_, mix3_, mixk_, qg_sgd_, rank_mean, sgd_, slowmo_sync_, topk_select,
                       trigger_step)
 
 
@@ -126,6 +128,13 @@ class CollectiveBackend(CommBackend):
         self.consensus_rows = []
         # --gossip-rounds Q (decent, R >= 2): Q - 1 mix-only rounds before the decent step's exchange
         self.gossip_rounds = int(getattr(cfg, "gossip_rounds", 1)) if cfg.algo == "decent" and ring.world > 1 else 1
+        # --gossip-accel chebyshev (decent, R >= 2): each of the Q rounds combines its mix with x_{q-1} and x_{q-2} by
+        # the fp32 (alpha_q, omega_q) of parallel/topology.py, as 0-dim tensors on theta's device
+        self.cheb_coef = None
+        if getattr(cfg, "gossip_accel", "none") == "chebyshev" and cfg.algo == "decent" and ring.world > 1:
+            f = lambda v: torch.tensor(v, dtype=torch.float32, device=dev)
+            self.cheb_coef = [(f(al), f(om)) for al, om in
+                              chebyshev_coefficients(ring.offsets, ring.world, self.gossip_rounds)]
         self.theta_k = None
         if self.want_logs:
             z = lambda: torch.zeros(t.n_tensors, dtype=torch.float32, device=dev)
@@ -257,6 +266,15 @@ class CollectiveBackend(CommBackend):
             return self._step_tracking()
         if self.ed:
             return self._step_ed()
+        if self.cheb_coef is not None:
+            # --gossip-accel chebyshev: theta <- P_Q(W) theta, one exchange, mix and combine per round
+            x_prev = None
+            for alpha, omega in self.cheb_coef:
+                x = a.theta.clone()
+                self._mix_round()
+                cheb_combine_(a.theta, x, x_prev, alpha, omega)
+                x_prev = x
+            return self._opt()
         for _ in range(self.gossip_rounds):            # --gossip-rounds Q: Q - 1 mix-only rounds, then the step's mix
             self._mix_round()
         self._opt()

@@ -25,6 +25,8 @@ Per training step, after backward():
            (--gossip-rounds Q, decent on the ring / a static graph: Q - 1 mix-only round launches of
            csrc/gossip_rounds.cu before the step kernel, each pushing theta into its own round inboxes and mixing it in
            place with the step's mix)
+           (--gossip-accel chebyshev, the same with all Q rounds as Chebyshev round launches, each combining its mix
+           with x_{q-1} and x_{q-2}, then the step kernel as the serial step: no push, mix or handshake)
            (--topology random-match, decent: csrc/gossip_match.cu derives this step's partner from the seed, waits for
            the partner's `done` word of the previous step, pushes theta into its single inbox -> flags -> (t+in)/2 ->
            SGD, and publishes `done`; an idle rank of an odd world takes the plain SGD step)
@@ -46,7 +48,7 @@ from .arena import TILE, ParamArena, TensorTable
 from .base import (CommBackend, StepLog, check_compress_state, check_exact_diffusion_state, check_global_avg_state,
                    check_choco_state, check_local_steps_state, check_slowmo_state, slowmo_state, check_qg_state, check_topology_state, check_tracking_state,
                    check_trigger_state)
-from .topology import Graph, is_match
+from .topology import Graph, chebyshev_coefficients, is_match
 from .trigger import codec_of
 from .window import DistBootstrap, Layout, SymmWindow, Window, wants_symm_window
 
@@ -73,7 +75,8 @@ def _wants_dbuf(cfg) -> bool:
             and not getattr(cfg, "overlap_push", False) and getattr(cfg, "ring_topology", True)
             and not _wants_q8(cfg) and not getattr(cfg, "gradient_tracking", False)
             and getattr(cfg, "local_steps", 1) == 1 and not getattr(cfg, "exact_diffusion", False)
-            and not getattr(cfg, "global_avg_period", 0) and not getattr(cfg, "slowmo_period", 0))
+            and not getattr(cfg, "global_avg_period", 0) and not getattr(cfg, "slowmo_period", 0)
+            and getattr(cfg, "gossip_accel", "none") == "none")
 
 
 def _wants_q8(cfg) -> bool:
@@ -113,10 +116,23 @@ def _add_consensus(lay: Layout, table: TensorTable, cfg, world: int) -> Layout:
     return lay
 
 
+def _wants_cheb(cfg) -> bool:
+    """--gossip-accel chebyshev: every one of the Q rounds is a Chebyshev round kernel launch, then the serial step."""
+    return getattr(cfg, "gossip_accel", "none") == "chebyshev"
+
+
+def _rounds_per_step(cfg) -> int:
+    """Round kernel launches per step: Q - 1 ahead of the step kernel's own mix under --gossip-rounds Q, all Q under
+    --gossip-accel chebyshev (whose step kernel then mixes nothing).  The round handshake counter of round q of step k
+    is h = n (k - 1) + q with n this number."""
+    Q = int(getattr(cfg, "gossip_rounds", 1))
+    return Q if _wants_cheb(cfg) else Q - 1
+
+
 def _wants_rounds(cfg, world: int) -> bool:
-    """--gossip-rounds Q >= 2 on decent with peers: the round kernel runs, and the window gets its sections.  At R = 1
-    nothing extra runs."""
-    return int(getattr(cfg, "gossip_rounds", 1)) > 1 and cfg.algo == "decent" and world > 1
+    """--gossip-rounds Q >= 2, or --gossip-accel chebyshev at any Q, on decent with peers: the round kernel runs, and
+    the window gets its sections.  At R = 1 nothing extra runs."""
+    return _rounds_per_step(cfg) >= 1 and cfg.algo == "decent" and world > 1
 
 
 def _add_rounds(lay: Layout, table: TensorTable, cfg, world: int, n_slots: int) -> Layout:
@@ -330,6 +346,16 @@ class P2PBackend(CommBackend):
             raise ValueError("p2p backend: --gossip-rounds runs decent on the fused single-kernel ring, "
                              "double-buffered ring or static graph step only")
         self.round_ticket = None
+        # --gossip-accel chebyshev: all Q rounds are Chebyshev round launches (x_{q-1} kept in `cheb_prev`, local and
+        # outside the window), then the step kernel runs as the serial step: no push, no mix, no handshake
+        self.cheb = _wants_cheb(cfg) and self.rounds
+        if _wants_cheb(cfg) and (cfg.algo != "decent" or self.overlap or getattr(cfg, "double_buffer", None)
+                                 or self.q8 or self.gt or self.ed or self.local_steps > 1 or self.global_avg_period
+                                 or self.slowmo_period or self.qg or getattr(cfg, "ce_push", False) or self.want_logs
+                                 or not self.sync or getattr(self.graph, "period", 0) or self.match is not None):
+            raise ValueError("p2p backend: --gossip-accel chebyshev runs decent on the ring or a static graph, with "
+                             "the serial step after the rounds, only")
+        self.cheb_prev = self.d_cheb_coef = None
         if self.match is not None and (self.q8 or self.gt or self.ed or self.local_steps > 1 or self.global_avg_period
                                        or self.slowmo_period or self.qg or self.gossip_rounds > 1):
             raise ValueError("p2p backend: random-match runs plain decent only (no compression, tracking, exact "
@@ -431,6 +457,13 @@ class P2PBackend(CommBackend):
         self.ar_ctr = zi(1)
         if self.rounds:
             self.round_ticket = zi(1)
+        if self.cheb:
+            # x_{q-1} of the rounds (rewritten by round q < Q before round q + 1 reads it) and the fp32
+            # (alpha_q, omega_q)
+            Q = self.gossip_rounds
+            self.cheb_prev = zf(t.n_padded)
+            self.d_cheb_coef = torch.tensor(chebyshev_coefficients(ring.offsets, ring.world, Q), dtype=torch.float32,
+                                            device=dev).reshape(Q * 2)
         if self.cons:
             self.cons_ring = torch.zeros(self.cons_cap * t.n_tensors * 2, dtype=torch.float64, device=dev)
             self.cons_step, self.cons_ctr = zi(self.cons_cap), zi(1)
@@ -447,7 +480,7 @@ class P2PBackend(CommBackend):
         self.host_bytes = 0
         self._connected = False
         self.gp = self.ap = self.ap_avg = self.ap_pga = self.sm = self.sp = self.gs = self.qs = self.ts = self.es = None
-        self.rp = None
+        self.rp = self.cs = None
         self.ms = self.d_match_peers = None
         self.d_lr = None
         if hasattr(self.boot, "publish"):
@@ -521,8 +554,9 @@ class P2PBackend(CommBackend):
                                      if self.do_comm else 0,
                 "quasi_global": 1 if self.qg else 0,
             })
-            if self.slowmo_local:
-                # local-SGD base: every step the step kernel runs is the serial step -- no push, mix, flag or ack
+            if self.slowmo_local or self.cheb:
+                # local-SGD base / after the Chebyshev rounds: every step the step kernel runs is the serial step -- no
+                # push, mix, flag or ack
                 gp.update({"do_mix": 0, "do_push": 0, "send_ack": 0, "local_steps": 1})
             if self.match is not None:
                 # one inbox, one flag block and one `done` word per rank; every rank's three addresses in a device
@@ -647,7 +681,7 @@ class P2PBackend(CommBackend):
             rp.update({
                 "theta": P(a.theta), "pass_num": P(self.d_pass), "ticket": P(self.round_ticket),
                 "status": P(self.status), "timeout_ns": int(self.timeout_ns), "n_tiles": t.n_tiles,
-                "group_iters": int(self.group_iters), "rounds": self.gossip_rounds - 1, "n_slots": n,
+                "group_iters": int(self.group_iters), "rounds": _rounds_per_step(cfg), "n_slots": n,
                 "inbox": [win.addr("round_inbox_1" if dedup else f"round_inbox_{s}") for s in range(n)],
                 "push": [0 if (dedup and j == 0) else win.addr(f"round_inbox_{k}", p) for j, (p, k) in enumerate(outs)],
                 "flag_from": [win.addr(f"round_flag_{s}") for s in range(n)],
@@ -656,6 +690,10 @@ class P2PBackend(CommBackend):
                 "ack_to": [win.addr(f"round_ack_{s}", ins[s]) for s in range(n)],
             })
             self.rp = rp
+            if self.cheb:
+                cs = C.ChebParams()
+                cs.update({"prev": P(self.cheb_prev), "coef": P(self.d_cheb_coef)})
+                self.cs = cs
         # ---- all-reduce parameter blocks (cent step; final averaging for every algorithm) ----
         W = self.ring.world
         self.d_peer_grad = torch.tensor([win.addr("grad", r) for r in range(W)], dtype=torch.int64, device=self.dev)
@@ -904,7 +942,10 @@ class P2PBackend(CommBackend):
             if self.sm is not None:
                 # the sync comes first: the step kernel of a sync step runs SGD on theta <- x
                 C.slowmo_sync(self.sm, self.grid, s)
-            if self.rp is not None:
+            if self.cs is not None:
+                # theta <- P_Q(W) theta, then the step kernel as the serial step (gp: no push, mix or ack)
+                C.gossip_rounds_cheb(self.rp, self.cs, self.grid, s)
+            elif self.rp is not None:
                 # theta <- W^(Q-1) theta, then the step kernel's own push, mix and optimizer step
                 C.gossip_rounds(self.rp, self.grid, s)
             if self.sparse and self.do_comm:
@@ -923,7 +964,7 @@ class P2PBackend(CommBackend):
                 C.gossip_step_phase(self.gp, 2, self.grid, s)
             elif self.dbuf:
                 C.gossip_step_dbuf(self.gp, self.grid, s)
-            elif self.graph is not None and self.do_comm and not self.slowmo_local:
+            elif self.graph is not None and self.do_comm and not self.slowmo_local and not self.cheb:
                 C.gossip_step_graph(self.gp, self.gs, self.grid, s)
             else:
                 C.gossip_step(self.gp, self.grid, s)
@@ -1148,13 +1189,15 @@ class P2PBackend(CommBackend):
                 self.win.view(name, torch.int32).fill_(step)
 
     def _reset_rounds(self, step: int) -> None:
-        """--gossip-rounds: the round flags and acks restart at (Q - 1) * step, the counter of the last round of step
-        `step`, so the next step's first round waits for fresh flags and for no ack.  The round inboxes are not restored:
-        every round rewrites them before they are read."""
+        """--gossip-rounds: the round flags and acks restart at n * step (n = _rounds_per_step: Q - 1, or Q under
+        Chebyshev), the counter of the last round of step `step`, so the next step's first round waits for fresh flags
+        and for no ack.  The round inboxes and the Chebyshev `prev` are not restored: every round rewrites them before
+        they are read."""
         if self.rounds:
+            n = _rounds_per_step(self.cfg)
             for k in range(self.ring.n_slots):
-                self.win.view(f"round_flag_{k}", torch.int32).fill_((self.gossip_rounds - 1) * step)
-                self.win.view(f"round_ack_{k}", torch.int32).fill_((self.gossip_rounds - 1) * step)
+                self.win.view(f"round_flag_{k}", torch.int32).fill_(n * step)
+                self.win.view(f"round_ack_{k}", torch.int32).fill_(n * step)
 
     def close(self) -> None:
         try:

@@ -35,9 +35,15 @@ For odd R one rank is idle at each step (its own SGD step only).  The matching i
 is symmetric, doubly stochastic and idempotent, and lambda_2(E[W]) = (R - 2) / (2 (R - 1)) for even R, 1/2 for odd R.
 A rank sends ONE copy per step (none when idle).  At R == 1 the name resolves to the ring; at R == 2 the pair is fixed
 and the mix is onepeer-exp's.
+
+`circulant_spectrum` / `chebyshev_coefficients` give the closed-form spectrum of a circulant W on 1^perp and the
+coefficients of Chebyshev-accelerated gossip rounds (--gossip-accel chebyshev) fitted to it.  Every backend and the
+simulator take the coefficients from here; no other module derives the spectrum.
 """
 from __future__ import annotations
 
+import math
+import struct
 from dataclasses import dataclass
 from typing import List, Optional, Tuple
 
@@ -433,3 +439,53 @@ class RandomMatch:
             row[self.rank] += 0.5
             row[p] += 0.5
         return row
+
+
+# ---- Chebyshev-accelerated gossip rounds (--gossip-accel chebyshev) ---------------------------------------------------
+ACCELS = ("none", "chebyshev")
+CHEB_POINT = 1e-12       # half-width below which the spectrum on 1^perp is one point (the ring at R = 2 and R = 3)
+
+
+def _fp32(x: float) -> float:
+    """x rounded once to the nearest fp32 (round half to even), as a Python float."""
+    return struct.unpack("f", struct.pack("f", x))[0]
+
+
+def circulant_spectrum(offsets, world: int) -> Tuple[float, float]:
+    """(a, b) = (min, max) of W's eigenvalues on 1^perp, in float64, for the circulant graph of `offsets` at `world`
+    ranks: lambda_j = (1 + 2 sum_o cos(2 pi j o / R)) / (2|O| + 1), j = 1 .. R - 1.  This is mixing_row()'s W, the
+    double count at o = R/2 (and so the ring at R = 2, quirk Q15) included."""
+    offs = parse_topology(tuple(offsets), world)
+    if world < 2:
+        raise ValueError("the spectrum on 1^perp needs at least 2 ranks")
+    n = 2 * len(offs)
+    lam = [(1.0 + 2.0 * sum(math.cos(2.0 * math.pi * j * o / world) for o in offs)) / (n + 1)
+           for j in range(1, world)]
+    return min(lam), max(lam)
+
+
+def chebyshev_coefficients(offsets, world: int, rounds: int, fp32: bool = True) -> List[Tuple[float, float]]:
+    """The (alpha_q, omega_q), q = 1 .. `rounds`, of Chebyshev-accelerated gossip on the circulant graph of `offsets`:
+    round q mixes w = W x_{q-1} and forms
+        x_q = x_{q-1} + alpha_q (w - x_{q-1}) + omega_q (x_{q-1} - x_{q-2})        (no omega term at q = 1)
+    so that x_Q = P_Q(W) x_0 with P_Q(W) = T_Q((W - c) / delta) / T_Q(mu), the degree-Q polynomial with P_Q(1) = 1 that
+    is smallest on W's spectrum [a, b] (circulant_spectrum): c = (a + b) / 2, delta = (b - a) / 2, mu = (1 - c) / delta,
+    rho_1 = 1 / mu, rho_q = 1 / (2 mu - rho_{q-1}); alpha_1 = rho_1 / delta, omega_1 = 0, alpha_q = 2 rho_q / delta,
+    omega_q = rho_q rho_{q-1}.  On 1^perp P_Q(W) contracts by 1 / T_Q(mu).  A one-point spectrum (delta <= 1e-12) gives
+    alpha_q = 1 / (1 - c) and omega_q = 0: one round is the exact average.  Everything is float64; `fp32` rounds each
+    coefficient once to fp32, the values every backend and the simulator use."""
+    if isinstance(rounds, bool) or int(rounds) != rounds or rounds < 1:
+        raise ValueError(f"rounds must be an integer >= 1, got {rounds!r}")
+    a, b = circulant_spectrum(offsets, world)
+    c, delta = (a + b) / 2.0, (b - a) / 2.0
+    out = []
+    if delta <= CHEB_POINT:
+        out = [(1.0 / (1.0 - c), 0.0)] * int(rounds)
+    else:
+        mu = (1.0 - c) / delta
+        rho = 1.0 / mu
+        out.append((rho / delta, 0.0))
+        for _ in range(2, int(rounds) + 1):
+            rho_prev, rho = rho, 1.0 / (2.0 * mu - rho)
+            out.append((2.0 * rho / delta, rho * rho_prev))
+    return [(_fp32(al), _fp32(om)) for al, om in out] if fp32 else out

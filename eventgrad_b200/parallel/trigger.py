@@ -19,6 +19,7 @@ Two trigger metrics (TriggerConfig.metric):
 from __future__ import annotations
 
 from dataclasses import dataclass
+from typing import Optional
 
 import torch
 
@@ -122,6 +123,20 @@ def mixk_(theta: torch.Tensor, slots) -> torch.Tensor:
     for s in slots:
         theta.add_(s)
     return theta.div_(len(slots) + 1)
+
+
+@torch.no_grad()
+def cheb_combine_(theta_mixed: torch.Tensor, x: torch.Tensor, x_prev: Optional[torch.Tensor], alpha: torch.Tensor,
+                  omega: torch.Tensor) -> torch.Tensor:
+    """One Chebyshev-accelerated gossip round (--gossip-accel chebyshev), given theta_mixed = w, the round's mix of x:
+        theta_mixed <- (x + alpha * (w - x)) + omega * (x - x_prev)
+    with alpha, omega 0-dim fp32 tensors (parallel/topology.py chebyshev_coefficients).  Separate rounded sub, mul and add
+    calls in the kernel's order (csrc/gossip_rounds.cu: __fsub_rn, __fmul_rn, __fadd_rn), so nothing fuses into an FMA.
+    x_prev None (round 1): the omega term is absent, not multiplied by zero."""
+    out = x.add(torch.mul(alpha, theta_mixed.sub(x)))
+    if x_prev is not None:
+        out.add_(torch.mul(omega, x.sub(x_prev)))
+    return theta_mixed.copy_(out)
 
 
 @torch.no_grad()

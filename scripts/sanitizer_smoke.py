@@ -27,7 +27,8 @@ def exchange(algo, **kw):
     t = w.arenas[0].table
     sim = RingSimulator(2, w.arenas[0].theta.cpu(), t, algo, TriggerConfig.from_train(cfg), lr=cfg.lr,
                         momentum=cfg.momentum, topk_percent=10.0, serial_skip=False, gossip_rounds=cfg.gossip_rounds,
-                        offsets=cfg.for_world(2).topology, topology_seed=cfg.topology_seed)
+                        offsets=cfg.for_world(2).topology, topology_seed=cfg.topology_seed,
+                        gossip_accel=cfg.gossip_accel)
     mask = torch.zeros(t.n_padded, device="cuda")
     for o, n in zip(t.offsets, t.numels):
         mask[o:o + n] = 1
@@ -55,6 +56,7 @@ def main():
     exchange("decent", overlap_push=True)
     exchange("decent", overlap_push=False, gossip_rounds=2)       # the mix-only round kernel ahead of the step
     exchange("decent", topology="random-match", topology_seed=3)  # the single-inbox random-match step
+    exchange("decent", overlap_push=False, gossip_rounds=2, gossip_accel="chebyshev")  # Chebyshev rounds, serial step
     # fused BN (+res)(+relu), both paths
     from eventgrad_b200.ops.bn_act import FusedBNAct, _workspace
     for fused in (0, 1):
